@@ -1,9 +1,10 @@
 #!/usr/bin/env python
 """Benchmark of the tokenizer hot path: frames/sec for full encode -> regularize -> decode on synthetic clips.
 
-  python bench.py --gpus N --steps K --warmup W                       # B200 arm, BASELINE.json configs[1] (the headline)
+  python bench.py --gpus N --steps K --warmup W                       # GPU arm, BASELINE.json configs[1] (the headline)
   python bench.py --config {kl488,fsq488,v11long,kl41616} [--precision {bf16,exact,mixed,fma}]
   python bench.py --impl reference [--config ...] --steps K ...        # reference arm: the reference's CPU path (oracle port)
+  python bench.py ... --dump-outputs DIR                               # also write the last timed step's outputs as DIR/*.npy
 
 A "step" is one pass of the hot path over one batch of clips per GPU (weak scaling; one process per GPU under torchrun for
 N > 1).  `value` is timed with CUDA events with the inputs already resident in HBM; `e2e` goes through the public Python API
@@ -90,9 +91,9 @@ def load_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return {"tflops": float(d.get("bf16_tflops_sustained", d.get("bf16_tflops", 1431.0))), "hbm_gbs": float(d.get("hbm_gbs", 6568.0)),
+        return {"tflops": float(d.get("bf16_tflops_sustained", d.get("bf16_tflops", 989.0))), "hbm_gbs": float(d.get("hbm_gbs", 3350.0)),
                 "source": "MEASURED_PEAKS.json (bf16_tflops_sustained: kernel timed inside a long step)"}
-    return {"tflops": 1400.0, "hbm_gbs": 6650.0, "source": "fallback (B200_PROFILING.md: ~1.4 PFLOP/s sustained)"}
+    return {"tflops": 989.0, "hbm_gbs": 3350.0, "source": "H100 SXM data sheet (dense BF16, HBM3; a card below 700 W reaches less)"}
 
 
 # --------------------------------------------------------------------------------------------------
@@ -205,6 +206,32 @@ def cpu_units_scale(c, T_s, S):
     return (T_s * S * S) / float(c["T"] * c["H"] * c["W"]) * c["T"]
 
 
+DUMP_MAX_BYTES = 64 << 20   # all dumped arrays together
+
+
+def dump_outputs(out_dir, z, dec, log):
+    """The arrays a caller of the timed path receives from its last step, as float32 .npy files, at most DUMP_MAX_BYTES in
+    all.  Outputs are written whole, in the order below, while they fit the remaining budget; one that does not is written
+    as `<name>_sample.npy` filling the rest: the elements at a fixed set of flat indices (torch.randperm with seed 0 over the flattened
+    output, first n, sorted), so the same arguments give the same sample and two builds can be compared output for output."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"kl_loss": log.get("kl_loss"), "indices": log.get("indices"), "z": z, "dec": dec}
+    budget = DUMP_MAX_BYTES - 4096   # .npy headers
+    for name, t in arrays.items():
+        if t is None:
+            continue
+        flat = t.detach().reshape(-1).float().cpu()
+        if 4 * flat.numel() <= budget:
+            np.save(os.path.join(out_dir, f"{name}.npy"), flat.reshape(tuple(t.shape)).numpy())
+        else:
+            n = budget // 4
+            idx = torch.randperm(flat.numel(), generator=torch.Generator().manual_seed(0))[:n].sort().values
+            flat = flat[idx]
+            np.save(os.path.join(out_dir, f"{name}_sample.npy"), flat.numpy())
+        budget -= 4 * flat.numel()
+
+
 def run_reference_arm(args, c):
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
@@ -240,7 +267,7 @@ def run_reference_arm(args, c):
 
 
 # --------------------------------------------------------------------------------------------------
-# B200 arm
+# GPU arm
 # --------------------------------------------------------------------------------------------------
 def run_b200_arm(args, c):
     import __graft_entry__ as ge
@@ -251,7 +278,7 @@ def run_b200_arm(args, c):
     from vidtok_b200.synth import synth_clip, synth_state_dict
 
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device (the B200 arm has no CPU fallback; use --impl reference for the CPU path)")
+        raise SystemExit("bench.py: no CUDA device (the GPU arm has no CPU fallback; use --impl reference for the CPU path)")
     rank, world, local = vdist.init_from_env("nccl")
     dev = torch.device("cuda", local)
     torch.cuda.set_device(dev)
@@ -332,7 +359,7 @@ def run_b200_arm(args, c):
     run_e2e = run_e2e_video if c["tiling"] else run_e2e_clips
 
     # the clock sampler starts BEFORE the warm-up: nvidia-smi takes ~1 s to initialise NVML, and doing that inside the
-    # timed region cost the first steps ~10 % (profiles/notes_r1.md); its samples cover warm-up + timed steps, all under load
+    # timed region costs the first steps; its samples cover warm-up + timed steps, all under load
     sampler = ClockSampler(local)
     sampler.start()
     for _ in range(max(args.warmup, 3)):
@@ -354,6 +381,8 @@ def run_b200_arm(args, c):
     clocks = sampler.stop()
     ms = torch.tensor([e0.elapsed_time(e1)], dtype=torch.float64, device=dev)
     ms = float(vdist.allreduce_max(ms)[0])
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, z, dec, log)
     frames = world * B * T * args.steps
     value = frames / (ms / 1e3)
 
@@ -376,17 +405,6 @@ def run_b200_arm(args, c):
 
     # ---- per-kernel attribution of one step (CUDA events around every launch, on the launch stream)
     peaks = load_peaks()
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "ncu_conv_tc_r2.json")
-    if not os.path.exists(tpath):
-        tpath = os.path.join(ROOT, "profiles", "ncu_conv_tc_r1.json")
-    if os.path.exists(tpath) and args.config == "kl488":  # dram__bytes_read+write per launch from the committed `ncu --set full` capture
-        try:
-            cap = json.load(open(tpath))
-            vals = [l["dram_read_bytes"] + l["dram_write_bytes"] for l in cap["launches"] if l.get("dram_read_bytes") is not None]
-            traffic = {"bytes_per_launch_avg": sum(vals) / len(vals), "launches_captured": len(vals), "source": os.path.relpath(tpath, ROOT)}
-        except Exception:
-            traffic = None
     roof = None
     if rank == 0:
         # PROF_STEPS steps back to back under the profiler, long enough to be at the sustained (power-capped) clock and for
@@ -421,7 +439,7 @@ def run_b200_arm(args, c):
             bound = "tensor" if d["flops"] > 0 and dom.startswith("conv") else "hbm"
             peak = peaks["tflops"] if bound == "tensor" else peaks["hbm_gbs"]
             roof = {"kernel": dom, "bound": bound, "achieved": ach, "peak": peak, "unit": "TFLOP/s" if bound == "tensor" else "GB/s",
-                    "frac": ach / peak, "traffic": traffic, "launches_per_step": d["launches"],
+                    "frac": ach / peak, "launches_per_step": d["launches"],
                     "avg_launch_ms": d["ms"] / max(d["launches"], 1), "share_of_step": d["ms"] / tot_ms,
                     "algorithmic_flops_per_step": d["flops"], "peak_source": peaks["source"],
                     "note": ("achieved = algorithmic FLOPs of the kernel's launches / their summed durations; conv_tc3 (split operands) executes "
@@ -475,7 +493,7 @@ def run_b200_arm(args, c):
             "config": {"workload": workload_string(c, precision, B), "bench_config": args.config, "precision": precision,
                        "clips_per_gpu": B, "parallelism": f"dp{world} (clips sharded, no data-path collective)",
                        "weights": "random (synth_state_dict seed 0)", "algorithmic_flops_per_clip": c["flops"],
-                       "l2": "per-step activations are GBs, far larger than the 126 MB L2"},
+                       "l2": "per-step activations are GBs, far larger than the 50 MB L2"},
             "clocks": clocks,
             "e2e": {"value": e2e_value, "unit": "frames/s", "ms_per_step": ms_e2e / args.steps,
                     "h2d_bytes_per_step": nbytes + noise_bytes, "d2h_bytes_per_step": nbytes,
@@ -505,6 +523,8 @@ def main():
     ap.add_argument("--precision", default=None, choices=["bf16", "exact", "mixed", "fma"], help="default: the config's")
     ap.add_argument("--batch", type=int, default=0, help="clips per GPU (default: the config's)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned (latents, reconstruction sample, KL loss) as DIR/<name>.npy")
     args = ap.parse_args()
     c = CONFIGS[args.config]
     if args.impl == "reference":

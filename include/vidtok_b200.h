@@ -1,5 +1,5 @@
 /*
- * vidtok_b200 -- C ABI of the B200-native VidTok causal tokenizer hot path
+ * vidtok_b200 -- C ABI of the H100-native (sm_90a) VidTok causal tokenizer hot path
  * (encode -> KL/FSQ regularize -> decode).
  *
  * The reference (microsoft/VidTok @ d6ad92d) has no FFI / plugin registry: the only indirection on this
@@ -35,13 +35,13 @@ typedef enum {
   VT_ERR_CUDA = -2,       /* CUDA runtime or driver error */
   VT_ERR_NOT_READY = -3,  /* parameters missing or vt_model_finalize not called */
   VT_ERR_WORKSPACE = -4,  /* workspace too small */
-  VT_ERR_NO_DEVICE = -5   /* no sm_100 device: there is deliberately no CPU fallback */
+  VT_ERR_NO_DEVICE = -5   /* no sm_90a (H100) device: there is deliberately no CPU fallback */
 } vt_status;
 
 /* Precision modes.
- * EXACT_TC (the parity mode): fp32-class results on the tcgen05 tensor cores.  Activations and weights are kept as
+ * EXACT_TC (the parity mode): fp32-class results on the tensor cores (wgmma).  Activations and weights are kept as
  *   two fp16 planes (hi = fp16(v), lo = fp16(v - hi): 11 + 11 mantissa bits); every K step issues hi*hi + lo*hi + hi*lo
- *   into the fp32 TMEM accumulator ("fp16x3": products good to ~2^-21), LayerNorm / SiLU / regularizers in fp32.
+ *   into the fp32 register accumulator ("fp16x3": products good to ~2^-21), LayerNorm / SiLU / regularizers in fp32.
  *   Gate: 1e-3 max-abs, FSQ codes equal.
  * BF16 (the throughput mode): bf16 activations / weights, fp32 accumulation.  Gate: PSNR within 0.01 dB.
  * MIXED: encoder in EXACT_TC (bit-exact FSQ codes / 1e-3 latents), decoder in BF16.
@@ -119,7 +119,7 @@ int32_t vt_model_param_info(const vt_model* m, int32_t index, char* name, int32_
  * (replaces load_state_dict, autoencoder.py:164). */
 int32_t vt_model_load_param(vt_model* m, const char* name, const float* data, int64_t numel, int32_t is_device,
                             void* stream);
-/* Repacks all parameters for the kernels (K-major bf16 tiles for tcgen05, [K][Cout] fp32 for the FMA
+/* Repacks all parameters for the kernels (K-major bf16 tiles for wgmma, [K][Cout] fp32 for the FMA
  * path).  Must be called after the last vt_model_load_param and before encode/decode. */
 int32_t vt_model_finalize(vt_model* m, void* stream);
 
@@ -208,7 +208,7 @@ typedef struct vt_conv_desc {
 } vt_conv_desc;
 /* x/res/out are channels-last activations in the precision's activation type: fp32 (FMA32), bf16 (BF16), or hi|lo split
  * bf16 rows [..., hi(C) | lo(C)] (EXACT_TC; value = hi + lo); w fp32 [Co,Ci,kt,kh,kw]; bias fp32 [Co].
- * BF16 / EXACT_TC run the tcgen05 kernel (an unsupported geometry is an error, never a silent fallback) unless
+ * BF16 / EXACT_TC run the wgmma kernel (an unsupported geometry is an error, never a silent fallback) unless
  * force_simt != 0, which runs the fp32-FMA kernel on the same operands. */
 int32_t vt_op_conv(int32_t precision, int32_t force_simt, const vt_conv_desc* d, const void* x, const float* w,
                    const float* bias, const void* res, void* out, void* stream);
@@ -262,7 +262,7 @@ int32_t vt_op_groupnorm(int32_t precision, const void* x, const float* gamma, co
                         int64_t frames, int64_t positions_per_frame, int32_t C, int32_t per_position,
                         int32_t apply_silu, void* workspace, int64_t workspace_bytes, void* stream);
 /* per-frame single-head attention core: q,k,v,o channels-last [frames, tokens, C]; scale = C^-0.5.  Runs what the
- * model path runs: tcgen05 GEMMs in BF16 / EXACT_TC when tokens % 64 == 0 and C % 64 == 0, fp32 FMAs otherwise.
+ * model path runs: wgmma GEMMs in BF16 / EXACT_TC when tokens % 64 == 0 and C % 64 == 0, fp32 FMAs otherwise.
  * workspace: frames*tokens*(8*tokens + 24*C) + 65536 bytes is always enough. */
 int32_t vt_op_attention(int32_t precision, const void* q, const void* k, const void* v, void* o, int32_t frames,
                         int32_t tokens, int32_t C, void* workspace, int64_t workspace_bytes, void* stream);

@@ -6,7 +6,7 @@ causal / non-causal, KL / FSQ, 4x4x4 ... 8x8x8 ... 4x16x16 compression) and reco
   * the latent and reconstruction shapes the reference produces for a 1x3x17x64x64 clip,
   * the largest |reference - oracle| over latents and reconstruction on seeded weights (asserted <= 2e-5; FSQ indices equal),
 
-into tests/golden/zoo_manifest.json.gz.  tests/test_zoo_cpu.py checks the B200 engine's module tree, latent geometry and
+into tests/golden/zoo_manifest.json.gz.  tests/test_zoo_cpu.py checks the engine's module tree, latent geometry and
 workspace planning against it on any machine (the GPU box has no /root/reference), and regenerates the key tables when the
 reference is present.
 

@@ -15,7 +15,7 @@ GOLDEN_DIR = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA (sm_100a) device; run on the B200 box with -m gpu")
+    config.addinivalue_line("markers", "gpu: needs a CUDA (sm_90a, H100) device; run on an H100 machine with -m gpu")
     # make sure the CUDA library exists before anything imports it (nvcc cross-compiles without a GPU)
     import __graft_entry__ as ge
     ge.build()

@@ -1,125 +1,32 @@
-"""Script-level drop-in (SURVEY.md section 8f-1): with this repo AND a reference checkout on PYTHONPATH, the reference's own
-scripts import unchanged -- hot-path modules resolve to the B200 shims, everything else (vidtok.data.*, vidtok.modules.lpips)
-to the reference -- and `load_model_from_config` (scripts/inference_evaluate.py:26-32) builds the B200 engine.
-
-Needs the reference checkout (VIDTOK_REFERENCE_ROOT or /root/reference): skipped on the GPU box.  Runs in subprocesses so
-the import state of the test process is untouched.  Also: the oracle pin is reproducible (oracle/make_golden.py), the
-oracle's parameter table equals the reference's state_dict, and compute_ssim equals the reference formula."""
+"""Drop-in surface without the reference checkout: a v1.1 configuration from the committed zoo manifest
+(tests/golden/zoo_manifest.json.gz, the `model:` section of the reference YAML) resolves to the tiling engine and takes the
+tiling attributes exactly as scripts/inference_evaluate.py:144-150 sets them; the oracle's parameter table equals the
+reference's state_dict (pinned in the golden fixtures), and compute_ssim equals the reference formula."""
+import gzip
 import json
 import os
-import subprocess
-import sys
-import textwrap
 
-import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
-from conftest import GOLDEN_DIR, ROOT, golden_cases, load_golden
+from conftest import ROOT, golden_cases, load_golden
 
-REF = os.environ.get("VIDTOK_REFERENCE_ROOT", "/root/reference")
-needs_ref = pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "vidtok", "modules")), reason="reference checkout not present")
-
-# Modules the scripts import that are absent offline (SURVEY.md section 0.5).  Stubs only: no behaviour is borrowed.
-STUBS = textwrap.dedent('''
-    import sys, types, copy, yaml
-    def _mod(name, **attrs):
-        m = types.ModuleType(name); m.__dict__.update(attrs); sys.modules[name] = m; return m
-    class _Cfg(dict):
-        """attribute access + item access, like an OmegaConf DictConfig"""
-        def __getattr__(self, k):
-            try: return self[k]
-            except KeyError: raise AttributeError(k)
-        def __setattr__(self, k, v): self[k] = v
-    def _wrap(o):
-        if isinstance(o, dict): return _Cfg({k: _wrap(v) for k, v in o.items()})
-        if isinstance(o, list): return [_wrap(v) for v in o]
-        return o
-    def _load(path):
-        cfg = yaml.safe_load(open(path))
-        dp = cfg["model"]["params"]["decoder_config"]
-        if isinstance(dp.get("params"), str):   # ${model.params.encoder_config.params}
-            dp["params"] = copy.deepcopy(cfg["model"]["params"]["encoder_config"]["params"])
-        return _wrap(cfg)
-    _mod("omegaconf", OmegaConf=types.SimpleNamespace(load=_load), ListConfig=list)
-    _mod("decord", bridge=types.SimpleNamespace(set_bridge=lambda *_: None), VideoReader=object, cpu=lambda *_: None)
-    lt = _mod("lightning"); pl = _mod("lightning.pytorch", seed_everything=lambda *a, **k: None)
-    lt.pytorch = pl
-    ut = _mod("lightning.pytorch.utilities"); rz = _mod("lightning.pytorch.utilities.rank_zero", rank_zero_only=lambda f: f)
-    ut.rank_zero = rz; ut.rank_zero_only = rz.rank_zero_only; pl.utilities = ut
-    import torchvision.io as _tvio
-    if not hasattr(_tvio, "write_video"):   # removed from recent torchvision; the script only calls it when saving mp4s
-        _tvio.write_video = lambda *a, **k: None
-''')
+ZOO = json.load(gzip.open(os.path.join(ROOT, "tests", "golden", "zoo_manifest.json.gz"), "rt"))
 
 
-def run_py(code, extra_env=None):
-    env = dict(os.environ)
-    env["PYTHONPATH"] = os.pathsep.join([ROOT, REF])   # INTEGRATION.md: this repo first, then the reference checkout
-    env.update(extra_env or {})
-    r = subprocess.run([sys.executable, "-c", STUBS + textwrap.dedent(code)], capture_output=True, text=True, env=env, cwd="/tmp",
-                       timeout=600)
-    assert r.returncode == 0, r.stdout + "\n" + r.stderr
-    return r.stdout
-
-
-@needs_ref
-def test_reference_scripts_import_unchanged_and_build_the_b200_engine():
-    cfg = os.path.join(REF, "configs", "vidtok_kl_causal_488_4chn.yaml")
-    out = run_py(f'''
-        import inspect, json
-        import scripts.inference_evaluate as ev          # the reference's script, unmodified
-        import scripts.inference_reconstruct as rc
-        import vidtok, vidtok.data.vidtok, vidtok.modules.lpips, vidtok.modules.util, vidtok.models.autoencoder
-        model = ev.load_model_from_config({cfg!r}, None)
-        print(json.dumps({{
-            "script": inspect.getfile(ev), "dataset": inspect.getfile(vidtok.data.vidtok), "lpips": inspect.getfile(vidtok.modules.lpips),
-            "engine": inspect.getfile(type(model)), "engine_cls": type(model).__name__, "is_causal": model.is_causal,
-            "tdf": model.encoder.time_downsample_factor, "has_tiling": hasattr(model, "use_tiling"),
-            "ssim": ev.compute_ssim is vidtok.modules.util.compute_ssim, "nparams": len(model.state_dict()),
-            "dataset_cls": ev.MultiVideoDataset.__mro__[1].__module__,
-        }}))
-    ''')
-    info = json.loads(out.strip().splitlines()[-1])
-    assert info["script"].startswith(REF) and info["dataset"].startswith(REF) and info["lpips"].startswith(REF)
-    assert info["engine"].startswith(ROOT) and info["engine_cls"] == "AutoencodingEngine"
-    assert info["is_causal"] is True and info["tdf"] == 4 and info["has_tiling"] is False and info["ssim"] is True
-    assert info["nparams"] == 416 and info["dataset_cls"] == "vidtok.data.vidtok"
-
-
-@needs_ref
 def test_v11_config_resolves_to_the_tiling_engine():
-    cfg = os.path.join(REF, "configs", "vidtok_v1_1", "vidtok_kl_causal_488_16chn_v1_1.yaml")
-    out = run_py(f'''
-        import json
-        import scripts.inference_evaluate as ev
-        model = ev.load_model_from_config({cfg!r}, None)
-        # scripts/inference_evaluate.py:144-150
-        assert hasattr(model, "use_tiling")
-        model.use_tiling = True; model.t_chunk_enc = 16
-        model.t_chunk_dec = model.t_chunk_enc // model.encoder.time_downsample_factor; model.use_overlap = True
-        print(json.dumps({{"cls": type(model).__name__, "z": model.spec.z_channels, "interp": model.spec.interpolation_mode,
-                           "chunks": model.build_chunk_start_end(129)[:3]}}))
-    ''')
-    info = json.loads(out.strip().splitlines()[-1])
+    from vidtok_b200.compat_util import instantiate_from_config
+    model = instantiate_from_config(ZOO["vidtok_v1_1/vidtok_kl_causal_488_16chn_v1_1.yaml"]["model"])
+    # scripts/inference_evaluate.py:144-150
+    assert hasattr(model, "use_tiling")
+    model.use_tiling = True
+    model.t_chunk_enc = 16
+    model.t_chunk_dec = model.t_chunk_enc // model.encoder.time_downsample_factor
+    model.use_overlap = True
+    info = {"cls": type(model).__name__, "z": model.spec.z_channels, "interp": model.spec.interpolation_mode,
+            "chunks": [list(c) for c in model.build_chunk_start_end(129)[:3]]}
     assert info == {"cls": "AutoencodingEngineV11", "z": 16, "interp": "trilinear", "chunks": [[0, 1], [1, 17], [17, 33]]}
-
-
-@needs_ref
-def test_golden_fixture_regenerates_bit_identically(tmp_path):
-    """python oracle/make_golden.py runs as committed (the shim package no longer shadows the reference) and reproduces
-    the committed fixture bit for bit."""
-    env = dict(os.environ)
-    env["VIDTOK_GOLDEN_OUT"] = str(tmp_path)
-    r = subprocess.run([sys.executable, os.path.join(ROOT, "oracle", "make_golden.py"), "tiny_kl_v10"], capture_output=True, text=True,
-                       env=env, cwd=ROOT, timeout=900)
-    assert r.returncode == 0, r.stdout + r.stderr
-    a, b = np.load(tmp_path / "tiny_kl_v10.npz"), np.load(os.path.join(GOLDEN_DIR, "tiny_kl_v10.npz"))
-    assert set(a.files) == set(b.files)
-    for k in a.files:
-        if k != "meta_json":
-            assert np.array_equal(a[k], b[k]), k
 
 
 @pytest.mark.parametrize("case", golden_cases())

@@ -3,7 +3,7 @@
 The oracle is only affordable on one clip, so the full-size checks combine (i) one-clip comparisons against the oracle
 run on the box's host cores and (ii) size-independent properties at the BASELINE batch sizes: batch independence,
 determinism, exact-vs-bf16 agreement, decode(indices) == decode(codes), tiled-encode == untiled-encode.
-"exact" is the split-operand (fp16 hi|lo x 3 MMAs) tensor-core mode (VT_PREC_EXACT_TC): the 1e-3 / bit-exact gates below run on tcgen05."""
+"exact" is the split-operand (fp16 hi|lo x 3 MMAs) tensor-core mode (VT_PREC_EXACT_TC): the 1e-3 / bit-exact gates below run on wgmma."""
 import os
 
 import pytest
@@ -71,7 +71,7 @@ def test_config2_kl_488_one_clip_vs_oracle_and_batch8_properties():
         torch.manual_seed(4321)
         (z_e, dec_e, _), ln = launches_of(lambda: model(x1.cuda()))
         dz, dd = float((z_e.cpu() - z_o).abs().max()), float((dec_e.cpu() - dec_o).abs().max())
-        print(f"[config2] exact (fp16x3 tcgen05) vs oracle: max|dz|={dz:.2e} max|ddec|={dd:.2e}; launches {ln}")
+        print(f"[config2] exact (fp16x3 wgmma) vs oracle: max|dz|={dz:.2e} max|ddec|={dd:.2e}; launches {ln}")
         assert dz <= 1e-3 and dd <= 1e-3
         assert ln.get("conv_tc3", 0) >= 100 and ln.get("conv_simt", 0) <= 1 and "conv_tc" not in ln, ln
         model.precision = "bf16"
@@ -99,7 +99,7 @@ def test_config2_kl_488_one_clip_vs_oracle_and_batch8_properties():
 
 
 def test_config3_fsq_488_codes_equal_at_full_size():
-    """configs[2]: vidtok_fsq_causal_488_32768, 17x256x256: indices of the exact mode (fp16x3 on tcgen05, asserted through
+    """configs[2]: vidtok_fsq_causal_488_32768, 17x256x256: indices of the exact mode (fp16x3 on wgmma, asserted through
     the launch profile) equal the oracle's on two clips (raw mismatches reported; none allowed outside the 1e-4 tie guard
     band); the mixed mode (exact encoder, bf16 decoder) reproduces those indices bit for bit on the 8-clip batch;
     decode(indices) == decode(codes)."""
@@ -117,7 +117,7 @@ def test_config3_fsq_488_codes_equal_at_full_size():
         bad = idx != log_o["indices"]
         pre = log_o["pre_round"]
         near = ((pre - pre.floor() - 0.5).abs() < 1e-4).any(dim=-1)
-        print(f"[config3] exact (tcgen05) FSQ raw mismatches {int(bad.sum())}/{bad.numel()} (outside tie band: {int((bad & ~near).sum())})")
+        print(f"[config3] exact (wgmma) FSQ raw mismatches {int(bad.sum())}/{bad.numel()} (outside tie band: {int((bad & ~near).sum())})")
         assert not (bad & ~near).any()
         assert int(bad.sum()) <= 2
         assert idx.dtype == torch.int32 and tuple(idx.shape) == (2, 5, 32, 32)

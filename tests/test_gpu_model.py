@@ -2,7 +2,7 @@
 (vidtok.models.autoencoder[_v1_1].AutoencodingEngine resolved from the YAML target strings) against the golden
 fixtures produced by the unmodified reference, and against the oracle.
 
-Gates (BASELINE.json north_star): "exact" mode -- fp16 hi|lo split operands (3 MMAs per K step) on the tcgen05 tensor cores -- max-abs <= 1e-3 on
+Gates (BASELINE.json north_star): "exact" mode -- fp16 hi|lo split operands (3 MMAs per K step) on the wgmma tensor cores -- max-abs <= 1e-3 on
 latents and reconstructions, FSQ indices equal (0 mismatches outside a 1e-4 guard band around rounding ties, raw count
 reported); the same gates for the fp32-FMA cross-check mode ("fma"); BF16 mode PSNR within 0.01 dB."""
 import numpy as np
@@ -75,7 +75,7 @@ def test_exact_mode_matches_reference_fixture(case, mode):
     ch = meta["model"]["params"]["encoder_config"]["params"]["ch"]
     if mode == "exact" and ch % 64 == 0 and meta["model"]["params"]["encoder_config"]["params"].get("norm_type") == "layernorm":
         # the parity gate runs on the tensor cores: every convolution but the z -> 512 decoder conv_in (Cin = z_channels)
-        # is a tcgen05 launch, per chunk when tiled
+        # is a wgmma launch, per chunk when tiled
         n_chunks = 1
         if meta["tiling_chunk"]:
             n_chunks = 2 * (2 + (meta["input"][2] - 1) // meta["tiling_chunk"])
@@ -276,7 +276,7 @@ def test_video_calls_with_host_staging_equal_device_path(case):
 @pytest.mark.gpu
 def test_two_models_on_two_devices_in_one_process():
     """Kernel attributes (227 KB dynamic shared memory) and the SM count are per device: a second model on another GPU of the
-    same process must launch every tcgen05 kernel there (ADVICE r1: a process-wide `static bool` guarded the opt-in)."""
+    same process must launch every wgmma kernel there (ADVICE r1: a process-wide `static bool` guarded the opt-in)."""
     if torch.cuda.device_count() < 2:
         pytest.skip("needs two visible GPUs")
     d, meta = load_golden("tiny_kl_v10")

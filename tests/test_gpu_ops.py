@@ -224,7 +224,7 @@ def test_kl_reparameterise():
 
 
 # ---------------------------------------------------------------------------------------------------------------
-# tcgen05 / TMA implicit-GEMM kernel (BF16 mode) against fp32 torch on the same bf16-rounded operands
+# wgmma / TMA implicit-GEMM kernel (BF16 mode) against fp32 torch on the same bf16-rounded operands
 # ---------------------------------------------------------------------------------------------------------------
 TC_CASES = [
     # name, Ci, Co, k, stride, (B,T,H,W), res_mode
@@ -274,7 +274,7 @@ def test_conv_tc(case):
 
 
 def test_conv_tc_downsample_stride2():
-    """Downsample (pad (0,1,0,1), 3x3 stride 2) on the tcgen05 path: parity-view tensor maps."""
+    """Downsample (pad (0,1,0,1), 3x3 stride 2) on the wgmma path: parity-view tensor maps."""
     from gpu_util import op_conv
     for (B, T, H, W, Ci, Co) in [(1, 2, 32, 32, 64, 64), (2, 3, 64, 32, 128, 128)]:
         x = rnd(B, Ci, T, H, W, seed=1).bfloat16().float()

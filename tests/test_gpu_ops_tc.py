@@ -324,7 +324,7 @@ def test_time_upsample_conv_two_phases(precision, fuse_ln):
 
 
 # ---------------------------------------------------------------------------------------------------------------
-# attention core on tcgen05 (per-frame K / V^T as the B operand), LayerNorm / GroupNorm on split rows
+# attention core on wgmma (per-frame K / V^T as the B operand), LayerNorm / GroupNorm on split rows
 # ---------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("precision", PRECS, ids=PIDS)
 def test_attention_core_tcgen05(precision):

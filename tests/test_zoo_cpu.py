@@ -1,5 +1,5 @@
 """Every tokenizer configuration the reference ships (23 YAMLs: causal / non-causal, KL / FSQ, 4x4x4 ... 8x8x8 ... 4x16x16, v1.0 / v1.1)
-against the B200 engine's host side, from the committed manifest tests/golden/zoo_manifest.json.gz (written by
+against the engine's host side, from the committed manifest tests/golden/zoo_manifest.json.gz (written by
 oracle/make_zoo_manifest.py from the UNMODIFIED reference; the same run asserts oracle == reference to 2e-5 on each of them)."""
 import gzip
 import json
@@ -48,20 +48,3 @@ def test_engine_module_tree_geometry_and_workspace_plan(name):
     for prec in (N.PREC_BF16, N.PREC_EXACT_TC, N.PREC_MIXED, N.PREC_FMA32):
         ws = N.lib().vt_workspace_bytes(nm.handle, prec, B, T, H, W)
         assert ws > 0, (name, prec, N.lib().vt_last_error())
-
-
-def test_manifest_key_tables_regenerate_from_the_reference(tmp_path):
-    """Container only: the key tables in the manifest are what the unmodified reference builds today."""
-    from oracle import ref_shim
-    if not ref_shim.reference_available():
-        pytest.skip("reference checkout not present")
-    import subprocess
-    code = ("import sys; sys.path.insert(0, %r); import oracle.make_zoo_manifest as m; m.OUT = %r; m.main(numerics=False)"
-            % (ROOT, str(tmp_path / "zoo.json.gz")))
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stderr[-2000:]
-    new = json.load(gzip.open(tmp_path / "zoo.json.gz", "rt"))
-    assert set(new) == set(ZOO)
-    for name in ZOO:
-        assert new[name]["shapes"] == ZOO[name]["shapes"], name
-        assert new[name]["model"] == ZOO[name]["model"], name

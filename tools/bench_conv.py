@@ -1,4 +1,4 @@
-"""Time one conv geometry on the tcgen05 path (CUDA events, 20 launches).  VT_TC_PAIR=0/1/2 selects the CTA-pair mode.
+"""Time one conv geometry on the wgmma path (CUDA events, 20 launches).
 usage: python tools/bench_conv.py Ci Co kt kh kw B T H W [res]"""
 import ctypes as C
 import os
@@ -44,4 +44,4 @@ import json
 prof = json.loads(buf.value.decode())
 for k, v in prof.items():
     if k.startswith("conv_tc"):
-        print(f"PAIR={os.environ.get('VT_TC_PAIR', '1')} {v['ms'] / v['launches']:.4f} ms  {v['flops'] / v['ms'] / 1e9:.1f} TF/s  {k}")
+        print(f"{v['ms'] / v['launches']:.4f} ms  {v['flops'] / v['ms'] / 1e9:.1f} TF/s  {k}")

@@ -7,7 +7,7 @@ Everything else of the reference's `vidtok` package (vidtok.data.*, vidtok.modul
 reference ships `vidtok/` as a namespace package (no __init__.py), so when a reference checkout is importable
 (VIDTOK_REFERENCE_ROOT, or any sys.path entry that holds the reference's vidtok/data/), its directories are appended to
 this package's __path__ -- `from vidtok.data.vidtok import VidTokValDataset` (scripts/inference_evaluate.py:20) then
-resolves to the reference's file while `vidtok.models.autoencoder` resolves to the B200 path."""
+resolves to the reference's file while `vidtok.models.autoencoder` resolves to the CUDA path."""
 import os as _os
 import sys as _sys
 

@@ -6,7 +6,7 @@ import ctypes as C
 import os
 
 VT_MAX_LEVELS = 8
-# include/vidtok_b200.h: FMA32 (fp32 FMA kernels), BF16 (tcgen05), EXACT_TC (fp16 hi|lo split operands, 3 MMAs per K step, on tcgen05), MIXED
+# include/vidtok_b200.h: FMA32 (fp32 FMA kernels), BF16 (wgmma), EXACT_TC (fp16 hi|lo split operands, 3 MMAs per K step, on wgmma), MIXED
 PREC_FMA32, PREC_BF16, PREC_EXACT_TC, PREC_MIXED = 0, 1, 2, 3
 PREC_EXACT = PREC_EXACT_TC  # the parity mode
 _HERE = os.path.dirname(os.path.abspath(__file__))

@@ -1,5 +1,5 @@
-"""In-tree build of libvidtok_b200.so (nvcc, sm_100a only).  No JIT cache: the .so sits next to this file so it
-travels to the GPU box with the repo snapshot."""
+"""In-tree build of libvidtok_b200.so (nvcc, sm_90a only: the kernels use wgmma, TMA and setmaxnreg).  No JIT cache: the
+.so sits next to this file, so the package imports from the repository tree."""
 from __future__ import annotations
 
 import os
@@ -13,7 +13,7 @@ OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libvidtok_b200.so")
 SOURCES = ["conv_simt.cu", "conv_tc.cu", "conv_stem.cu", "tblock_tc.cu", "elementwise.cu", "model.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
 ]
 
@@ -52,7 +52,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
 
     with ThreadPoolExecutor(max_workers=len(srcs)) as ex:
         objs = list(ex.map(compile_one, srcs))
-    cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB] + objs
+    cmd = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB] + objs
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

@@ -1,4 +1,4 @@
-// FP32-FMA implicit-GEMM convolution (the EXACT-mode kernel, and the fallback for shapes the tcgen05 kernel
+// FP32-FMA implicit-GEMM convolution (the EXACT-mode kernel, and the fallback for shapes the wgmma kernel
 // does not take: Cin=3 stem, Cout<=8 heads).  One kernel covers every convolution geometry of the path via
 // ConvP (common.cuh).  GEMM view: M = B*To*Ho*Wo output positions, N = Cout, K = kt*kh*kw*Cin ordered
 // tap-major / channel-minor; weights are pre-packed as [K][Cout] fp32.

@@ -1,15 +1,17 @@
 // Stem convolution of the encoder (conv_in: CausalConv3d(in_channels=3 -> ch, k=3), model_3dcausal.py:535,634) on
-// tcgen05: the input is the caller's fp32 [B,3,T,H,W] tensor, far too thin (K = 27*3 = 81) for the TMA-box
+// wgmma: the input is the caller's fp32 [B,3,T,H,W] tensor, far too thin (K = 27*3 = 81) for the TMA-box
 // formulation of conv_tc.cu, so the A tile is built by the CTA's threads: a halo patch of the 3 input frames is
 // staged in shared memory (coalesced fp32 loads, replicate front padding and causal zero padding resolved while
 // loading), every thread then writes im2col rows (81 values, bf16) straight into the canonical K-major
 // SWIZZLE_128B layout (16-byte unit u of row r lives at unit u ^ (r & 7)), fences the generic->async proxy, and one
-// thread issues 8 tcgen05.mma (M=128, N=Cout, K=128 with zero padding).  The epilogue adds the bias and writes the
-// bf16 channels-last activation.  The patch loads of tile i+1 are in flight (registers) during the epilogue of tile i.
+// each of the two warpgroups issues 8 wgmma (M=64 rows of the tile, N=Cout, K=128 with zero padding) into register
+// accumulators.  The epilogue adds the bias and writes the bf16 channels-last activation.  The patch loads of tile i+1 are
+// in flight (registers) during the MMAs and the epilogue of tile i.
 #include <cstdio>
 
 #include "common.cuh"
 #include "kernels.h"
+#include "tc_ptx.cuh"
 
 namespace vt {
 namespace {
@@ -26,7 +28,6 @@ struct StemParams {
   bf16* out;       // [B,To,H,W,Co]
   long long num_tiles;
   int tilesW, tilesH;
-  uint32_t tmem_cols;
   float acc_scale;   // split: 2^-s of the pre-scaled weights (1 otherwise)
 };
 
@@ -36,78 +37,36 @@ constexpr int kATile = 2 * 128 * 128;  // two 64-wide K chunks of 128 rows x 128
 constexpr int kPatchIt = 9;            // patch values per thread: Ci * 3 * PH * PW <= 4 * 540 = 2160 <= 9 * 256
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
-  return ok != 0;
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  if (mbar_try_wait(bar, parity)) return;
-  const long long t0 = clock64();
-  while (!mbar_try_wait(bar, parity))
-    if (clock64() - t0 > 8000000000LL) __trap();
-}
-__device__ __forceinline__ uint64_t make_sdesc(uint32_t addr) {
-  return (uint64_t)((addr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)64 << 32) | ((uint64_t)1 << 46) |
-         ((uint64_t)2 << 61);
-}
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr) : "memory");
-}
-
 // kSplit (EXACT_TC mode): the im2col rows and the weights are hi|lo fp16 pairs, every K=16 step issues hi*hi + lo*hi +
 // hi*lo into the same accumulator, and the output is written as hi | lo planes ([..., 2*Co]).
-// The bf16 variant (110 KB of shared memory, 2*Co = 256 TMEM columns for Co = 128) is sized so that TWO CTAs share an SM:
-// the phases of a tile (patch loads -> im2col -> MMA -> epilogue) are serialised inside a CTA by block barriers, and a
-// second resident CTA fills the bubbles.
-template <bool kSplit>
-__global__ void __launch_bounds__(256, kSplit ? 1 : 2) conv_stem_kernel(const StemParams p, const bf16* __restrict__ wpk /*[Co][128] or [Co][hi 128 | lo 128]*/) {
+template <int CO, bool kSplit>
+__global__ void __launch_bounds__(256, 1) conv_stem_kernel(const StemParams p, const bf16* __restrict__ wpk /*[Co][128] or [Co][hi 128 | lo 128]*/) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* gen = smem_raw + (base - smem_u32(smem_raw));
   constexpr uint32_t kPl = kSplit ? 2u : 1u;
-  // layout: A[2 buffers][planes] (32 KB each) | B[planes] (Co x 256 B each) | patch (Ci*3*PH*PW floats) | bias | barriers | tmem slot
-  const uint32_t offA = 0, offB = 2 * kPl * kATile;
-  const uint32_t offP = offB + kPl * (uint32_t)p.Co * 256u;
+  // layout: A[planes] (32 KB each) | B[planes] (Co x 256 B each) | patch (Ci*3*PH*PW floats) | bias | im2col lut
+  const uint32_t offA = 0, offB = kPl * kATile;
+  const uint32_t offP = offB + kPl * (uint32_t)CO * 256u;
   const uint32_t patch_floats = (uint32_t)p.Ci * 3 * PH * PW;
   const uint32_t offBias = offP + ((patch_floats * 4 + 15) & ~15u);
   const uint32_t offLut = offBias + 256 * 4;   // im2col k -> patch offset (or -1)
-  const uint32_t offBar = offLut + 128 * 4;
   float* patch = reinterpret_cast<float*>(gen + offP);
   float* sbias = reinterpret_cast<float*>(gen + offBias);
   int* lut = reinterpret_cast<int*>(gen + offLut);
-  const uint32_t bar0 = base + offBar, bar1 = bar0 + 8, tmem_slot = bar0 + 16;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int K = p.Ci * 27;
   const int units = (K + 7) / 8;  // 16-byte units of real data per im2col row (11 for Ci = 3)
 
-  // ---- one-time setup: zero both A buffers, stage weights (swizzled) and bias, barriers, TMEM
-  for (uint32_t i = tid; i < 2 * kPl * kATile / 16; i += 256) reinterpret_cast<uint4*>(gen + offA)[i] = make_uint4(0, 0, 0, 0);
-  for (int i = tid; i < p.Co * 16 * (int)kPl; i += 256) {
-    const int pl = i / (p.Co * 16), r = i % (p.Co * 16);
+  // ---- one-time setup: zero the A tile, stage weights (swizzled) and bias
+  for (uint32_t i = tid; i < kPl * kATile / 16; i += 256) reinterpret_cast<uint4*>(gen + offA)[i] = make_uint4(0, 0, 0, 0);
+  for (int i = tid; i < CO * 16 * (int)kPl; i += 256) {
+    const int pl = i / (CO * 16), r = i % (CO * 16);
     const int row = r >> 4, U = r & 15, kc = U >> 3, u = U & 7;
     const uint4 v = *reinterpret_cast<const uint4*>(wpk + (long long)row * 128 * kPl + pl * 128 + U * 8);
-    *reinterpret_cast<uint4*>(gen + offB + pl * (p.Co * 256) + kc * (p.Co * 128) + row * 128 + ((u ^ (row & 7)) << 4)) = v;
+    *reinterpret_cast<uint4*>(gen + offB + pl * (CO * 256) + kc * (CO * 128) + row * 128 + ((u ^ (row & 7)) << 4)) = v;
   }
-  for (int i = tid; i < p.Co; i += 256) sbias[i] = p.bias ? p.bias[i] : 0.f;
+  for (int i = tid; i < CO; i += 256) sbias[i] = p.bias ? p.bias[i] : 0.f;
   if (tid < 128) {
     int off = -1;
     if (tid < K) {
@@ -117,22 +76,8 @@ __global__ void __launch_bounds__(256, kSplit ? 1 : 2) conv_stem_kernel(const St
     }
     lut[tid] = off;
   }
-  if (tid == 0) {
-    mbar_init(bar0, 1);
-    mbar_init(bar1, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(p.tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(gen + offBar + 16);
-  constexpr uint32_t kFmt = kSplit ? 0u : 1u;   // operand format: bf16, or fp16 for the split planes
-  const uint32_t idesc = (1u << 4) | (kFmt << 7) | (kFmt << 10) | ((uint32_t)(p.Co >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
 
   auto decode = [&](long long tile, int& b, int& t, int& h0, int& w0) {
     const int tw = (int)(tile % p.tilesW);
@@ -145,7 +90,7 @@ __global__ void __launch_bounds__(256, kSplit ? 1 : 2) conv_stem_kernel(const St
     w0 = tw * BW;
   };
   // Halo patch of one tile: the global loads are issued back to back into registers (kPatchIt per thread) so that their
-  // latency overlaps the epilogue of the previous tile; they are stored to shared memory afterwards.
+  // latency overlaps the MMAs and the epilogue of the previous tile; they are stored to shared memory afterwards.
   auto load_patch = [&](long long tile, float (&pv)[kPatchIt]) {
     int b, t, h0, w0;
     decode(tile, b, t, h0, w0);
@@ -185,12 +130,12 @@ __global__ void __launch_bounds__(256, kSplit ? 1 : 2) conv_stem_kernel(const St
       if (i < patch_floats) patch[i] = pv[k];
     }
   };
-  // im2col rows of the staged patch into A buffer `buf` (canonical K-major SWIZZLE_128B layout)
-  auto im2col = [&](int buf) {
+  // im2col rows of the staged patch into the A tile (canonical K-major SWIZZLE_128B layout)
+  auto im2col = [&]() {
     const int row = tid & 127, half = tid >> 7;
     const int dh = row / BW, dw = row % BW;
     const float* prow = patch + dh * PW + dw;
-    uint8_t* arow = gen + offA + buf * (kPl * kATile) + row * 128;
+    uint8_t* arow = gen + offA + row * 128;
     const int u_begin = half == 0 ? 0 : (units + 1) / 2, u_end = half == 0 ? (units + 1) / 2 : units;
     for (int u = u_begin; u < u_end; ++u) {
       float f[8];
@@ -220,102 +165,80 @@ __global__ void __launch_bounds__(256, kSplit ? 1 : 2) conv_stem_kernel(const St
     }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   };
-  auto issue = [&](int buf) {
-    if (tid == 0) {
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t sa = base + offA + buf * (kPl * kATile), sb = base + offB;
-      uint32_t accum = 0;
+  // warpgroup g multiplies rows [64 g, 64 g + 64) of the A tile by the weights
+  const int g = warp >> 2, wq = warp & 3;
+  float acc[CO / 2];
+  auto issue = [&]() {
+    const uint32_t sa = base + offA + (uint32_t)g * 64u * 128u, sb = base + offB;
+    const uint32_t hi = tcx::desc_hi(1024u);
+    tcx::wgmma_fence();
 #pragma unroll
-      for (int kc = 0; kc < 2; ++kc)
+    for (int kc = 0; kc < 2; ++kc)
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const uint64_t ah = make_sdesc(sa + kc * (128 * 128)) + (uint64_t)(k * 2);
-          const uint64_t bh = make_sdesc(sb + kc * (p.Co * 128)) + (uint64_t)(k * 2);
-          umma_f16(tmem_base + (uint32_t)(buf * p.Co), ah, bh, idesc, accum);
-          accum = 1;
-          if constexpr (kSplit) {
-            const uint64_t al = make_sdesc(sa + kATile + kc * (128 * 128)) + (uint64_t)(k * 2);
-            const uint64_t bl = make_sdesc(sb + p.Co * 256 + kc * (p.Co * 128)) + (uint64_t)(k * 2);
-            umma_f16(tmem_base + (uint32_t)(buf * p.Co), al, bh, idesc, 1u);
-            umma_f16(tmem_base + (uint32_t)(buf * p.Co), ah, bl, idesc, 1u);
-          }
+      for (int k = 0; k < 4; ++k) {
+        const uint32_t al = tcx::desc_lo(sa + kc * (128 * 128)) + (uint32_t)(k * 2);
+        const uint32_t bl = tcx::desc_lo(sb + kc * (CO * 128)) + (uint32_t)(k * 2);
+        tcx::wgmma_k16<CO, kSplit>(acc, tcx::desc(al, hi), tcx::desc(bl, hi), (kc | k) ? 1u : 0u);
+        if constexpr (kSplit) {
+          tcx::wgmma_k16<CO, kSplit>(acc, tcx::desc(al + (kATile >> 4), hi), tcx::desc(bl, hi), 1u);
+          tcx::wgmma_k16<CO, kSplit>(acc, tcx::desc(al, hi), tcx::desc(bl + ((CO * 256) >> 4), hi), 1u);
         }
-      asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(buf ? bar1 : bar0) : "memory");
-    }
+      }
+    tcx::wgmma_commit();
   };
-  auto epilogue = [&](long long tile, int buf, uint32_t parity) {
-    mbar_wait(buf ? bar1 : bar0, parity);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+  auto epilogue = [&](long long tile) {
     int b, t, h0, w0;
     decode(tile, b, t, h0, w0);
-    const int q = warp & 3, half = warp >> 2;
-    const int row = q * 32 + lane;
-    const int h = h0 + row / BW, w = w0 + row % BW;
-    const bool valid = h < p.H && w < p.W;
-    const int ncols = p.Co / 2;
-    bf16* orow = p.out + ((((long long)b * p.To + t) * p.H + h) * p.W + w) * (p.Co * (int)kPl) + half * ncols;
-    const uint32_t tb = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * p.Co + half * ncols);
-    for (int j = 0; j < ncols; j += 32) {
-      uint32_t v[32];
-      tmem_ld32(tb + (uint32_t)j, v);
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      if (valid) {
+    const int cq = 2 * (lane & 3);
 #pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          uint4 pk, pl;
+    for (int r = 0; r < 2; ++r) {
+      const int row = 64 * g + 16 * wq + (lane >> 2) + 8 * r;
+      const int h = h0 + row / BW, w = w0 + row % BW;
+      if (h >= p.H || w >= p.W) continue;
+      bf16* orow = p.out + ((((long long)b * p.To + t) * p.H + h) * p.W + w) * (CO * (int)kPl);
 #pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const int c = j + g * 8 + 2 * e;
-            if constexpr (kSplit) {
-              const float f0 = fmaf(__uint_as_float(v[g * 8 + 2 * e]), p.acc_scale, sbias[half * ncols + c]);
-              const float f1 = fmaf(__uint_as_float(v[g * 8 + 2 * e + 1]), p.acc_scale, sbias[half * ncols + c + 1]);
-              __half2* h2 = reinterpret_cast<__half2*>(&pk);
-              __half2* l2 = reinterpret_cast<__half2*>(&pl);
-              h2[e] = __floats2half2_rn(split_sat(f0), split_sat(f1));
-              const float2 hf = __half22float2(h2[e]);
-              l2[e] = __floats2half2_rn(split_sat(f0 - hf.x), split_sat(f1 - hf.y));
-            } else {
-              const float f0 = __uint_as_float(v[g * 8 + 2 * e]) + sbias[half * ncols + c];
-              const float f1 = __uint_as_float(v[g * 8 + 2 * e + 1]) + sbias[half * ncols + c + 1];
-              reinterpret_cast<__nv_bfloat162*>(&pk)[e] = __floats2bfloat162_rn(f0, f1);
-            }
-          }
-          *reinterpret_cast<uint4*>(orow + j + g * 8) = pk;
-          if constexpr (kSplit) *reinterpret_cast<uint4*>(orow + p.Co + j + g * 8) = pl;
+      for (int j = 0; j < CO / 8; ++j) {
+        const int c = 8 * j + cq;
+        if constexpr (kSplit) {
+          const float f0 = fmaf(acc[4 * j + 2 * r], p.acc_scale, sbias[c]);
+          const float f1 = fmaf(acc[4 * j + 2 * r + 1], p.acc_scale, sbias[c + 1]);
+          const __half2 h2 = __floats2half2_rn(split_sat(f0), split_sat(f1));
+          const float2 hf = __half22float2(h2);
+          const __half2 l2 = __floats2half2_rn(split_sat(f0 - hf.x), split_sat(f1 - hf.y));
+          *reinterpret_cast<__half2*>(orow + c) = h2;
+          *reinterpret_cast<__half2*>(orow + CO + c) = l2;
+        } else {
+          *reinterpret_cast<__nv_bfloat162*>(orow + c) =
+              __floats2bfloat162_rn(acc[4 * j + 2 * r] + sbias[c], acc[4 * j + 2 * r + 1] + sbias[c + 1]);
         }
       }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   };
 
   long long tile = blockIdx.x;
-  uint32_t it = 0;
   float pv[kPatchIt];
   if (tile < p.num_tiles) {
     load_patch(tile, pv);
     store_patch(pv);
     __syncthreads();
-    im2col(0);
+    im2col();
     __syncthreads();
-    issue(0);
   }
-  for (; tile < p.num_tiles; tile += gridDim.x, ++it) {
+  for (; tile < p.num_tiles; tile += gridDim.x) {
     const long long next = tile + gridDim.x;
     const bool has_next = next < p.num_tiles;
-    const int buf = it & 1;
-    if (has_next) load_patch(next, pv);     // loads in flight across the epilogue
-    epilogue(tile, buf, (it >> 1) & 1u);
-    if (has_next) store_patch(pv);
-    __syncthreads();
-    if (has_next) im2col(buf ^ 1);
-    __syncthreads();
-    if (has_next) issue(buf ^ 1);
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 2) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(p.tmem_cols) : "memory");
+    issue();
+    if (has_next) load_patch(next, pv);     // loads in flight across the MMAs and the epilogue
+    tcx::wgmma_wait<0>();
+    tcx::acc_fence(acc);
+    epilogue(tile);
+    __syncthreads();                        // both warpgroups are done with the A tile and the patch
+    if (has_next) {
+      store_patch(pv);
+      __syncthreads();
+      im2col();
+      __syncthreads();
+    }
   }
 }
 
@@ -342,7 +265,7 @@ cudaError_t launch_stem_cache_update(const float* x, float* cache, int B, int Ci
   if (t_rep + T < 2) return cudaErrorInvalidValue;
   const long long total = (long long)B * Ci * 2 * H * W;
   long long g = (total + 255) / 256;
-  if (g > 148 * 8) g = 148 * 8;
+  if (g > 132 * 8) g = 132 * 8;
   stem_cache_update_kernel<<<(unsigned)g, 256, 0, s>>>(x, cache, B, Ci, T, t_rep, (long long)H * W);
   count_launch();
   return cudaGetLastError();
@@ -351,7 +274,7 @@ cudaError_t launch_stem_cache_update(const float* x, float* cache, int B, int Ci
 bool conv_stem_supported(const ConvP& p) {
   if (p.kt != 3 || p.kh != 3 || p.kw != 3 || p.st != 1 || p.sh != 1 || p.sw != 1) return false;
   if (p.ut != 1 || p.uh != 1 || p.uw != 1 || p.to_off != 0 || p.res_mode != 0) return false;
-  if (p.Ci * 27 > 128 || p.Co % 64 != 0 || p.Co > (p.split ? 128 : 256)) return false;
+  if (p.Ci * 27 > 128 || (p.Co != 64 && p.Co != 128 && p.Co != 256) || p.Co > (p.split ? 128 : 256)) return false;
   if (p.t_mode == 2 && (!p.cache || p.cacheT != 2)) return false;
   if ((p.pt != 2 && p.pt != 1) || p.ph != 1 || p.pw != 1) return false;
   if (p.pt == 1 && (p.t_mode != 0 || p.t_rep != 0)) return false;   // symmetric padding: v1.0 non-causal only
@@ -373,36 +296,33 @@ cudaError_t launch_conv_stem(const ConvP& p, const float* x, const bf16* wpk, bf
   t.acc_scale = (p.split && p.acc_scale != 0.f) ? p.acc_scale : 1.0f;
   t.tilesW = (p.Wi + BW - 1) / BW; t.tilesH = (p.Hi + BH - 1) / BH;
   t.num_tiles = (long long)p.B * p.To * t.tilesH * t.tilesW;
-  uint32_t cols = 32;
-  while (cols < (uint32_t)(2 * p.Co)) cols <<= 1;
-  t.tmem_cols = cols;
   const size_t pl = p.split ? 2 : 1;
-  const size_t smem = 1024 + pl * 2 * kATile + pl * (size_t)p.Co * 256 + (((size_t)p.Ci * 3 * PH * PW * 4 + 15) & ~(size_t)15) + 256 * 4 + 128 * 4 + 64;
-  // per-device state: the attribute applies to the current device only (ADVICE r1)
-  static bool attr[64] = {false};
-  static int sms[64] = {0};
+  const size_t smem = 1024 + pl * kATile + pl * (size_t)p.Co * 256 + (((size_t)p.Ci * 3 * PH * PW * 4 + 15) & ~(size_t)15) + 256 * 4 + 128 * 4;
   int dev = 0;
   cudaGetDevice(&dev);
-  if (dev < 0 || dev >= 64) return cudaErrorInvalidDevice;
-  if (!attr[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(conv_stem_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_stem_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
-    if (e != cudaSuccess) return e;
-    attr[dev] = true;
-    cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, dev);
-    if (sms[dev] <= 0) sms[dev] = 148;
-  }
-  const int num_sms = sms[dev];
+  int num_sms = 0;
+  cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
+  if (num_sms <= 0) num_sms = 132;
   const double M = (double)t.num_tiles * 128;
   char det[96] = "";
   if (prof_enabled()) snprintf(det, sizeof(det), "k333 %d->%d @%dx%dx%d", p.Ci, p.Co, p.To, p.Hi, p.Wi);
   ProfScope _ps(p.split ? "conv_stem3" : "conv_stem", 2.0 * M * 27 * p.Ci * p.Co, (double)p.B * p.Ci * p.Ti * p.Hi * p.Wi * 4.0 + M * p.Co * 2.0 * pl, s, det);
-  // two CTAs per SM when both fit (shared memory and the 512 TMEM columns)
-  const int per_sm = (!p.split && 2 * (smem + 1024) <= 227 * 1024 && 2 * (int)t.tmem_cols <= 512) ? 2 : 1;
-  const long long slots = (long long)per_sm * num_sms;
-  const unsigned grid = (unsigned)(t.num_tiles < slots ? t.num_tiles : slots);
-  if (p.split) conv_stem_kernel<true><<<grid, 256, smem, s>>>(t, wpk);
-  else conv_stem_kernel<false><<<grid, 256, smem, s>>>(t, wpk);
+  // as many resident CTAs per SM as fit: the phases of a tile (patch loads -> im2col -> MMA -> epilogue) are serialised
+  // inside a CTA by block barriers, and a second resident CTA fills the bubbles
+  auto launch = [&](auto kern) -> cudaError_t {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    int per_sm = 1;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 256, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
+    const long long slots = (long long)per_sm * num_sms;
+    const unsigned grid = (unsigned)(t.num_tiles < slots ? t.num_tiles : slots);
+    kern<<<grid, 256, smem, s>>>(t, wpk);
+    return cudaSuccess;
+  };
+  cudaError_t e;
+  if (p.split) e = p.Co == 64 ? launch(conv_stem_kernel<64, true>) : launch(conv_stem_kernel<128, true>);
+  else e = p.Co == 64 ? launch(conv_stem_kernel<64, false>) : p.Co == 128 ? launch(conv_stem_kernel<128, false>) : launch(conv_stem_kernel<256, false>);
+  if (e != cudaSuccess) return e;
   count_launch();
   return cudaGetLastError();
 }

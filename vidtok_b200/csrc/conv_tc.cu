@@ -1,23 +1,24 @@
-// tcgen05 / TMA implicit-GEMM convolution for sm_100a (the BF16-mode hot kernel).
+// wgmma / TMA implicit-GEMM convolution for sm_90a (the tensor-core hot kernel).
 //
 // GEMM view of a causal convolution on channels-last activations [B,T,H,W,C]:
-//   M = output positions, tiled as boxes of BT x BH x BW = 128 positions (one UMMA M=128 tile),
-//   N = Cout tile (BN <= 256 TMEM columns, fp32 accumulators, double-buffered: 2*BN columns),
+//   M = output positions, tiled as boxes of BT x BH x BW = 128 positions per CTA tile (two 64-row wgmma tiles, one per
+//       consumer warpgroup),
+//   N = Cout tile (BN in {32, 64, 128, 256}; fp32 accumulators in registers, BN / 2 per consumer thread),
 //   K = taps x Cin, consumed in steps of 64 channels (one 128-byte swizzle row) per tap.
 // A operand, two formulations:
 //   * halo mode (stride-1 kh x kw > 1 layers): ONE 5-D TMA box per (time tap, 64-channel chunk) loads the CTA tile's input
-//     window with its spatial halo; the kh*kw taps are UMMA descriptors that start (bb*hP + c) 128-byte rows into it
+//     window with its spatial halo; the kh*kw taps are wgmma descriptors that start (bb*hP + c) 128-byte rows into it
 //     (TcParams::halo).  ~3x fewer activation bytes cross L2 -> SM.
 //   * otherwise one box {64, BW, BH, BT, 1} at (c0, w0+dw, h0+dh, t, b) per (tap, 64-channel chunk).
 //   In both, spatial/temporal zero padding is the TMA out-of-bounds fill; the causal front pad is either skipped taps
 //   (zeros), a clamped coordinate (replicate, v1.1 first chunk) or a second tensor map over the per-layer cache (v1.1
 //   later chunks).  No im2col buffer, no padded copy.
-// B operand: TMA box {64, BN} of the pre-packed K-major bf16 weights [Cout][taps*Cin] (half of it per CTA in pair mode).
-// Both land in shared memory in the canonical K-major SWIZZLE_128B layout and feed tcgen05.mma.kind::f16 (K=16):
-// cta_group::1 with M=128, or cta_group::2 with M=256 across a CTA pair (template kPair); accumulators live in TMEM.
-// Warp roles (persistent CTA, one per SM): warp0 = TMA producer, warp1 = MMA issuer, warp2 = TMEM allocator,
-// warps 3-10 = epilogue (tcgen05.ld -> bias / residual / mix / LayerNorm -> bf16 -> per-warp swizzled staging -> TMA
-// store), overlapping the next tile's main loop through the second TMEM accumulator stage.
+// B operand: TMA box {64, BN} of the pre-packed K-major bf16 weights [Cout][taps*Cin].
+// Both land in shared memory in the canonical K-major SWIZZLE_128B layout and feed wgmma.mma_async m64nBNk16.
+// Warp roles (persistent CTA, one per SM): warps 0-7 = two consumer warpgroups (wgmma on rows [64 g, 64 g + 64) of the tile,
+// then the epilogue straight from the accumulator registers: bias / residual / mix / LayerNorm / regularizer -> global
+// memory), warp 8 = TMA producer, which runs up to `stages` K steps ahead, across tile boundaries too, so that the next
+// tile's operands load while the epilogue runs.
 #include <cuda.h>
 
 #include <cstdio>
@@ -35,21 +36,10 @@ namespace vt {
 namespace {
 
 thread_local std::string g_tc_err;
-// cta_group::2 (CTA pairs) halve the weight bytes each CTA stages and reads per FLOP (profiles/notes_r1.md).
-// VT_TC_PAIR: unset / 1 = every layer with enough tiles, 0 = off, 2 = forced whenever the geometry allows, 3 = N = 256 tiles only.
-int g_pair_mode = -2;   // -2 unread, -1 default policy, 0 off, 1 all large layers, 2 forced
-int pair_mode() {
-  if (g_pair_mode == -2) {
-    const char* e = getenv("VT_TC_PAIR");
-    g_pair_mode = e ? atoi(e) : -1;
-  }
-  return g_pair_mode;
-}
 
 struct TcParams {
   int B, To, Ho, Wo, Co, Ti;
-  int BW, BH, BT;            // TMA box = BT x BH x BW positions = MT * 128 rows
-  int MT;                    // M tiles (UMMA M=128 each) per CTA tile: 2 when BN <= 128 (shares one B tile)
+  int BW, BH, BT;            // TMA box = BT x BH x BW positions = 128 rows
   int tilesW, tilesH, tilesT;
   int num_n_tiles, BN;
   long long num_tiles;
@@ -58,7 +48,6 @@ struct TcParams {
   int sp;                    // spatial stride (1 or 2, same in H and W)
   int t_mode, cacheT;
   int stages;
-  uint32_t tmem_cols;
   const float* bias;
   int res_mode;
   const bf16* res;
@@ -79,42 +68,32 @@ struct TcParams {
   // residual add through the tensor pipe: BN/64 extra K steps with A = residual tile (TMA) and B = a slice of the
   // identity matrix, so `+ x` costs no epilogue work at all (res_mode 1 with ra == rb == 1)
   int res_mma;
-  // coalesced epilogue: every epilogue warp stages its 32 rows x 64 channels of bf16 results in shared memory
-  // (SWIZZLE_128B rows) and writes them with its own TMA tensor store of a {64, qw, qh, qt} box (partial tiles are
-  // clipped by the tensor bounds)
-  int tma_store;
-  int stg_bufs;              // staging buffers per warp (4 KB each): 2 when shared memory allows, else 1
-  int store_stream;          // TMA stores carry an L2 evict-first hint (outputs much larger than L2)
-  uint32_t stage_off;        // byte offset of the staging buffers [8 warps][stg_bufs][4 KB] from the aligned smem base
-  // cta_group::2: two CTAs of a cluster (one TPC) work on one 2*MT*128-row tile; each loads its own rows of A and half of
-  // the B (weight) rows, the leader issues M=256 MMAs that read both halves -> weight bytes per FLOP are halved again
-  int pair;
-  int tileBH, tileBT;        // box of the whole (pair) tile; BH/BT above are the per-CTA box
   // halo mode (stride-1 spatial kernels): ONE TMA box per (time tap, 64-channel chunk) brings the input window of the
   // whole CTA tile plus its spatial halo ({64, hP, BH + kh - 1} rows of 128 B) into shared memory; the kh*kw spatial taps
-  // are then UMMA descriptors that start (bb * hP + c) rows into that window, so the activation bytes pulled from L2
-  // drop by ~kh*kw.  The CTA tile is 16 rows x (8 * MT) columns: an 8-row UMMA core group = 8 consecutive columns,
-  // group stride (SBO) = hP rows, and hP % 8 == 0 keeps the swizzle phase of every group equal (= descriptor base offset).
+  // are then wgmma descriptors that start (bb * hP + c) rows into that window, so the activation bytes pulled from L2
+  // drop by ~kh*kw.  The CTA tile is 16 rows x 8 columns: an 8-row core group = 8 consecutive columns, group stride
+  // (SBO) = hP rows, and hP % 8 == 0 keeps the swizzle phase of every group equal.
   int halo, hP, a_stages;
   uint32_t halo_bytes;
   // split operands (EXACT_TC mode, kernel template kSplit): activations and weights are stored as two fp16 planes
   // hi = fp16(v), lo = fp16(v - hi) side by side in the channel dimension ([..., hi(C) | lo(C)]); every K step loads
-  // A_hi, A_lo, B_hi, B_lo and issues A_hi*B_hi + A_lo*B_hi + A_hi*B_lo into the same fp32 TMEM accumulator
+  // A_hi, A_lo, B_hi, B_lo and issues A_hi*B_hi + A_lo*B_hi + A_hi*B_lo into the same fp32 accumulator
   // (error ~2^-21 per product: fp32-class results on the 16-bit tensor pipe).  Channel coordinate of the lo plane:
   int split, a_lo, b_lo, o_lo;   // = Cin, Kpad, Cout
   float acc_scale;               // split: accumulator scale 2^-s of the pre-scaled weights
   // split, long K: the tensor core's fp32 accumulation is the dominant error there (it grows with the number of chained
-  // MMAs: measured 2e-4 at K = 13824 against 1e-5 at K = 200), so the K steps of a tile are dealt round-robin onto `kparts`
-  // partial accumulators in TMEM which the epilogue adds in fp32 (round-to-nearest); the accumulator is then not double
-  // buffered across tiles (acc_stages = 1)
-  int kparts, acc_stages;
-  // regularizer epilogue on the fp32 heads (TcRegFusion): the owner of a row holds every channel of its position
+  // MMAs), so the K steps of a tile are summed in `kparts` consecutive groups, each accumulated by the tensor core from
+  // zero and added to a running fp32 sum with round-to-nearest (BN <= 128: the sum needs a second register set)
+  int kparts;
+  // regularizer epilogue on the fp32 heads (TcRegFusion): the row of a position is gathered in shared memory and the
+  // thread that owns it holds every channel
   int reg_mode, reg_zc, reg_sample;
   const float* reg_noise;
   float* reg_z;
   int* reg_idx;
   double* reg_kl;
   FsqConst reg_fsq;
+  uint32_t misc_off;         // byte offset of [bias | gamma | beta] x 2 and the regularizer row buffer from the aligned base
 };
 
 struct TcMaps {
@@ -123,22 +102,21 @@ struct TcMaps {
   CUtensorMap b;             // weights
   CUtensorMap r;             // residual tensor (output geometry), box = A box
   CUtensorMap e;             // 256 x 256 bf16 identity
-  CUtensorMap o;             // output store map
-  CUtensorMap o2;            // second output (fused LayerNorm result)
 };
 
-constexpr int kEpiWarps = 8;
-constexpr int kEpiWarp0 = 3;            // first epilogue warp (any 8 consecutive warps cover every TMEM lane quarter twice)
-constexpr int kThreads = (kEpiWarp0 + kEpiWarps) * 32;
-constexpr int kABytes = 128 * 128;  // 128 rows x 64 bf16
+constexpr int kConsumerWarps = 8;       // warps 0-7: two wgmma warpgroups
+constexpr int kProducerWarp = kConsumerWarps;
+// warps 8-11: the producer warpgroup (warp 8 issues the TMA loads); registers are allocated per warpgroup, so it hands
+// most of its share to the consumers (setmaxnreg)
+constexpr int kThreads = (kConsumerWarps + 4) * 32;
+constexpr int kABytes = 128 * 128;      // 128 rows x 64 bf16
 
 using namespace tcx;
 
 struct TileCoord {
   int b, t0, h0, w0, n0;
-  int tt0;   // first frame of the whole (pair) tile: tap skipping must be decided identically by both CTAs of a pair
 };
-__device__ __forceinline__ TileCoord decode_tile(const TcParams& p, long long tile, int rank) {
+__device__ __forceinline__ TileCoord decode_tile(const TcParams& p, long long tile) {
   TileCoord c;
   const int nt = (int)(tile % p.num_n_tiles);
   long long m = tile / p.num_n_tiles;
@@ -146,20 +124,14 @@ __device__ __forceinline__ TileCoord decode_tile(const TcParams& p, long long ti
   const int th = (int)(m % p.tilesH); m /= p.tilesH;
   const int tt = (int)(m % p.tilesT);
   c.b = (int)(m / p.tilesT);
-  // origin of THIS CTA's box inside the (pair) tile: the second CTA takes the upper half in t (if the tile spans
-  // several frames) or in h
-  c.tt0 = tt * p.tileBT;
-  c.t0 = c.tt0 + ((p.pair && p.tileBT != p.BT) ? rank * p.BT : 0);
-  c.h0 = th * p.tileBH + ((p.pair && p.tileBT == p.BT) ? rank * p.BH : 0);
-  c.w0 = tw * p.BW; c.n0 = nt * p.BN;
+  c.t0 = tt * p.BT; c.h0 = th * p.BH; c.w0 = tw * p.BW; c.n0 = nt * p.BN;
   return c;
 }
 // time coordinate of a tap for a tile; returns false when the whole box is causal zero padding (tap skipped)
 __device__ __forceinline__ bool tap_time(const TcParams& p, const TileCoord& tc, int a, int& tv, bool& from_cache) {
   tv = (tc.t0 + p.to_off) * p.st + a - p.pt;
   from_cache = false;
-  const int tv_tile = (tc.tt0 + p.to_off) * p.st + a - p.pt;
-  if (tv_tile + p.tileBT <= 0) {
+  if (tv + p.BT <= 0) {
     if (p.t_mode == 0) return false;
     if (p.t_mode == 1) { tv = 0; return true; }
     from_cache = true;
@@ -169,133 +141,93 @@ __device__ __forceinline__ bool tap_time(const TcParams& p, const TileCoord& tc,
   return true;
 }
 
-// Warp roles: 0 = TMA producer, 1 = MMA issuer, 2 = TMEM allocator, 3..10 = epilogue (two warps per TMEM
-// lane quarter, alternating 32-column chunks).
-template <bool kPair, bool kSplit>
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  v += __shfl_xor_sync(0xffffffffu, v, 2);
+  return v;
+}
+
+template <int BN, bool kSplit>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_tc_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  int rank = 0;
-  if constexpr (kPair) rank = (int)cluster_ctarank();     // 0 = leader of the CTA pair
-  const long long tile0 = kPair ? (long long)(blockIdx.x >> 1) : (long long)blockIdx.x;
-  const long long tile_step = kPair ? (long long)(gridDim.x >> 1) : (long long)gridDim.x;
-  const uint32_t a_bytes = (uint32_t)p.MT * kABytes;
-  const int bn_local = kPair ? p.BN / 2 : p.BN;           // weight rows this CTA stages
-  const uint32_t b_bytes = (uint32_t)bn_local * 128u;
+  const uint32_t a_bytes = kABytes;
+  constexpr uint32_t b_bytes = (uint32_t)BN * 128u;
   constexpr uint32_t kPl = kSplit ? 2u : 1u;               // operand planes per tile (hi | lo)
   // stage layout: [A_hi | A_lo | B_hi | B_lo] (A part absent in halo mode: the stage ring then holds B tiles only)
   const uint32_t stage_bytes = kPl * (p.halo ? b_bytes : a_bytes + b_bytes);
   const uint32_t win_bytes = kPl * p.halo_bytes;           // one halo window slot: [hi window | lo window]
   const uint32_t ring_base = smem_base + (p.halo ? (uint32_t)p.a_stages * win_bytes : 0u);
-  const uint32_t bar_base = ring_base + p.stages * stage_bytes + (p.tma_store ? (uint32_t)(kEpiWarps * p.stg_bufs) * 4096u : 0u);
-  // barriers: full[stages], empty[stages], tmem_full[2], tmem_empty[2], fullA[a_stages], emptyA[a_stages];
-  // then tmem ptr; then bias[2][256]
+  const uint32_t bar_base = ring_base + p.stages * stage_bytes;
+  // barriers: full[stages], empty[stages], fullA[a_stages], emptyA[a_stages]
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (p.stages + s); };
-  auto tfull_bar = [&](int s) { return bar_base + 8u * (2 * p.stages + s); };
-  auto tempty_bar = [&](int s) { return bar_base + 8u * (2 * p.stages + 2 + s); };
-  auto fullA_bar = [&](int s) { return bar_base + 8u * (2 * p.stages + 4 + s); };
-  auto emptyA_bar = [&](int s) { return bar_base + 8u * (2 * p.stages + 4 + p.a_stages + s); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * p.stages + 4 + 2 * p.a_stages);
-  const uint32_t bias_base = tmem_slot + 16u;
-  uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(smem_gen + (tmem_slot - smem_base));
-  float* sbias = reinterpret_cast<float*>(smem_gen + (bias_base - smem_base));   // [2][bias 256 | gamma 256 | beta 256]
-  float* stat_s = sbias + 2 * 768;                                                // [tile parity][2 groups][128 rows][sum, sumsq]
+  auto fullA_bar = [&](int s) { return bar_base + 8u * (2 * p.stages + s); };
+  auto emptyA_bar = [&](int s) { return bar_base + 8u * (2 * p.stages + p.a_stages + s); };
+  float* sbias = reinterpret_cast<float*>(smem_gen + p.misc_off);   // [2][bias 256 | gamma 256 | beta 256]
+  float* rowbuf = sbias + 2 * 768;                                   // regularizer: [128 rows][33]
 
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&maps.a[0]);
-    prefetch_tmap(&maps.b);
-    if (p.sp == 2) { prefetch_tmap(&maps.a[1]); prefetch_tmap(&maps.a[2]); prefetch_tmap(&maps.a[3]); }
-    if (p.t_mode == 2) prefetch_tmap(&maps.c);
-    if (p.res_mma) { prefetch_tmap(&maps.r); prefetch_tmap(&maps.e); }
-    if (p.tma_store) { prefetch_tmap(&maps.o); if (p.ln_mode == 2) prefetch_tmap(&maps.o2); }
-  }
-  if (warp == 1 && lane == 0) {
-    // pair mode: the leader's full barrier collects the transaction bytes of both CTAs' TMA loads; the leader's tmem_empty
-    // barrier collects both CTAs' epilogue warps
+  if (threadIdx.x == 0) {
+    // a stage / window is released by every consumer warp once its own wait has seen the MMAs that read it complete
+    // (wgmma.wait_group tracks the executing warp's share of the warpgroup's MMAs)
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(tfull_bar(s), 1);
-      mbar_init(tempty_bar(s), kPair ? 2 * kEpiWarps : kEpiWarps);
+      mbar_init(empty_bar(s), kConsumerWarps);
     }
     for (int s = 0; s < p.a_stages; ++s) {
       mbar_init(fullA_bar(s), 1);
-      mbar_init(emptyA_bar(s), 1);
+      mbar_init(emptyA_bar(s), kConsumerWarps);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) {
-    if constexpr (kPair) {
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(p.tmem_cols) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    } else {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(p.tmem_cols) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-  }
-  tc_fence_before();
-  if constexpr (kPair) cluster_sync_all(); else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
+  __syncthreads();
 
-  // Producer and MMA issuer run with the WHOLE warp converged and elect one lane only around the asynchronous
-  // instructions: all addresses / coordinates are then warp-uniform values the compiler keeps on the uniform datapath,
-  // so a K step costs a few dozen issue slots.  (A single-lane `if (lane == 0)` loop makes every UTCHMMA / UTMALDG a
-  // vote + broadcast sequence; the issuing thread, not the tensor pipe, was the limit: profiles/notes_r1.md.)
   const int nsp = p.kh * p.kw;
   const int num_kc = p.num_kc, nstages = p.stages;
   const bool halo = p.halo != 0;
-  const int res_steps = p.res_mma ? p.BN / 64 : 0;
+  const int res_steps = p.res_mma ? BN / 64 : 0;
 
-  if (warp == 0) {
+  if (warp >= kProducerWarp) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+    if (warp != kProducerWarp) return;
     // ===================== TMA producer =====================
+    // The whole warp stays converged and elects one lane around the asynchronous instructions: addresses and
+    // coordinates are warp-uniform values on the uniform datapath.
     const bool el = elect_one();
+    if (el) {
+      prefetch_tmap(&maps.a[0]);
+      prefetch_tmap(&maps.b);
+      if (p.sp == 2) { prefetch_tmap(&maps.a[1]); prefetch_tmap(&maps.a[2]); prefetch_tmap(&maps.a[3]); }
+      if (p.t_mode == 2) prefetch_tmap(&maps.c);
+      if (p.res_mma) { prefetch_tmap(&maps.r); prefetch_tmap(&maps.e); }
+    }
     int stage = 0, sA = 0;
     uint32_t phase = 0, phA = 0;
-    // B (or A|B) stage: wait for the slot, post the expected bytes (pair mode: the leader posts both CTAs' bytes, the
-    // peer's loads credit the leader's barrier directly; the peer cannot run ahead of the phase because it waits on its
-    // own empty barrier, which the leader's multicast commit signals)
     auto acquire = [&](uint32_t bytes) {
       mbar_wait(empty_bar(stage), phase ^ 1u);
-      if (el) {
-        if constexpr (!kPair) mbar_expect_tx(full_bar(stage), bytes);
-        else if (rank == 0) mbar_expect_tx(full_bar(stage), 2u * bytes);
-      }
+      if (el) mbar_expect_tx(full_bar(stage), bytes);
     };
     auto advance = [&]() { if (++stage == nstages) { stage = 0; phase ^= 1u; } };
-    auto load_b = [&](uint32_t dst, const CUtensorMap* m, int c0, int c1, int c2) {
-      if constexpr (kPair) tma_load_3d_2sm(dst, m, full_bar(stage), c0, c1, c2);
-      else tma_load_3d(dst, m, full_bar(stage), c0, c1, c2);
-    };
-    auto load_a = [&](uint32_t dst, uint32_t bar, const CUtensorMap* m, int c0, int cw, int ch, int ct, int cb) {
-      if constexpr (kPair) tma_load_5d_2sm(dst, m, bar, c0, cw, ch, ct, cb);
-      else tma_load_5d(dst, m, bar, c0, cw, ch, ct, cb);
-    };
     // weight tile(s) of one K step into the B part of the current stage (split: hi plane, then lo plane at k + b_lo)
     auto load_b_planes = [&](uint32_t dst, const CUtensorMap* m, int kcol, int n, int wb_) {
-      load_b(dst, m, kcol, n, wb_);
-      if constexpr (kSplit) load_b(dst + b_bytes, m, p.b_lo + kcol, n, wb_);
+      tma_load_3d(dst, m, full_bar(stage), kcol, n, wb_);
+      if constexpr (kSplit) tma_load_3d(dst + b_bytes, m, full_bar(stage), p.b_lo + kcol, n, wb_);
     };
     // halo window of one (time tap, 64-channel chunk); lo_off = channel offset of the lo plane in that tensor
     auto load_window = [&](const CUtensorMap* m, int c0, int lo_off, int cw, int ch, int ct, int cb) {
       mbar_wait(emptyA_bar(sA), phA ^ 1u);
       if (el) {
-        if constexpr (!kPair) mbar_expect_tx(fullA_bar(sA), win_bytes);
-        else if (rank == 0) mbar_expect_tx(fullA_bar(sA), 2u * win_bytes);
-        load_a(smem_base + (uint32_t)sA * win_bytes, fullA_bar(sA), m, c0, cw, ch, ct, cb);
-        if constexpr (kSplit) load_a(smem_base + (uint32_t)sA * win_bytes + p.halo_bytes, fullA_bar(sA), m, lo_off + c0, cw, ch, ct, cb);
+        mbar_expect_tx(fullA_bar(sA), win_bytes);
+        tma_load_5d(smem_base + (uint32_t)sA * win_bytes, m, fullA_bar(sA), c0, cw, ch, ct, cb);
+        if constexpr (kSplit) tma_load_5d(smem_base + (uint32_t)sA * win_bytes + p.halo_bytes, m, fullA_bar(sA), lo_off + c0, cw, ch, ct, cb);
       }
       if (++sA == p.a_stages) { sA = 0; phA ^= 1u; }
     };
-    const int n_off = kPair ? rank * bn_local : 0;
-    for (long long tile = tile0; tile < p.num_tiles; tile += tile_step) {
-      const TileCoord tc = decode_tile(p, tile, rank);
+    for (long long tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+      const TileCoord tc = decode_tile(p, tile);
       const int wb = p.w_batched ? tc.b : 0;
       for (int a = 0; a < p.kt; ++a) {
         int tv;
@@ -308,7 +240,7 @@ conv_tc_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
             int kcol = a * nsp * p.Ci + kc * 64;
             for (int sp = 0; sp < nsp; ++sp, kcol += p.Ci) {
               acquire(stage_bytes);
-              if (el) load_b_planes(ring_base + stage * stage_bytes, &maps.b, kcol, tc.n0 + n_off, wb);
+              if (el) load_b_planes(ring_base + stage * stage_bytes, &maps.b, kcol, tc.n0, wb);
               advance();
             }
           }
@@ -335,9 +267,9 @@ conv_tc_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
                 acquire(stage_bytes);
                 if (el) {
                   const uint32_t sa = smem_base + stage * stage_bytes;
-                  load_a(sa, full_bar(stage), mapA, kc * 64, cw, ch, tv, tc.b);
-                  if constexpr (kSplit) load_a(sa + a_bytes, full_bar(stage), mapA, p.a_lo + kc * 64, cw, ch, tv, tc.b);
-                  load_b_planes(sa + kPl * a_bytes, &maps.b, kcol + kc * 64, tc.n0 + n_off, wb);
+                  tma_load_5d(sa, mapA, full_bar(stage), kc * 64, cw, ch, tv, tc.b);
+                  if constexpr (kSplit) tma_load_5d(sa + a_bytes, mapA, full_bar(stage), p.a_lo + kc * 64, cw, ch, tv, tc.b);
+                  load_b_planes(sa + kPl * a_bytes, &maps.b, kcol + kc * 64, tc.n0, wb);
                 }
                 advance();
               }
@@ -351,612 +283,402 @@ conv_tc_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
         if (halo) {
           load_window(&maps.r, tc.n0 + g * 64, p.o_lo, tc.w0 - p.pw, tc.h0 - p.ph, tc.t0, tc.b);
           acquire(b_bytes);
-          if (el) load_b(ring_base + stage * stage_bytes, &maps.e, g * 64, n_off, 0);
+          if (el) tma_load_3d(ring_base + stage * stage_bytes, &maps.e, full_bar(stage), g * 64, 0, 0);
         } else {
           acquire(kPl * a_bytes + b_bytes);
           if (el) {
             const uint32_t sa = smem_base + stage * stage_bytes;
-            load_a(sa, full_bar(stage), &maps.r, tc.n0 + g * 64, tc.w0, tc.h0, tc.t0, tc.b);
-            if constexpr (kSplit) load_a(sa + a_bytes, full_bar(stage), &maps.r, p.o_lo + tc.n0 + g * 64, tc.w0, tc.h0, tc.t0, tc.b);
-            load_b(sa + kPl * a_bytes, &maps.e, g * 64, n_off, 0);
+            tma_load_5d(sa, &maps.r, full_bar(stage), tc.n0 + g * 64, tc.w0, tc.h0, tc.t0, tc.b);
+            if constexpr (kSplit) tma_load_5d(sa + a_bytes, &maps.r, full_bar(stage), p.o_lo + tc.n0 + g * 64, tc.w0, tc.h0, tc.t0, tc.b);
+            tma_load_3d(sa + kPl * a_bytes, &maps.e, full_bar(stage), g * 64, 0, 0);
           }
         }
         advance();
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (rank == 0) {
-      const bool el = elect_one();
-      const uint32_t idesc = make_idesc(p.BN, kPair ? 256 : 128, kSplit);   // split planes are fp16
-      const int MT = p.MT;
-      const uint32_t BNu = (uint32_t)p.BN;
-      // descriptor words: lo = start >> 4 | LBO(1) << 16 ; hi = SBO >> 4 | version 1 << 14 | SWIZZLE_128B (2) << 29
-      const uint32_t hi_b = 64u | (1u << 14) | (2u << 29);
-      const uint32_t hi_a = halo ? (((uint32_t)p.hP * 8u) | (1u << 14) | (2u << 29)) : hi_b;
-      const uint32_t mt_step = halo ? 64u : (uint32_t)(kABytes >> 4);   // next M tile: 8 window rows / 16 KB
-      const uint32_t b_addr0 = halo ? ring_base : smem_base + kPl * a_bytes;
-      const uint32_t a_pl = (halo ? p.halo_bytes : a_bytes) >> 4;       // descriptor distance hi plane -> lo plane (A)
-      const uint32_t b_pl = b_bytes >> 4;                               // (B)
-      int stage = 0, sA = 0;
-      uint32_t phase = 0, phA = 0;
-      uint32_t it = 0;
-      uint32_t tmem_d = 0;
-      auto mma = [&](uint32_t d, uint32_t alo, uint32_t blo, uint32_t acc) {
-        if constexpr (kPair) umma_f16_2sm_lohi(d, alo, hi_a, blo, hi_b, idesc, acc);
-        else umma_f16_lohi(d, alo, hi_a, blo, hi_b, idesc, acc);
-      };
-      // the 4 K=16 MMAs of one 64-channel step for one M tile; split: hi*hi + lo*hi (+ hi*lo unless `res`: the residual
-      // steps multiply by the identity, which has no lo plane)
-      auto mma64 = [&](uint32_t d, uint32_t a_lo, uint32_t b_lo, uint32_t acc, bool res) {
+    return;
+  }
+
+  // ===================== consumers: wgmma main loop, then the epilogue from the accumulator registers =====================
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+  constexpr int R = BN / 2;                  // accumulator registers per thread
+  constexpr bool kSum = kSplit && BN <= 128;  // running fp32 sum of the K groups (TcParams::kparts)
+  const int g = warp >> 2, wq = warp & 3;
+  const bool leader = lane == 0;
+  const uint32_t hi_b = desc_hi(1024u);
+  const uint32_t hi_a = halo ? desc_hi((uint32_t)p.hP * 128u) : hi_b;
+  // first A row of this warpgroup: 64 rows further into a dense tile, 8 window rows (h) further in halo mode
+  const uint32_t a_row_off = halo ? (uint32_t)(8 * g) * (uint32_t)p.hP * 128u : (uint32_t)g * 64u * 128u;
+  const uint32_t a_pl = halo ? p.halo_bytes : a_bytes;        // hi plane -> lo plane (A)
+  const uint32_t b_addr0 = halo ? ring_base : smem_base + kPl * a_bytes;
+  float acc[R];
+  float sum[kSum ? R : 1];
+  int stage = 0, sA = 0, sR = 0;
+  uint32_t phase = 0, phA = 0;
+  // resources read by the most recent committed MMA group, released once it has completed
+  int pend_stage = -1;
+  bool pend_win = false;
+  auto release = [&]() {
+    if (leader) {
+      if (pend_stage >= 0) mbar_arrive(empty_bar(pend_stage));
+      if (pend_win) mbar_arrive(emptyA_bar(sR));
+    }
+    if (pend_win && ++sR == p.a_stages) sR = 0;
+    pend_stage = -1;
+    pend_win = false;
+  };
+  // one K step (64 channels): this group's 64 A rows at byte address a_addr (a window row), or of the stage's A tile when
+  // a_from_stage, against the B tile of the current stage; split: hi*hi + lo*hi (+ hi*lo unless `res`: the residual steps
+  // multiply by the identity, which has no lo plane)
+  auto kstep = [&](bool a_from_stage, uint32_t a_addr, uint32_t scale, bool res, bool last_of_window) {
+    mbar_wait(full_bar(stage), phase);
+    if (a_from_stage) a_addr = smem_base + stage * stage_bytes + a_row_off;
+    const uint32_t b_addr = b_addr0 + stage * stage_bytes;
+    const uint32_t al = desc_lo(a_addr), bl = desc_lo(b_addr);
+    wgmma_fence();
 #pragma unroll
-        for (uint32_t j = 0; j < 8u; j += 2u) {
-          mma(d, a_lo + j, b_lo + j, j == 0 ? acc : 1u);
-          if constexpr (kSplit) {
-            mma(d, a_lo + a_pl + j, b_lo + j, 1u);
-            if (!res) mma(d, a_lo + j, b_lo + b_pl + j, 1u);
-          }
-        }
-      };
-      // one K step (64 channels): A tile(s) at descriptor word a_lo against the B tile of the current stage
-      uint32_t ks = 0;                                          // K steps issued for the current tile
-      const uint32_t kparts = kSplit ? (uint32_t)p.kparts : 1u;
-      const uint32_t part_cols = (uint32_t)MT * BNu;
-      auto kstep = [&](uint32_t a_lo, uint32_t acc, bool res) {
-        mbar_wait(full_bar(stage), phase);
-        tc_fence_after();
-        if (el) {
-          const uint32_t b_lo = (((b_addr0 + stage * stage_bytes) & 0x3FFFFu) >> 4) | 0x10000u;
-          uint32_t d = tmem_d;
-          if constexpr (kSplit) {
-            if (kparts > 1) { d += (ks % kparts) * part_cols; acc = ks >= kparts ? 1u : 0u; }
-          }
-          mma64(d, a_lo, b_lo, acc, res);
-          if (MT == 2) mma64(d + BNu, a_lo + mt_step, b_lo, acc, res);
-          if constexpr (kPair) umma_commit_2sm(empty_bar(stage)); else umma_commit(empty_bar(stage));
-        }
-        ++ks;
-        if (++stage == nstages) { stage = 0; phase ^= 1u; }
-      };
-      auto stage_a_lo = [&]() { return (((smem_base + stage * stage_bytes) & 0x3FFFFu) >> 4) | 0x10000u; };
-      auto window_lo = [&](int row0) {
-        return (((smem_base + (uint32_t)sA * win_bytes + (uint32_t)row0 * 128u) & 0x3FFFFu) >> 4) | 0x10000u;
-      };
-      auto release_window = [&]() {
-        if (el) { if constexpr (kPair) umma_commit_2sm(emptyA_bar(sA)); else umma_commit(emptyA_bar(sA)); }
-        if (++sA == p.a_stages) { sA = 0; phA ^= 1u; }
-      };
-      for (long long tile = tile0; tile < p.num_tiles; tile += tile_step, ++it) {
-        const TileCoord tc = decode_tile(p, tile, rank);
-        const uint32_t as = p.acc_stages == 2 ? (it & 1u) : 0u, aphase = p.acc_stages == 2 ? ((it >> 1) & 1u) : (it & 1u);
-        mbar_wait(tempty_bar(as), aphase ^ 1u);
-        tc_fence_after();
-        tmem_d = tmem_base + as * kparts * part_cols;
-        ks = 0;
-        uint32_t accum = 0;
-        for (int a = 0; a < p.kt; ++a) {
-          int tv;
-          bool from_cache;
-          if (!tap_time(p, tc, a, tv, from_cache)) continue;
-          if (halo) {
-            for (int kc = 0; kc < num_kc; ++kc) {
-              mbar_wait(fullA_bar(sA), phA);
-              for (int bb = 0; bb < p.kh; ++bb)
-                for (int c = 0; c < p.kw; ++c) {
-                  kstep(window_lo(bb * p.hP + c), accum, false);
-                  accum = 1;
-                }
-              release_window();
-            }
-          } else {
-            for (int s = nsp * num_kc; s > 0; --s) {
-              kstep(stage_a_lo(), accum, false);
-              accum = 1;
-            }
-          }
-        }
-        for (int g = 0; g < res_steps; ++g) {
-          if (halo) {
-            mbar_wait(fullA_bar(sA), phA);
-            kstep(window_lo(p.ph * p.hP + p.pw), 1u, true);
-            release_window();
-          } else {
-            kstep(stage_a_lo(), 1u, true);
-          }
-        }
-        if (el) { if constexpr (kPair) umma_commit_2sm(tfull_bar(as)); else umma_commit(tfull_bar(as)); }
+    for (uint32_t j = 0; j < 4u; ++j) {
+      const uint64_t ah = desc(al + 2u * j, hi_a), bh = desc(bl + 2u * j, hi_b);
+      wgmma_k16<BN, kSplit>(acc, ah, bh, j == 0 ? scale : 1u);
+      if constexpr (kSplit) {
+        wgmma_k16<BN, kSplit>(acc, desc(al + (a_pl >> 4) + 2u * j, hi_a), bh, 1u);
+        if (!res) wgmma_k16<BN, kSplit>(acc, ah, desc(bl + (b_bytes >> 4) + 2u * j, hi_b), 1u);
       }
     }
-  } else if (warp >= kEpiWarp0) {
-    // ===================== epilogue =====================
-    // Two groups of four warps (one warp per TMEM lane quarter).  MT == 2: group g owns the rows of M tile g;
-    // MT == 1: the groups alternate 64-channel slices of the same 128 rows.  A thread owns one output row and at most
-    // 128 of its channels.  Every WARP stages its 32 rows x 64 channels in its own swizzled buffer and issues its own TMA
-    // store (no block-level barrier on the store path); LayerNorm keeps the bf16-packed row in registers between the
-    // statistics pass and the normalisation pass, so the accumulator is read once and released before the second pass.
-    const int q = warp & 3;            // TMEM lane quarter this warp may read
-    const int grp = (warp - kEpiWarp0) >> 2;   // 0 / 1
-    const int et = threadIdx.x - kEpiWarp0 * 32;
-    const int nchunks = p.BN / 32;
-    const int mt = (p.MT == 2) ? grp : 0;
-    const int sb = (p.MT == 2) ? 0 : grp;      // first 64-channel slice
-    const int ss = (p.MT == 2) ? 1 : 2;        // slice step
-    const int rr = q * 32 + lane;              // row inside the M tile
-    const uint32_t stg_bytes = (uint32_t)p.stg_bufs * 4096u;
-    const uint32_t wstg = smem_base + p.stage_off + (uint32_t)(warp - kEpiWarp0) * stg_bytes;
-    uint8_t* wstg_gen = smem_gen + p.stage_off + (uint32_t)(warp - kEpiWarp0) * stg_bytes;
-    const int swz = lane & 7;
-    uint32_t nstore = 0;                       // TMA stores issued by this warp (selects the staging buffer)
-    // origin of this warp's 32 rows inside the CTA tile (the store box is {64, qw, qh, qt})
-    int qw0, qh0, qt0;
-    if (p.halo) { qw0 = 8 * mt; qh0 = 4 * q; qt0 = 0; }
-    else { const int row0 = mt * 128 + q * 32; qw0 = row0 % p.BW; qh0 = (row0 / p.BW) % p.BH; qt0 = row0 / (p.BW * p.BH); }
-    const bool res_direct = (p.res_mode == 1 && !p.res_mma);
-    const bool store_a = (p.ln_mode != 1);
-    const float inv_n = 1.0f / (float)p.BN;
-    uint32_t it = 0;
-    int last_n0 = -1;
-    uint32_t cbuf = 1;                         // bias / gamma / beta buffer in use (toggled whenever n0 changes)
-    for (long long tile = tile0; tile < p.num_tiles; tile += tile_step, ++it) {
-      const TileCoord tc = decode_tile(p, tile, rank);
-      const uint32_t as = p.acc_stages == 2 ? (it & 1u) : 0u, aphase = p.acc_stages == 2 ? ((it >> 1) & 1u) : (it & 1u);
-      if (tc.n0 != last_n0) {
-        // all epilogue warps walk the same tile sequence, so this branch is uniform across them; a warp can only be one
-        // barrier behind, which is why two buffers are enough
-        last_n0 = tc.n0;
-        cbuf ^= 1u;
-        float* b_ = sbias + cbuf * 768;
-        for (int i = et; i < p.BN; i += kEpiWarps * 32) {
-          b_[i] = (p.bias && tc.n0 + i < p.Co_real) ? p.bias[tc.n0 + i] : 0.f;
-          // with SiLU the normalisation produces y/2 directly (silu(y) = h + h*tanh(h), h = y/2)
-          if (p.ln_mode) { const float sc = (p.ln_silu && !kSplit) ? 0.5f : 1.0f; b_[256 + i] = sc * p.ln_gamma[tc.n0 + i]; b_[512 + i] = sc * p.ln_beta[tc.n0 + i]; }
-        }
-        asm volatile("bar.sync 1, %0;" ::"n"(kEpiWarps * 32) : "memory");
-      }
-      const float* bias_s = sbias + cbuf * 768;
-      const float* gamma_s = bias_s + 256;
-      const float* beta_s = bias_s + 512;
+    wgmma_commit();
+    wgmma_wait<1>();
+    release();
+    pend_stage = stage;
+    pend_win = last_of_window;
+    if (++stage == nstages) { stage = 0; phase ^= 1u; }
+  };
 
-      const int row = mt * 128 + rr;
-      // halo mode: M tile mt covers columns [8 mt, 8 mt + 8) of the 16-row CTA tile
-      const int dw = p.halo ? 8 * mt + (rr & 7) : row % p.BW;
-      const int dh = p.halo ? (rr >> 3) : (row / p.BW) % p.BH;
-      const int dt = p.halo ? 0 : row / (p.BW * p.BH);
-      const int t = tc.t0 + dt, h = tc.h0 + dh, w = tc.w0 + dw;
-      const bool valid = (t < p.To) && (h < p.Ho) && (w < p.Wo);
-      const long long ooff = (long long)tc.b * p.osB + (long long)t * p.osT + (long long)h * p.osH + (long long)w * p.osW;
-      const bf16* r0 = nullptr;
-      const bf16* r1 = nullptr;
-      const bf16* r2 = nullptr;
-      if (valid && res_direct) {
-        r0 = p.res + (long long)tc.b * p.rsB + (long long)t * p.rsT + (long long)h * p.rsH + (long long)w * p.rsW + tc.n0;
-      } else if (valid && p.res_mode == 3) {
+  const int rbase = 64 * g + 16 * wq + (lane >> 2);   // this thread's rows: rbase and rbase + 8
+  const int cq = 2 * (lane & 3);                      // and columns 8j + cq, 8j + cq + 1
+  const bool res_direct = (p.res_mode == 1 && !p.res_mma);
+  const bool store_a = (p.ln_mode != 1);
+  const float inv_n = 1.0f / (float)BN;
+  int last_n0 = -1;
+  uint32_t cbuf = 1;                         // bias / gamma / beta buffer in use (toggled whenever n0 changes)
+
+  for (long long tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+    const TileCoord tc = decode_tile(p, tile);
+    // ---- main loop
+    uint32_t G = 0xFFFFFFFFu;                // K steps per group (kparts)
+    if constexpr (kSum) {
+      if (p.kparts > 1) {
+        uint32_t nk = 0;
+        for (int a = 0; a < p.kt; ++a) {
+          int tv_;
+          bool fc_;
+          if (tap_time(p, tc, a, tv_, fc_)) nk += (uint32_t)(nsp * num_kc);
+        }
+        nk += (uint32_t)res_steps;
+        G = (nk + (uint32_t)p.kparts - 1u) / (uint32_t)p.kparts;
+      }
+#pragma unroll
+      for (int i = 0; i < R; ++i) sum[i] = 0.f;
+    }
+    uint32_t ks = 0, accum = 0;
+    auto step = [&](bool a_from_stage, uint32_t a_addr, bool res, bool last_of_window) {
+      if constexpr (kSum) {
+        if (ks > 0 && ks % G == 0) {
+          wgmma_wait<0>();
+          acc_fence(acc);
+          release();
+#pragma unroll
+          for (int i = 0; i < R; ++i) sum[i] += acc[i];
+          accum = 0;
+        }
+      }
+      kstep(a_from_stage, a_addr, accum, res, last_of_window);
+      accum = 1;
+      ++ks;
+    };
+    for (int a = 0; a < p.kt; ++a) {
+      int tv;
+      bool from_cache;
+      if (!tap_time(p, tc, a, tv, from_cache)) continue;
+      if (halo) {
+        for (int kc = 0; kc < num_kc; ++kc) {
+          mbar_wait(fullA_bar(sA), phA);
+          const uint32_t win = smem_base + (uint32_t)sA * win_bytes + a_row_off;
+          for (int bb = 0; bb < p.kh; ++bb)
+            for (int c = 0; c < p.kw; ++c)
+              step(false, win + (uint32_t)(bb * p.hP + c) * 128u, false, bb == p.kh - 1 && c == p.kw - 1);
+          if (++sA == p.a_stages) { sA = 0; phA ^= 1u; }
+        }
+      } else {
+        for (int s = nsp * num_kc; s > 0; --s) step(true, 0u, false, false);
+      }
+    }
+    for (int gr = 0; gr < res_steps; ++gr) {
+      if (halo) {
+        mbar_wait(fullA_bar(sA), phA);
+        step(false, smem_base + (uint32_t)sA * win_bytes + a_row_off + (uint32_t)(p.ph * p.hP + p.pw) * 128u, true, true);
+        if (++sA == p.a_stages) { sA = 0; phA ^= 1u; }
+      } else {
+        step(true, 0u, true, false);
+      }
+    }
+    wgmma_wait<0>();
+    acc_fence(acc);
+    release();
+    if constexpr (kSum) {
+#pragma unroll
+      for (int i = 0; i < R; ++i) acc[i] += sum[i];
+    }
+
+    // ---- epilogue
+    if (tc.n0 != last_n0) {
+      // all consumer warps walk the same tile sequence, so this branch is uniform across them; a warp can only be one
+      // barrier behind, which is why two buffers are enough
+      last_n0 = tc.n0;
+      cbuf ^= 1u;
+      float* b_ = sbias + cbuf * 768;
+      for (int i = threadIdx.x; i < BN; i += kConsumerWarps * 32) {
+        b_[i] = (p.bias && tc.n0 + i < p.Co_real) ? p.bias[tc.n0 + i] : 0.f;
+        // with SiLU the bf16 normalisation produces y/2 directly (silu(y) = h + h*tanh(h), h = y/2)
+        if (p.ln_mode) { const float sc = (p.ln_silu && !kSplit) ? 0.5f : 1.0f; b_[256 + i] = sc * p.ln_gamma[tc.n0 + i]; b_[512 + i] = sc * p.ln_beta[tc.n0 + i]; }
+      }
+      asm volatile("bar.sync 1, %0;" ::"n"(kConsumerWarps * 32) : "memory");
+    }
+    const float* bias_s = sbias + cbuf * 768;
+    const float* gamma_s = bias_s + 256;
+    const float* beta_s = bias_s + 512;
+
+    // geometry of this thread's two rows
+    bool valid[2];
+    long long ooff[2];
+    const bf16* r0[2];
+    const bf16* r1[2];
+    const bf16* r2[2];
+    auto row_geom = [&](int row, int& t, int& h, int& w) {
+      const int dw = halo ? (row & 7) : row % p.BW;
+      const int dh = halo ? (row >> 3) : (row / p.BW) % p.BH;
+      const int dt = halo ? 0 : row / (p.BW * p.BH);
+      t = tc.t0 + dt; h = tc.h0 + dh; w = tc.w0 + dw;
+      return (t < p.To) && (h < p.Ho) && (w < p.Wo);
+    };
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      int t, h, w;
+      valid[r] = row_geom(rbase + 8 * r, t, h, w);
+      ooff[r] = (long long)tc.b * p.osB + (long long)t * p.osT + (long long)h * p.osH + (long long)w * p.osW;
+      r0[r] = r1[r] = r2[r] = nullptr;
+      if (valid[r] && res_direct) {
+        r0[r] = p.res + (long long)tc.b * p.rsB + (long long)t * p.rsT + (long long)h * p.rsH + (long long)w * p.rsW + tc.n0;
+      } else if (valid[r] && p.res_mode == 3) {
         // avg-pool of residual frames 2t-1, 2t, 2t+1 (front pad: zero / frame 0 / 1-frame cache)
         const long long sp = (long long)tc.b * p.rsB + (long long)h * p.rsH + (long long)w * p.rsW + tc.n0;
         const int ta = 2 * t - 1 + p.res_pool_off, tb = ta + 1, tcn = ta + 2;
-        if (ta >= 0) r0 = p.res + sp + (long long)ta * p.rsT;
-        else if (p.res_t_mode == 1) r0 = p.res + sp;
-        else if (p.res_t_mode == 2) r0 = p.res_cache + (((long long)tc.b * p.Ho + h) * p.Wo + w) * (long long)p.Co * (kSplit ? 2 : 1) + tc.n0;
-        if (tb < p.resT) r1 = p.res + sp + (long long)tb * p.rsT;
-        if (tcn < p.resT) r2 = p.res + sp + (long long)tcn * p.rsT;
+        if (ta >= 0) r0[r] = p.res + sp + (long long)ta * p.rsT;
+        else if (p.res_t_mode == 1) r0[r] = p.res + sp;
+        else if (p.res_t_mode == 2) r0[r] = p.res_cache + (((long long)tc.b * p.Ho + h) * p.Wo + w) * (long long)p.Co * (kSplit ? 2 : 1) + tc.n0;
+        if (tb < p.resT) r1[r] = p.res + sp + (long long)tb * p.rsT;
+        if (tcn < p.resT) r2[r] = p.res + sp + (long long)tcn * p.rsT;
       }
-      // this lane's row in the next staging buffer, once the TMA store that last used the buffer has read it
-      auto stage_row = [&]() -> uint8_t* {
-        const uint32_t b = (p.stg_bufs == 2) ? (nstore & 1u) : 0u;
-        if (lane == 0) { if (p.stg_bufs == 2) tma_store_wait_read1(); else tma_store_wait_read(); }
-        __syncwarp();
-        return wstg_gen + b * 4096u + (uint32_t)lane * 128u;
-      };
-      auto store_rows = [&](const CUtensorMap* m, int c0) {
-        fence_async_smem();
-        __syncwarp();
-        if (lane == 0) {
-          const uint32_t b = (p.stg_bufs == 2) ? (nstore & 1u) : 0u;
-          if (p.store_stream) tma_store_5d_stream(m, wstg + b * 4096u, c0, tc.w0 + qw0, tc.h0 + qh0, tc.t0 + qt0, tc.b);
-          else tma_store_5d(m, wstg + b * 4096u, c0, tc.w0 + qw0, tc.h0 + qh0, tc.t0 + qt0, tc.b);
-          tma_store_commit();
-        }
-        ++nstore;
-      };
-      // packed bf16 words of 64 channels -> staging row (TMA store) or global memory
-      // (coff: channel offset of the plane being written: 0, or Cout for the lo plane of a split tensor)
-      auto put64 = [&](const uint32_t* pk, int ncol, const CUtensorMap* m, bf16* grow, int j, int coff = 0) {
-        if (p.tma_store) {
-          uint8_t* my = stage_row();
-#pragma unroll
-          for (int g = 0; g < 8; ++g)
-            *reinterpret_cast<uint4*>(my + ((g ^ swz) << 4)) = make_uint4(pk[4 * g], pk[4 * g + 1], pk[4 * g + 2], pk[4 * g + 3]);
-          store_rows(m, coff + tc.n0 + j);
-        } else if (valid) {
-#pragma unroll
-          for (int g = 0; g < 8; ++g)
-            if (g * 8 < ncol) *reinterpret_cast<uint4*>(grow + coff + j + g * 8) = make_uint4(pk[4 * g], pk[4 * g + 1], pk[4 * g + 2], pk[4 * g + 3]);
-        }
-      };
-
-      // regularizer on the complete fp32 row f[0..31] of this thread's position (heads with Cout <= 32: one 32-column
-      // chunk, tile n0 == 0).  Called by all 32 lanes (the KL partial sums are reduced across the warp).
-      auto regularize_row = [&](const float (&f)[32]) {
-        const long long plane = p.osC;                                  // T*H*W of the [B,C,T,H,W] tensors
-        const long long pos = ooff - (long long)tc.b * p.osB;
-        if (p.reg_mode == 1) {
-          float part = 0.f;
-          // z_channels is a compile-time constant inside each case: f[] stays in registers (no dynamic indexing)
-          auto kl_row = [&](auto ZC) {
-            constexpr int zc = decltype(ZC)::value;
-            const long long zb = (long long)tc.b * zc * plane + pos;
-#pragma unroll
-            for (int c = 0; c < zc; ++c) {
-              float zv;
-              part += kl_sample_one(f[c], f[zc + c], p.reg_sample ? p.reg_noise[zb + c * plane] : 0.f, p.reg_sample, zv);
-              p.reg_z[zb + c * plane] = zv;
-            }
-          };
-          if (valid) {
-            if (p.reg_zc == 4) kl_row(std::integral_constant<int, 4>());
-            else if (p.reg_zc == 8) kl_row(std::integral_constant<int, 8>());
-            else kl_row(std::integral_constant<int, 16>());
-          }
-          double dsum = (double)part;
-#pragma unroll
-          for (int o = 16; o > 0; o >>= 1) dsum += __shfl_xor_sync(0xffffffffu, dsum, o);
-          if (lane == 0) atomicAdd(p.reg_kl, dsum);
-        } else if (valid) {
-          const long long zb = (long long)tc.b * p.reg_zc * plane + pos;
-          float idx = 0.f;
-#pragma unroll
-          for (int c = 0; c < VT_MAX_FSQ; ++c)
-            if (c < p.reg_zc) p.reg_z[zb + c * plane] = fsq_code(p.reg_fsq, c, f[c], idx);
-          if (p.reg_idx) p.reg_idx[(long long)tc.b * plane + pos] = (int)idx;
-        }
-      };
-      mbar_wait(tfull_bar(as), aphase);
-      tc_fence_after();
-      const uint32_t eparts = kSplit ? (uint32_t)p.kparts : 1u;
-      const uint32_t tbase = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)((as * eparts * p.MT + mt) * p.BN);
+    }
+    // residual value of channel pair (c, c + 1) of a row: bf16 pair, or hi + lo fp16 pairs (split)
+    auto res_pair = [&](const bf16* rp, int c, float& x0, float& x1) {
+      const uint32_t hw = *reinterpret_cast<const uint32_t*>(rp + c);
       if constexpr (kSplit) {
-        // partial accumulators in use for this tile: min(kparts, K steps of the tile) (causally skipped taps shorten the loop)
-        uint32_t nparts = 1;
-        if (eparts > 1) {
-          uint32_t nk = 0;
-          for (int a = 0; a < p.kt; ++a) {
-            int tv_;
-            bool fc_;
-            if (tap_time(p, tc, a, tv_, fc_)) nk += (uint32_t)(p.kh * p.kw * p.num_kc);
-          }
-          nparts = nk < eparts ? nk : eparts;
-        }
-        const uint32_t part_stride = (uint32_t)(p.MT * p.BN);
-        // ---- EXACT_TC epilogue: fp32 values straight from the accumulator (re-read per pass: the main loop is three
-        // times as long as in bf16 mode, the epilogue has the time), two-pass LayerNorm statistics, full-precision
-        // SiLU, results written as hi | lo fp16 planes.
-        const bf16* rl0 = r0 ? r0 + p.o_lo : nullptr;   // lo planes of the residual rows
-        const bf16* rl1 = r1 ? r1 + p.o_lo : nullptr;
-        const bf16* rl2 = r2 ? r2 + p.o_lo : nullptr;
-        auto add_row = [&](const bf16* rh, const bf16* rl, int jj, float sc, float (&f)[32]) {
-#pragma unroll
-          for (int g = 0; g < 4; ++g) {
-            float a[8], b[8];
-            unpack8h(*reinterpret_cast<const uint4*>(rh + jj + g * 8), a);
-            unpack8h(*reinterpret_cast<const uint4*>(rl + jj + g * 8), b);
-#pragma unroll
-            for (int e = 0; e < 8; ++e) f[g * 8 + e] = fmaf(sc, a[e] + b[e], f[g * 8 + e]);
-          }
-        };
-        // v = rb * (acc + bias) + ra * R for the 32 channels [jj, jj + 32) of this thread's row
-        // `finished` (later passes of a LayerNorm epilogue): the row was parked in the accumulator by the first pass
-        auto chunk = [&](int jj, float (&f)[32], bool finished, bool park) {
-          uint32_t v[32];
-          tmem_ld32(tbase + (uint32_t)jj, v);
-          tmem_ld_wait();
-          if (finished) {
-#pragma unroll
-            for (int e = 0; e < 32; ++e) f[e] = __uint_as_float(v[e]);
-            return;
-          }
-          if (nparts > 1) {   // fp32 (round-to-nearest) sum of the partial accumulators
-#pragma unroll 1
-            for (uint32_t pi = 1; pi < nparts; ++pi) {
-              uint32_t u[32];
-              tmem_ld32(tbase + pi * part_stride + (uint32_t)jj, u);
-              tmem_ld_wait();
-#pragma unroll
-              for (int e = 0; e < 32; ++e) v[e] = __float_as_uint(__uint_as_float(v[e]) + __uint_as_float(u[e]));
-            }
-          }
-          // (the split weights carry a power-of-two scale: undo it on the accumulator, exactly, before the bias)
-#pragma unroll
-          for (int e = 0; e < 32; ++e) f[e] = fmaf(__uint_as_float(v[e]), p.acc_scale, bias_s[jj + e]);
-          if (p.rb != 1.0f) {
-#pragma unroll
-            for (int e = 0; e < 32; ++e) f[e] *= p.rb;
-          }
-          if (valid && res_direct) {
-            add_row(r0, rl0, jj, p.ra, f);
-          } else if (valid && p.res_mode == 3) {
-            float acc3[32];
-#pragma unroll
-            for (int e = 0; e < 32; ++e) acc3[e] = 0.f;
-            if (r0) add_row(r0, rl0, jj, 1.0f, acc3);
-            if (r1) add_row(r1, rl1, jj, 1.0f, acc3);
-            if (r2) add_row(r2, rl2, jj, 1.0f, acc3);
-            const float s3 = p.ra * (1.0f / 3.0f);
-#pragma unroll
-            for (int e = 0; e < 32; ++e) f[e] = fmaf(s3, acc3[e], f[e]);
-          }
-          if (park) {   // partial sums, bias and residual (global loads) are paid once per row, not once per pass
-#pragma unroll
-            for (int e = 0; e < 32; ++e) v[e] = __float_as_uint(f[e]);
-            tmem_st32(tbase + (uint32_t)jj, v);
-            tmem_st_wait();
-          }
-        };
-        // sum over this thread's channels of g(v); completed across the two groups when they share a row (MT == 1)
-        float mean = 0.f, rstd = 0.f;
-        if (p.ln_mode) {
-          float* st_ = stat_s + (it & 1u) * 512u;
-          float part = 0.f;
-#pragma unroll 1
-          for (int i = 0; i < 2; ++i) {
-            const int sl = sb + i * ss;
-            if (sl * 2 >= nchunks) break;
-            const int ncol = (sl * 2 + 1 < nchunks) ? 64 : 32;
-#pragma unroll 1
-            for (int hc = 0; hc * 32 < ncol; ++hc) {
-              float f[32];
-              chunk(sl * 64 + hc * 32, f, false, true);
-#pragma unroll
-              for (int e = 0; e < 32; ++e) part += f[e];
-            }
-          }
-          if (p.MT == 1) {
-            st_[(grp * 128 + rr) << 1] = part;
-            asm volatile("bar.sync 2, %0;" ::"n"(kEpiWarps * 32) : "memory");
-            part += st_[((grp ^ 1) * 128 + rr) << 1];
-          }
-          mean = part * inv_n;
-          part = 0.f;
-#pragma unroll 1
-          for (int i = 0; i < 2; ++i) {
-            const int sl = sb + i * ss;
-            if (sl * 2 >= nchunks) break;
-            const int ncol = (sl * 2 + 1 < nchunks) ? 64 : 32;
-#pragma unroll 1
-            for (int hc = 0; hc * 32 < ncol; ++hc) {
-              float f[32];
-              chunk(sl * 64 + hc * 32, f, true, false);
-#pragma unroll
-              for (int e = 0; e < 32; ++e) { const float d = f[e] - mean; part = fmaf(d, d, part); }
-            }
-          }
-          if (p.MT == 1) {
-            st_[((grp * 128 + rr) << 1) + 1] = part;
-            asm volatile("bar.sync 2, %0;" ::"n"(kEpiWarps * 32) : "memory");
-            part += st_[(((grp ^ 1) * 128 + rr) << 1) + 1];
-          }
-          rstd = 1.0f / sqrtf(part * inv_n + 1e-6f);
-        }
-        auto emit = [&](bool normalized, void* optr, const CUtensorMap* m) {
-          bf16* grow = reinterpret_cast<bf16*>(optr) + ooff + tc.n0;
-#pragma unroll 1
-          for (int i = 0; i < 2; ++i) {
-            const int sl = sb + i * ss;
-            if (sl * 2 >= nchunks) break;
-            const int j = sl * 64;
-            const int ncol = (sl * 2 + 1 < nchunks) ? 64 : 32;
-            uint32_t hw[32], lw[32];
-#pragma unroll
-            for (int hc = 0; hc < 2; ++hc) {
-              if (hc * 32 >= ncol) break;
-              const int jj = j + hc * 32;
-              float f[32];
-              chunk(jj, f, p.ln_mode != 0, false);
-              if (normalized) {
-#pragma unroll
-                for (int e = 0; e < 32; ++e) {
-                  float y = (f[e] - mean) * rstd * gamma_s[jj + e] + beta_s[jj + e];
-                  if (p.ln_silu) y = silu_tc(y);
-                  f[e] = y;
-                }
-              }
-              if (p.out_f32) {
-                // external fp32 heads / attention scores: direct stores, only the real output channels
-                if (p.reg_mode) regularize_row(f);
-                if (valid && optr) {
-                  float* of = reinterpret_cast<float*>(optr) + ooff;
-                  if (p.osC == 1 && tc.n0 + jj + 32 <= p.Co_real) {
-#pragma unroll
-                    for (int g = 0; g < 8; ++g)
-                      *reinterpret_cast<float4*>(of + tc.n0 + jj + g * 4) = make_float4(f[g * 4], f[g * 4 + 1], f[g * 4 + 2], f[g * 4 + 3]);
-                  } else {
-#pragma unroll
-                    for (int e = 0; e < 32; ++e)
-                      if (tc.n0 + jj + e < p.Co_real) of[(long long)(tc.n0 + jj + e) * p.osC] = f[e];
-                  }
-                }
-              } else {
-#pragma unroll
-                for (int e = 0; e < 16; ++e) {
-                  const uint32_t h2 = pack_f16x2(f[2 * e], f[2 * e + 1]);
-                  hw[hc * 16 + e] = h2;
-                  lw[hc * 16 + e] = pack_f16x2(f[2 * e] - f16_lo(h2), f[2 * e + 1] - f16_hi(h2));
-                }
-              }
-            }
-            if (!p.out_f32) {
-              put64(hw, ncol, m, grow, j, 0);
-              put64(lw, ncol, m, grow, j, p.o_lo);
-            }
-          }
-        };
-        if (store_a) emit(false, p.out, &maps.o);
-        if (p.ln_mode) emit(true, p.ln_mode == 1 ? p.out : p.out2, p.ln_mode == 1 ? &maps.o : &maps.o2);
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) {
-          if constexpr (kPair) mbar_arrive_remote(tempty_bar(as), 0); else mbar_arrive(tempty_bar(as));
-        }
+        const uint32_t lw = *reinterpret_cast<const uint32_t*>(rp + p.o_lo + c);
+        x0 = f16_lo(hw) + f16_lo(lw);
+        x1 = f16_hi(hw) + f16_hi(lw);
       } else {
-      uint64_t lsum2 = 0ull, lsq2 = 0ull;      // (even, odd) column partial sums
-      uint32_t keep[64];                       // bf16 pairs of this thread's (up to) 128 channels
-      // ---- pass A: v = rb*(acc+bias) + ra*R ; stored unless the LayerNorm replaces it; statistics for the LayerNorm
-#pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        const int sl = sb + i * ss;
-        if (sl * 2 >= nchunks) break;
-        const int j = sl * 64;
-        const int ncol = (sl * 2 + 1 < nchunks) ? 64 : 32;
-#pragma unroll
-        for (int hc = 0; hc < 2; ++hc) {
-          if (hc * 32 >= ncol) break;
-          uint32_t v[32];
-          tmem_ld32(tbase + (uint32_t)(j + hc * 32), v);
-          tmem_ld_wait();
-          float f[32];
-#pragma unroll
-          for (int g = 0; g < 8; ++g) {
-            const ulonglong2 bv = *reinterpret_cast<const ulonglong2*>(bias_s + j + hc * 32 + g * 4);
-            uint64_t a0 = add2(pk2(__uint_as_float(v[g * 4 + 0]), __uint_as_float(v[g * 4 + 1])), bv.x);
-            uint64_t a1 = add2(pk2(__uint_as_float(v[g * 4 + 2]), __uint_as_float(v[g * 4 + 3])), bv.y);
-            if (p.rb != 1.0f) { const uint64_t rb2 = pk2(p.rb, p.rb); a0 = mul2(a0, rb2); a1 = mul2(a1, rb2); }
-            upk2(a0, f[g * 4 + 0], f[g * 4 + 1]);
-            upk2(a1, f[g * 4 + 2], f[g * 4 + 3]);
-          }
-          const int jj = j + hc * 32;
-          if (valid && res_direct) {
-#pragma unroll
-            for (int g = 0; g < 4; ++g) {
-              float rv[8];
-              unpack8(*reinterpret_cast<const uint4*>(r0 + jj + g * 8), rv);
-#pragma unroll
-              for (int e = 0; e < 8; ++e) f[g * 8 + e] = fmaf(p.ra, rv[e], f[g * 8 + e]);
-            }
-          } else if (valid && p.res_mode == 3) {
-            const float s3 = p.ra * (1.0f / 3.0f);
-#pragma unroll
-            for (int g = 0; g < 4; ++g) {
-              float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-              float rv[8];
-              if (r0) { unpack8(*reinterpret_cast<const uint4*>(r0 + jj + g * 8), rv);
-#pragma unroll
-                for (int e = 0; e < 8; ++e) acc[e] += rv[e]; }
-              if (r1) { unpack8(*reinterpret_cast<const uint4*>(r1 + jj + g * 8), rv);
-#pragma unroll
-                for (int e = 0; e < 8; ++e) acc[e] += rv[e]; }
-              if (r2) { unpack8(*reinterpret_cast<const uint4*>(r2 + jj + g * 8), rv);
-#pragma unroll
-                for (int e = 0; e < 8; ++e) acc[e] += rv[e]; }
-#pragma unroll
-              for (int e = 0; e < 8; ++e) f[g * 8 + e] = fmaf(s3, acc[e], f[g * 8 + e]);
-            }
-          }
-          if (p.out_f32) {
-            // external fp32 heads (never fused with LayerNorm): direct stores, only the real output channels
-            if (p.reg_mode) regularize_row(f);
-            if (valid && p.out) {
-              float* of = reinterpret_cast<float*>(p.out) + ooff;
-              if (p.osC == 1 && tc.n0 + jj + 32 <= p.Co_real) {
-#pragma unroll
-                for (int g = 0; g < 8; ++g)
-                  *reinterpret_cast<float4*>(of + tc.n0 + jj + g * 4) = make_float4(f[g * 4], f[g * 4 + 1], f[g * 4 + 2], f[g * 4 + 3]);
-              } else {
-#pragma unroll
-                for (int e = 0; e < 32; ++e)
-                  if (tc.n0 + jj + e < p.Co_real) of[(long long)(tc.n0 + jj + e) * p.osC] = f[e];
-              }
-            }
-          } else {
-            if (p.ln_mode) {
-#pragma unroll
-              for (int e = 0; e < 16; ++e) {
-                const uint64_t f2 = pk2(f[2 * e], f[2 * e + 1]);
-                lsum2 = add2(lsum2, f2);
-                lsq2 = fma2(f2, f2, lsq2);
-              }
-            }
-#pragma unroll
-            for (int e = 0; e < 16; ++e) keep[i * 32 + hc * 16 + e] = pack_bf16x2(f[2 * e], f[2 * e + 1]);
-          }
-        }
-        if (!p.out_f32 && store_a) put64(&keep[i * 32], ncol, &maps.o, reinterpret_cast<bf16*>(p.out) + ooff + tc.n0, j);
+        x0 = bf16_lo(hw);
+        x1 = bf16_hi(hw);
       }
-      // the accumulator has been read: hand the TMEM stage back to the MMA issuer before the second pass
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if constexpr (kPair) mbar_arrive_remote(tempty_bar(as), 0); else mbar_arrive(tempty_bar(as));
+    };
+    // v = rb * (acc + bias) + ra * R, in place
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int c = 8 * j + cq;
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        float f = kSplit ? fmaf(acc[4 * j + e], p.acc_scale, bias_s[c + (e & 1)]) : acc[4 * j + e] + bias_s[c + (e & 1)];
+        if (p.rb != 1.0f) f *= p.rb;
+        acc[4 * j + e] = f;
+      }
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        if (!valid[r]) continue;
+        if (res_direct) {
+          float x0, x1;
+          res_pair(r0[r], c, x0, x1);
+          acc[4 * j + 2 * r] = fmaf(p.ra, x0, acc[4 * j + 2 * r]);
+          acc[4 * j + 2 * r + 1] = fmaf(p.ra, x1, acc[4 * j + 2 * r + 1]);
+        } else if (p.res_mode == 3) {
+          float s0 = 0.f, s1 = 0.f, x0, x1;
+          if (r0[r]) { res_pair(r0[r], c, x0, x1); s0 += x0; s1 += x1; }
+          if (r1[r]) { res_pair(r1[r], c, x0, x1); s0 += x0; s1 += x1; }
+          if (r2[r]) { res_pair(r2[r], c, x0, x1); s0 += x0; s1 += x1; }
+          const float s3 = p.ra * (1.0f / 3.0f);
+          acc[4 * j + 2 * r] = fmaf(s3, s0, acc[4 * j + 2 * r]);
+          acc[4 * j + 2 * r + 1] = fmaf(s3, s1, acc[4 * j + 2 * r + 1]);
+        }
+      }
+    }
+
+    if (p.out_f32) {
+      // external fp32 heads / attention scores: direct stores, only the real output channels
+      if (p.out) {
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          if (!valid[r]) continue;
+          float* of = reinterpret_cast<float*>(p.out) + ooff[r];
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int n = tc.n0 + 8 * j + cq + e;
+              if (n < p.Co_real) of[(long long)n * p.osC] = acc[4 * j + 2 * r + e];
+            }
+        }
+      }
+      if (p.reg_mode) {
+        // regularizer on the complete fp32 row of a position (heads with Cout <= 32: BN == 32, n0 == 0): the rows are
+        // gathered in shared memory, thread i < 128 then owns row i with all of its channels
+        if constexpr (BN == 32) {
+#pragma unroll
+          for (int j = 0; j < 4; ++j)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) rowbuf[(rbase + 8 * (e >> 1)) * 33 + 8 * j + cq + (e & 1)] = acc[4 * j + e];
+          asm volatile("bar.sync 2, %0;" ::"n"(kConsumerWarps * 32) : "memory");
+          if (threadIdx.x < 128) {
+            const int row = threadIdx.x;
+            float f[32];
+#pragma unroll
+            for (int c = 0; c < 32; ++c) f[c] = rowbuf[row * 33 + c];
+            int t, h, w;
+            const bool ok = row_geom(row, t, h, w);
+            const long long plane = p.osC;                                  // T*H*W of the [B,C,T,H,W] tensors
+            const long long pos = (long long)t * p.osT + (long long)h * p.osH + (long long)w * p.osW;
+            if (p.reg_mode == 1) {
+              float part = 0.f;
+              // z_channels is a compile-time constant inside each case: f[] stays in registers (no dynamic indexing)
+              auto kl_row = [&](auto ZC) {
+                constexpr int zc = decltype(ZC)::value;
+                const long long zb = (long long)tc.b * zc * plane + pos;
+#pragma unroll
+                for (int c = 0; c < zc; ++c) {
+                  float zv;
+                  part += kl_sample_one(f[c], f[zc + c], p.reg_sample ? p.reg_noise[zb + c * plane] : 0.f, p.reg_sample, zv);
+                  p.reg_z[zb + c * plane] = zv;
+                }
+              };
+              if (ok) {
+                if (p.reg_zc == 4) kl_row(std::integral_constant<int, 4>());
+                else if (p.reg_zc == 8) kl_row(std::integral_constant<int, 8>());
+                else kl_row(std::integral_constant<int, 16>());
+              }
+              double dsum = (double)part;
+#pragma unroll
+              for (int o = 16; o > 0; o >>= 1) dsum += __shfl_xor_sync(0xffffffffu, dsum, o);
+              if (lane == 0) atomicAdd(p.reg_kl, dsum);
+            } else if (ok) {
+              const long long zb = (long long)tc.b * p.reg_zc * plane + pos;
+              float idx = 0.f;
+#pragma unroll
+              for (int c = 0; c < VT_MAX_FSQ; ++c)
+                if (c < p.reg_zc) p.reg_z[zb + c * plane] = fsq_code(p.reg_fsq, c, f[c], idx);
+              if (p.reg_idx) p.reg_idx[(long long)tc.b * plane + pos] = (int)idx;
+            }
+          }
+          asm volatile("bar.sync 2, %0;" ::"n"(kConsumerWarps * 32) : "memory");
+        }
+      }
+      continue;
+    }
+
+    // 16-bit outputs: bf16 pairs, or hi | lo fp16 planes (split)
+    auto put = [&](void* optr, int r, int c, float y0, float y1) {
+      bf16* o = reinterpret_cast<bf16*>(optr) + ooff[r] + tc.n0 + c;
+      if constexpr (kSplit) {
+        const uint32_t hw = pack_f16x2(y0, y1);
+        *reinterpret_cast<uint32_t*>(o) = hw;
+        *reinterpret_cast<uint32_t*>(o + p.o_lo) = pack_f16x2(y0 - f16_lo(hw), y1 - f16_hi(hw));
+      } else {
+        *reinterpret_cast<uint32_t*>(o) = pack_bf16x2(y0, y1);
+      }
+    };
+    if constexpr (kSplit) {
+      // EXACT_TC: two-pass LayerNorm statistics on the fp32 values, full-precision SiLU
+      if (store_a) {
+#pragma unroll
+        for (int r = 0; r < 2; ++r)
+          if (valid[r])
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) put(p.out, r, 8 * j + cq, acc[4 * j + 2 * r], acc[4 * j + 2 * r + 1]);
       }
       if (p.ln_mode) {
-        // ---- LayerNorm over the Cout values of this row (model_3dcausal.py:62-80, eps 1e-6), optional SiLU (:26-27).
-        // Statistics come from the fp32 values, the normalised values from their bf16 rounding (what the unfused
-        // conv -> LayerNorm pair reads back from memory).
-        float lsum, lsq;
-        {
-          float a, b;
-          upk2(lsum2, a, b); lsum = a + b;
-          upk2(lsq2, a, b); lsq = a + b;
+        void* nout = p.ln_mode == 1 ? p.out : p.out2;
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          float s = 0.f;
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) s += acc[4 * j + 2 * r] + acc[4 * j + 2 * r + 1];
+          const float mean = quad_sum(s) * inv_n;
+          float q = 0.f;
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            const float d0 = acc[4 * j + 2 * r] - mean, d1 = acc[4 * j + 2 * r + 1] - mean;
+            q = fmaf(d0, d0, q);
+            q = fmaf(d1, d1, q);
+          }
+          const float rstd = 1.0f / sqrtf(quad_sum(q) * inv_n + 1e-6f);
+          if (!valid[r]) continue;
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            const int c = 8 * j + cq;
+            float y0 = (acc[4 * j + 2 * r] - mean) * rstd * gamma_s[c] + beta_s[c];
+            float y1 = (acc[4 * j + 2 * r + 1] - mean) * rstd * gamma_s[c + 1] + beta_s[c + 1];
+            if (p.ln_silu) { y0 = silu_tc(y0); y1 = silu_tc(y1); }
+            put(nout, r, c, y0, y1);
+          }
         }
-        if (p.MT == 1) {  // the other group holds the other slices of the row
-          // double-buffered by tile parity: the partner group reads right after the barrier, this group may already be
-          // writing the next tile's statistics
-          float* st_ = stat_s + (it & 1u) * 512u;
-          float* xs = st_ + ((grp * 128 + rr) << 1);
-          xs[0] = lsum; xs[1] = lsq;
-          asm volatile("bar.sync 2, %0;" ::"n"(kEpiWarps * 32) : "memory");
-          const float* ys = st_ + ((((grp ^ 1) * 128) + rr) << 1);
-          lsum += ys[0]; lsq += ys[1];
+      }
+    } else {
+      // BF16: statistics from the fp32 values, the normalised values from their bf16 rounding (what the unfused
+      // conv -> LayerNorm pair reads back from memory)
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        float s = 0.f, q = 0.f;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const float f0 = acc[4 * j + 2 * r], f1 = acc[4 * j + 2 * r + 1];
+          s += f0 + f1;
+          q = fmaf(f0, f0, q);
+          q = fmaf(f1, f1, q);
+          const uint32_t kp = pack_bf16x2(f0, f1);
+          if (store_a && valid[r]) *reinterpret_cast<uint32_t*>(reinterpret_cast<bf16*>(p.out) + ooff[r] + tc.n0 + 8 * j + cq) = kp;
+          acc[4 * j + 2 * r] = bf16_lo(kp);
+          acc[4 * j + 2 * r + 1] = bf16_hi(kp);
         }
-        const float mean = lsum * inv_n;
-        float var = fmaf(-mean, mean, lsq * inv_n);
+        if (!p.ln_mode) continue;
+        // LayerNorm over the Cout values of this row (model_3dcausal.py:62-80, eps 1e-6), optional SiLU (:26-27)
+        const float mean = quad_sum(s) * inv_n;
+        float var = fmaf(-mean, mean, quad_sum(q) * inv_n);
         var = var < 0.f ? 0.f : var;
         const float rstd = rsqrtf(var + 1e-6f);
         const float nmr = -mean * rstd;
-        const uint64_t rstd2 = pk2(rstd, rstd), nmr2 = pk2(nmr, nmr);
-        bf16* nrow = reinterpret_cast<bf16*>(p.ln_mode == 1 ? p.out : p.out2) + ooff + tc.n0;
-        const CUtensorMap* nmap = (p.ln_mode == 1) ? &maps.o : &maps.o2;
+        if (!valid[r]) continue;
+        void* nout = p.ln_mode == 1 ? p.out : p.out2;
 #pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          const int sl = sb + i * ss;
-          if (sl * 2 >= nchunks) break;
-          const int j = sl * 64;
-          const int ncol = (sl * 2 + 1 < nchunks) ? 64 : 32;
-          uint32_t o[32];
-#pragma unroll
-          for (int g = 0; g < 16; ++g) {
-            if (g * 4 >= ncol) break;
-            const ulonglong2 gv = *reinterpret_cast<const ulonglong2*>(gamma_s + j + g * 4);
-            const ulonglong2 bv = *reinterpret_cast<const ulonglong2*>(beta_s + j + g * 4);
-            const uint32_t a2 = keep[i * 32 + 2 * g], b2 = keep[i * 32 + 2 * g + 1];
-            uint64_t y0 = fma2(fma2(pk2(bf16_lo(a2), bf16_hi(a2)), rstd2, nmr2), gv.x, bv.x);
-            uint64_t y1 = fma2(fma2(pk2(bf16_lo(b2), bf16_hi(b2)), rstd2, nmr2), gv.y, bv.y);
-            if (p.ln_silu) {
-              // y holds h = LN(v)/2 (gamma, beta were halved): silu = h + h * tanh(h)
-              float h0, h1, h2, h3;
-              upk2(y0, h0, h1);
-              upk2(y1, h2, h3);
-              y0 = fma2(y0, pk2(tanh_approx(h0), tanh_approx(h1)), y0);
-              y1 = fma2(y1, pk2(tanh_approx(h2), tanh_approx(h3)), y1);
-            }
-            float o0, o1, o2, o3;
-            upk2(y0, o0, o1);
-            upk2(y1, o2, o3);
-            o[2 * g] = pack_bf16x2(o0, o1);
-            o[2 * g + 1] = pack_bf16x2(o2, o3);
+        for (int j = 0; j < BN / 8; ++j) {
+          const int c = 8 * j + cq;
+          float y0 = fmaf(fmaf(acc[4 * j + 2 * r], rstd, nmr), gamma_s[c], beta_s[c]);
+          float y1 = fmaf(fmaf(acc[4 * j + 2 * r + 1], rstd, nmr), gamma_s[c + 1], beta_s[c + 1]);
+          if (p.ln_silu) {
+            // y holds h = LN(v)/2 (gamma, beta were halved): silu = h + h * tanh(h)
+            y0 = fmaf(y0, tanh_approx(y0), y0);
+            y1 = fmaf(y1, tanh_approx(y1), y1);
           }
-          put64(o, ncol, nmap, nrow, j);
+          put(nout, r, c, y0, y1);
         }
       }
-      }  // !kSplit
     }
-    if (p.tma_store && lane == 0) tma_store_wait_all();
-  }
-
-  tc_fence_before();
-  if constexpr (kPair) cluster_sync_all(); else __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    if constexpr (kPair) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(p.tmem_cols) : "memory");
-    else asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(p.tmem_cols) : "memory");
   }
 }
 
@@ -993,11 +715,11 @@ int device_num_sms() {
   static int sms[kMaxDev] = {0};
   int dev = 0;
   cudaGetDevice(&dev);
-  if (dev < 0 || dev >= kMaxDev) return 148;
+  if (dev < 0 || dev >= kMaxDev) return 132;
   if (sms[dev] == 0) {
     int n = 0;
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    sms[dev] = n > 0 ? n : 148;
+    sms[dev] = n > 0 ? n : 132;
   }
   return sms[dev];
 }
@@ -1021,59 +743,49 @@ bool choose_tile(const ConvP& p, int rows, int& BW, int& BH, int& BT, long long*
   }
   return best >= 0;
 }
+// N tile: the widest wgmma instantiation (32, 64, 128, 256) that divides Cout
 int choose_bn(int Co) {
-  if (Co % 32 != 0) return 0;
-  if (Co <= 256) return Co;
-  if (Co % 256 == 0) return 256;
-  if (Co % 128 == 0) return 128;
-  if (Co % 64 == 0) return 64;
+  for (int bn = 256; bn >= 32; bn >>= 1)
+    if (Co % bn == 0) return bn;
   return 0;
 }
 
 }  // namespace
 
 namespace {
+template <int BN, bool kSplit>
+cudaError_t set_smem_attr() {
+  return cudaFuncSetAttribute(conv_tc_kernel<BN, kSplit>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+}
 cudaError_t ensure_func_attrs() {
   static bool done[kMaxDev] = {false};
   int dev = 0;
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= kMaxDev) return cudaErrorInvalidDevice;
   if (done[dev]) return cudaSuccess;
-  const int mx = 227 * 1024;
-  cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
+  cudaError_t e = cudaSuccess;
+  for (cudaError_t x : {set_smem_attr<32, false>(), set_smem_attr<64, false>(), set_smem_attr<128, false>(), set_smem_attr<256, false>(),
+                        set_smem_attr<32, true>(), set_smem_attr<64, true>(), set_smem_attr<128, true>(), set_smem_attr<256, true>()})
+    if (x != cudaSuccess) e = x;
   if (e == cudaSuccess) done[dev] = true;
   return e;
 }
 }  // namespace
 
 const char* conv_tc_last_error() { return g_tc_err.c_str(); }
-void conv_tc_set_pair(bool on) { g_pair_mode = on ? 1 : 0; }
 
-// diagnostics: how many 2-CTA clusters of conv_tc_kernel can be co-resident with `smem` dynamic bytes per CTA
 int conv_tc_cluster_query(int smem, char* msg, int cap) {
-  cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(148);
-  cfg.blockDim = dim3(kThreads);
-  cfg.dynamicSmemBytes = smem;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
+  cudaError_t e = set_smem_attr<128, false>();
   int n = -1;
-  cudaError_t e2 = cudaOccupancyMaxActiveClusters(&n, conv_tc_kernel<true, false>, &cfg);
+  cudaError_t e2 = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, conv_tc_kernel<128, false>, kThreads, smem);
   cudaFuncAttributes fa;
-  cudaFuncGetAttributes(&fa, conv_tc_kernel<true, false>);
-  snprintf(msg, cap, "setattr=%s occ=%s clusters=%d regs=%d static_smem=%zu maxdyn=%d", cudaGetErrorString(e), cudaGetErrorString(e2), n,
+  cudaFuncGetAttributes(&fa, conv_tc_kernel<128, false>);
+  snprintf(msg, cap, "setattr=%s occ=%s ctas_per_sm=%d regs=%d static_smem=%zu maxdyn=%d", cudaGetErrorString(e), cudaGetErrorString(e2), n,
            fa.numRegs, fa.sharedSizeBytes, fa.maxDynamicSharedSizeBytes);
   return n;
 }
 
-bool conv_tc_can_fuse_ln(const ConvP& p) { return p.Co % 32 == 0 && p.Co <= 256 && choose_bn(p.Co) == p.Co; }
+bool conv_tc_can_fuse_ln(const ConvP& p) { return p.Co <= 256 && choose_bn(p.Co) == p.Co; }
 
 bool conv_tc_supported(const ConvP& p, DType tout, bool planning) {
   g_tc_err.clear();
@@ -1115,140 +827,61 @@ cudaError_t launch_conv_tc(const ConvP& p, const bf16* x, const bf16* w_nk, int 
   memset(&t, 0, sizeof(t));
   const int Co_pad = (p.Co + 31) / 32 * 32;
   const int num_sms = device_num_sms();
-  static int mt_env = -1;     // VT_TC_MT=1: experiment knob, forces one M tile per CTA
-  if (mt_env < 0) { const char* e = getenv("VT_TC_MT"); mt_env = e ? atoi(e) : 2; }
   static int halo_env = -1;   // VT_TC_HALO=0 switches the halo windows off (experiment knob)
   if (halo_env < 0) { const char* e = getenv("VT_TC_HALO"); halo_env = e ? atoi(e) : 1; }
-  const bool pair_wanted = pair_mode() == 2 || pair_mode() == 1 || pair_mode() < 0 || (pair_mode() == 3 && choose_bn(Co_pad) == 256);
   size_t smem = 0;
-  int bn_local = 0;
-  // Tile geometry + shared-memory plan.  Split operands double every operand tile: when the preferred geometry (halo
-  // windows, two M tiles) leaves fewer than 2 pipeline stages, fall back to the next simpler one.
-  auto plan = [&](bool allow_halo, bool allow_mt2, bool allow_tma_store, int bn_cap) -> int {
-  const int mt_cap = allow_mt2 ? mt_env : 1;
-  t.halo = 0; t.hP = 0; t.a_stages = 0; t.halo_bytes = 0;
-  t.BN = choose_bn(Co_pad);
-  if (bn_cap && t.BN > bn_cap && Co_pad % bn_cap == 0) t.BN = bn_cap;
-  // two M tiles per CTA tile when the N tile is narrow: one B (weight) tile then feeds 256 output rows, which halves
-  // the weight bytes per FLOP (the N<=128 layers are operand-bandwidth bound otherwise)
-  t.MT = 1;
-  long long pad1 = 0, pad2 = 0;
-  if (!choose_tile(p, 128, t.BW, t.BH, t.BT, &pad1)) { g_tc_err = "no tile shape"; return -1; }
-  if (t.BN <= 128 && mt_cap >= 2) {
-    int bw2, bh2, bt2;
-    if (choose_tile(p, 256, bw2, bh2, bt2, &pad2) && pad2 <= pad1 + pad1 / 16 &&
-        (long long)p.B * pad2 / 256 * (Co_pad / t.BN) >= 2LL * num_sms) {
-      t.MT = 2; t.BW = bw2; t.BH = bh2; t.BT = bt2;
-    }
-  }
-  // CTA pairs (cta_group::2): the tile doubles again, each CTA keeps its own MT*128 rows and half of the weight rows
-  t.pair = 0;
-  t.tileBH = t.BH; t.tileBT = t.BT;
-  // default policy (VT_TC_PAIR unset): pairs wherever there are enough tiles (N = 128, k133: 1247 -> 1336 TF/s, with the
-  // halo window 1343 -> 1599; profiles/notes_r1.md)
-  if (w_batches <= 1 && pair_wanted) {
-    int bwp, bhp, btp;
-    long long padp = 0;
-    const int rows = 256 * t.MT;
-    const long long pad_single = (t.MT == 2) ? pad2 : pad1;
-    if (choose_tile(p, rows, bwp, bhp, btp, &padp) && padp <= pad_single + pad_single / 16 &&
-        (pair_mode() == 2 || (long long)p.B * padp / rows * (Co_pad / t.BN) >= (long long)(num_sms / 2) * 2)) {
-      int cbh = bhp, cbt = btp;
-      if (btp >= 2) cbt = btp / 2; else cbh = bhp / 2;
-      if (cbh >= 1 && bwp * cbh * cbt == 128 * t.MT) {
-        t.pair = 1; t.BW = bwp; t.BH = cbh; t.BT = cbt; t.tileBH = bhp; t.tileBT = btp;
-      }
-    }
-  }
-  // halo mode: spatial taps reuse one shared-memory window (see TcParams::halo)
-  {
+  // Tile geometry + shared-memory plan.  Split operands double every operand tile: when the halo windows leave fewer
+  // than 2 pipeline stages, fall back to one A box per tap.
+  auto plan = [&](bool allow_halo, int bn_cap) -> int {
+    t.halo = 0; t.hP = 0; t.a_stages = 0; t.halo_bytes = 0;
+    t.BN = choose_bn(Co_pad);
+    if (bn_cap && t.BN > bn_cap) t.BN = bn_cap;
+    if (!choose_tile(p, 128, t.BW, t.BH, t.BT)) { g_tc_err = "no tile shape"; return -1; }
+    // halo mode: spatial taps reuse one shared-memory window (see TcParams::halo)
     const bool geom = p.sh == 1 && p.sw == 1 && p.kh * p.kw > 1 && p.kh <= 3 && p.kw <= 3 && p.Ho == p.Hi && p.Wo == p.Wi &&
                       w_batches <= 1 && p.Wo % 8 == 0 && p.Ho % 16 == 0;
     if (allow_halo && halo_env && geom) {
-      const long long pos = (long long)p.B * p.To * p.Ho * p.Wo;
-      const long long ntl = Co_pad / t.BN;
-      int mt = 1;
-      if (t.BN <= 128 && mt_cap >= 2 && p.Wo % 16 == 0 && pos / 256 * ntl >= 2LL * num_sms) mt = 2;
-      int pr = 0;
-      if (pair_wanted && p.Ho % 32 == 0 && (pair_mode() == 2 || pos / (256 * mt) * ntl >= (long long)(num_sms / 2) * 2)) pr = 1;
       t.halo = 1;
-      t.MT = mt; t.pair = pr;
-      t.BW = 8 * mt; t.BH = 16; t.BT = 1;
-      t.tileBH = pr ? 32 : 16; t.tileBT = 1;
-      t.hP = 8 * mt + 8;
+      t.BW = 8; t.BH = 16; t.BT = 1;
+      t.hP = 16;
       t.halo_bytes = (uint32_t)((16 + p.kh - 1) * t.hP * 128);
       t.a_stages = 2;
     }
-  }
-  t.tilesW = (p.Wo + t.BW - 1) / t.BW; t.tilesH = (p.Ho + t.tileBH - 1) / t.tileBH; t.tilesT = (p.To + t.tileBT - 1) / t.tileBT;
-  t.num_n_tiles = Co_pad / t.BN;
-  t.num_tiles = (long long)p.B * t.tilesT * t.tilesH * t.tilesW * t.num_n_tiles;
-  // epilogue strategy
-  t.tma_store = (out_bf16 && p.osC == 1 && t.BN % 64 == 0 && p.osW % 8 == 0 && p.osH % 8 == 0 && p.osT % 8 == 0 && p.osB % 8 == 0 &&
-                 (((uintptr_t)out) & 15) == 0) ? 1 : 0;
-  {
-    // the staging buffers cost a pipeline stage; long-K layers hide the direct-store epilogue behind their main loop
-    int ntaps_eff = p.kt * p.kh * p.kw;
-    if (ntaps_eff * (p.Ci / 64) >= 48) t.tma_store = 0;
-  }
-  if (!allow_tma_store) t.tma_store = 0;
-  bn_local = t.pair ? t.BN / 2 : t.BN;
-  const size_t stage_bytes = (size_t)cw * ((t.halo ? 0 : (size_t)t.MT * kABytes) + (size_t)bn_local * 128);
-  const size_t budget = 222 * 1024;
-  const size_t fixed = 1024 /*align*/ + 8 * 2 * 8 + 64 + 2 * 768 * 4 + 2 * 2 * 128 * 2 * 4 + 256;
-  const size_t a_ring = (size_t)t.a_stages * t.halo_bytes * cw;
-  // one staging buffer per epilogue warp: a second one (VT_TC_STG=2, if the ring keeps >= 3 stages) costs operand
-  // stages, which was measured to matter more (model step 143.3 -> 140.6 ms, profiles/notes_r1.md)
-  t.stg_bufs = 1;
-  static int stg_env = -1;
-  if (stg_env < 0) { const char* e = getenv("VT_TC_STG"); stg_env = e ? atoi(e) : 1; }
-  if (stg_env >= 2 && t.tma_store && budget > fixed + a_ring + (size_t)kEpiWarps * 2 * 4096 &&
-      (budget - fixed - a_ring - (size_t)kEpiWarps * 2 * 4096) / stage_bytes >= 3) t.stg_bufs = 2;
-  const size_t staging = t.tma_store ? (size_t)kEpiWarps * t.stg_bufs * 4096 : 0;
-  if (budget < fixed + staging + a_ring + 2 * stage_bytes) return 1;
-  int stages = (int)((budget - fixed - staging - a_ring) / stage_bytes);
-  if (stages > 8) stages = 8;
-  {
-    static int cap = -1;   // VT_TC_STAGES: experiment knob (pipeline-depth sensitivity)
-    if (cap < 0) { const char* e = getenv("VT_TC_STAGES"); cap = e ? atoi(e) : 0; }
-    if (cap >= 2 && stages > cap) stages = cap;
-  }
-  if (stages < 2) return 1;
-  t.stages = stages;
-  // smem layout from the 1024-aligned base: [halo windows] [stages x (A | B)] [staging] [barriers | tmem slot | bias/gamma/beta | stats]
-  t.stage_off = (uint32_t)(a_ring + stages * stage_bytes);
-  t.kparts = 1; t.acc_stages = 2;
-  {
-    const int nk_ = p.kt * p.kh * p.kw * (p.Ci / 64);
-    if (split && nk_ >= 64) {          // K >= 4096: as many partial accumulators as TMEM holds, no double buffering
-      int parts = 512 / (t.MT * t.BN);
-      if (parts > 8) parts = 8;
-      if (parts >= 2) { t.kparts = parts; t.acc_stages = (2 * parts * t.MT * t.BN <= 512) ? 2 : 1; }
-    } else if (split && nk_ >= 16) {   // 1024 <= K < 4096: only what fits beside the double-buffered accumulator
-      int parts = 256 / (t.MT * t.BN);
-      if (parts > 8) parts = 8;
-      if (parts >= 2) t.kparts = parts;
+    t.tilesW = (p.Wo + t.BW - 1) / t.BW; t.tilesH = (p.Ho + t.BH - 1) / t.BH; t.tilesT = (p.To + t.BT - 1) / t.BT;
+    t.num_n_tiles = Co_pad / t.BN;
+    t.num_tiles = (long long)p.B * t.tilesT * t.tilesH * t.tilesW * t.num_n_tiles;
+    const size_t stage_bytes = (size_t)cw * ((t.halo ? 0 : (size_t)kABytes) + (size_t)t.BN * 128);
+    const size_t budget = 225 * 1024;
+    const size_t a_ring = (size_t)t.a_stages * t.halo_bytes * cw;
+    const size_t misc = 2 * 768 * 4 + ((reg && reg->mode) ? 128 * 33 * 4 : 0);
+    const size_t fixed = 1024 /*align*/ + misc + 16;
+    if (budget < fixed + a_ring + 2 * (stage_bytes + 16)) return 1;
+    int stages = (int)((budget - fixed - a_ring) / (stage_bytes + 16));
+    if (stages > 8) stages = 8;
+    {
+      static int cap = -1;   // VT_TC_STAGES: experiment knob (pipeline-depth sensitivity)
+      if (cap < 0) { const char* e = getenv("VT_TC_STAGES"); cap = e ? atoi(e) : 0; }
+      if (cap >= 2 && stages > cap) stages = cap;
     }
-  }
-  uint32_t cols = 32;
-  while (cols < (uint32_t)(t.acc_stages * t.kparts * t.MT * t.BN)) cols <<= 1;
-  t.tmem_cols = cols;
-  smem = fixed + staging + a_ring + (size_t)stages * stage_bytes + 8 * (2 * stages + 4 + 2 * t.a_stages);
-  return 0;
+    t.stages = stages;
+    // smem layout from the 1024-aligned base: [halo windows] [stages x (A | B)] [barriers] [bias/gamma/beta | regularizer rows]
+    const size_t bars = 8 * (2 * (size_t)stages + 2 * (size_t)t.a_stages);
+    t.misc_off = (uint32_t)((a_ring + stages * stage_bytes + bars + 15) & ~(size_t)15);
+    smem = 1024 + t.misc_off + misc;
+    // split + long K: the K steps of a tile are summed in groups (TcParams::kparts; needs BN <= 128)
+    t.kparts = 1;
+    const int nk_ = p.kt * p.kh * p.kw * (p.Ci / 64);
+    if (split && t.BN <= 128 && nk_ >= 16) t.kparts = nk_ >= 64 ? 8 : 4;
+    return 0;
   };
   {
-    // preference order; the later entries only matter for split operands (every operand tile doubled): give up the halo
-    // windows, the second M tile, the store staging buffers, and finally (when no LayerNorm needs the whole row) the wide N tile
+    // split + long K without a fused LayerNorm: narrow N tiles leave registers for the running sum (TcParams::kparts)
     const bool need_row = ln && ln->mode;
-    // split + long K: narrow N tiles leave TMEM room for more partial accumulators (TcParams::kparts)
     const int nk = p.kt * p.kh * p.kw * (p.Ci / 64);
-    const int bn_pref = (split && !need_row && w_batches <= 1) ? (nk >= 128 ? 64 : (nk >= 32 ? 128 : 0)) : 0;
-    int rc = plan(true, true, true, bn_pref);
-    if (rc == 1) rc = plan(false, true, true, bn_pref);
-    if (rc == 1) rc = plan(false, false, true, bn_pref);
-    if (rc == 1) rc = plan(false, false, false, bn_pref);
-    if (rc == 1 && !need_row) rc = plan(false, false, true, 128);
-    if (rc == 1 && !need_row) rc = plan(false, false, false, 128);
+    const int bn_pref = (split && !need_row && w_batches <= 1) ? (nk >= 128 ? 64 : (nk >= 16 ? 128 : 0)) : 0;
+    int rc = plan(true, bn_pref);
+    if (rc == 1) rc = plan(false, bn_pref);
+    if (rc == 1 && !need_row) rc = plan(false, 128);
     if (rc == 1) g_tc_err = "not enough shared memory for 2 stages";
     if (rc != 0) return cudaErrorInvalidValue;
   }
@@ -1284,12 +917,6 @@ cudaError_t launch_conv_tc(const ConvP& p, const bf16* x, const bf16* w_nk, int 
   }
   t.w_batched = w_batches > 1 ? 1 : 0;
   if (t.w_batched && w_batches != p.B) { g_tc_err = "batched weights need one weight matrix per batch element"; return cudaErrorInvalidValue; }
-  {
-    static int ev_env = -1;   // VT_TC_EVICT=0: experiment knob
-    if (ev_env < 0) { const char* e = getenv("VT_TC_EVICT"); ev_env = e ? atoi(e) : 1; }
-    const double out_bytes = (double)p.B * p.To * p.Ho * p.Wo * p.Co * 2.0 * cw;
-    t.store_stream = (ev_env && out_bytes > 256e6) ? 1 : 0;
-  }
   // (split mode: the weights carry a power-of-two scale 2^s that the epilogue removes from the whole accumulator, so the
   // residual is multiplied by 2^s * I -- exact in fp16 for s <= 15; larger scales fall back to the epilogue add)
   int ident_s = 0;
@@ -1338,7 +965,7 @@ cudaError_t launch_conv_tc(const ConvP& p, const bf16* x, const bf16* w_nk, int 
     // split weights: [Co_pad][hi(Kpad) | lo(Kpad)]
     cuuint64_t dims[3] = {(cuuint64_t)(cw * Kpad), (cuuint64_t)Co_pad, (cuuint64_t)nb};
     cuuint64_t strides[2] = {(cuuint64_t)(cw * Kpad) * 2, (cuuint64_t)(nb > 1 ? w_batch_stride : (long long)cw * Kpad * Co_pad) * 2};
-    cuuint32_t box[3] = {64, (cuuint32_t)bn_local, 1};
+    cuuint32_t box[3] = {64, (cuuint32_t)t.BN, 1};
     cuuint32_t es[3] = {1, 1, 1};
     CUresult r = enc(&maps.b, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<bf16*>(w_nk), dims, strides, box, es,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -1357,15 +984,7 @@ cudaError_t launch_conv_tc(const ConvP& p, const bf16* x, const bf16* w_nk, int 
     if (r != CUDA_SUCCESS) { g_tc_err = "cuTensorMapEncodeTiled(output/residual) failed: " + std::to_string((int)r); return false; }
     return true;
   };
-  maps.r = maps.a[0]; maps.e = maps.b; maps.o = maps.a[0]; maps.o2 = maps.a[0];
-  if (t.tma_store) {
-    // box of one warp's 32 rows: the first 32 positions of the (w, h, t) box order
-    int qw = t.halo ? 8 : (t.BW < 32 ? t.BW : 32);
-    int qh = t.halo ? 4 : (t.BH < 32 / qw ? t.BH : 32 / qw);
-    int qt = 32 / (qw * qh);
-    if (!encode_out(&maps.o, out, p.To, p.osW, p.osH, p.osT, p.osB, qw, qh, qt)) return cudaErrorInvalidValue;
-    if (t.ln_mode == 2 && !encode_out(&maps.o2, t.out2, p.To, p.osW, p.osH, p.osT, p.osB, qw, qh, qt)) return cudaErrorInvalidValue;
-  }
+  maps.r = maps.a[0]; maps.e = maps.b;
   if (t.res_mma) {
     // 256 x 256 identity: bf16 I, or the 16 fp16 matrices 2^s * I of the split mode; built once per device on the launching stream
     static bf16* ident_dev[2][64] = {{nullptr}};
@@ -1383,7 +1002,7 @@ cudaError_t launch_conv_tc(const ConvP& p, const bf16* x, const bf16* w_nk, int 
     if (!encode_out(&maps.r, p.res, p.resT, p.rsW, p.rsH, p.rsT, p.rsB, t.halo ? t.hP : t.BW, t.halo ? 16 + p.kh - 1 : t.BH, t.BT)) return cudaErrorInvalidValue;
     cuuint64_t dims[3] = {256, 256, 1};
     cuuint64_t strides[2] = {512, 256 * 512};
-    cuuint32_t box[3] = {64, (cuuint32_t)bn_local, 1};
+    cuuint32_t box[3] = {64, (cuuint32_t)t.BN, 1};
     cuuint32_t es[3] = {1, 1, 1};
     CUresult r = enc(&maps.e, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, ident, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
                      CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -1393,34 +1012,23 @@ cudaError_t launch_conv_tc(const ConvP& p, const bf16* x, const bf16* w_nk, int 
     cudaError_t e = ensure_func_attrs();
     if (e != cudaSuccess) { g_tc_err = "cudaFuncSetAttribute(smem)"; return e; }
   }
-  unsigned grid = (unsigned)(t.num_tiles < num_sms ? t.num_tiles : num_sms);
-  if (t.pair) {
-    const long long pairs = num_sms / 2;
-    grid = 2u * (unsigned)(t.num_tiles < pairs ? t.num_tiles : pairs);
-  }
+  const unsigned grid = (unsigned)(t.num_tiles < num_sms ? t.num_tiles : num_sms);
   const double Mrows = (double)p.B * p.To * p.Ho * p.Wo;
   char det[128] = "";
-  if (prof_enabled()) snprintf(det, sizeof(det), "k%d%d%d s%d%d %d->%d @%dx%dx%d tile%dx%dx%d bn%d mt%d%s ln%d r%d%s p%d", p.kt, p.kh, p.kw, p.st, p.sh, p.Ci, p.Co, p.To, p.Ho, p.Wo, t.tileBT, t.tileBH, t.BW, t.BN, t.MT, t.pair ? (t.halo ? " pair halo" : " pair") : (t.halo ? " halo" : ""), t.ln_mode, p.res_mode, t.res_mma ? "m" : "", split ? t.kparts : 1);
+  if (prof_enabled()) snprintf(det, sizeof(det), "k%d%d%d s%d%d %d->%d @%dx%dx%d tile%dx%dx%d bn%d%s ln%d r%d%s p%d", p.kt, p.kh, p.kw, p.st, p.sh, p.Ci, p.Co, p.To, p.Ho, p.Wo, t.BT, t.BH, t.BW, t.BN, t.halo ? " halo" : "", t.ln_mode, p.res_mode, t.res_mma ? "m" : "", split ? t.kparts : 1);
   ProfScope _ps(split ? "conv_tc3" : "conv_tc", 2.0 * Mrows * p.kt * p.kh * p.kw * p.Ci * p.Co,
                 2.0 * cw * ((double)p.B * p.Ti * p.Hi * p.Wi * p.Ci) + Mrows * p.Co * (tout == DT_F32 ? 4.0 : 2.0 * cw), s, det);
-  if (t.pair) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(kThreads);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = s;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    cudaError_t e = split ? cudaLaunchKernelEx(&cfg, conv_tc_kernel<true, true>, maps, t)
-                          : cudaLaunchKernelEx(&cfg, conv_tc_kernel<true, false>, maps, t);
-    count_launch();
-    return e != cudaSuccess ? e : cudaGetLastError();
+  auto launch = [&](auto kern) { kern<<<grid, kThreads, smem, s>>>(maps, t); };
+  switch (t.BN * 2 + (split ? 1 : 0)) {
+    case 64: launch(conv_tc_kernel<32, false>); break;
+    case 65: launch(conv_tc_kernel<32, true>); break;
+    case 128: launch(conv_tc_kernel<64, false>); break;
+    case 129: launch(conv_tc_kernel<64, true>); break;
+    case 256: launch(conv_tc_kernel<128, false>); break;
+    case 257: launch(conv_tc_kernel<128, true>); break;
+    case 512: launch(conv_tc_kernel<256, false>); break;
+    default: launch(conv_tc_kernel<256, true>); break;
   }
-  if (split) conv_tc_kernel<false, true><<<grid, kThreads, smem, s>>>(maps, t);
-  else conv_tc_kernel<false, false><<<grid, kThreads, smem, s>>>(maps, t);
   count_launch();
   return cudaGetLastError();
 }

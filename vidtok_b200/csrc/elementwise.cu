@@ -810,7 +810,7 @@ __global__ void __launch_bounds__(256) transpose_bf16_kernel(const bf16* __restr
 }
 
 // ---- decoder head as "tap planes": conv_out (Cin -> 3, 3x3x3) is first evaluated as ONE 1x1x1 GEMM producing, for
-// every input position, the 27 x 4 per-tap partial outputs P[pos][tap*4 + co] (tcgen05, input read once instead of 27
+// every input position, the 27 x 4 per-tap partial outputs P[pos][tap*4 + co] (wgmma, input read once instead of 27
 // times), then this kernel gathers the 27 shifted partials of each output position (causal zero padding in t, zero padding
 // in h/w, model_3dcausal.py:162-197) and writes the fp32 [B,C,T,H,W] reconstruction, dropping the first to_off frames
 // (model_3dcausal.py:883-885).
@@ -908,7 +908,7 @@ __global__ void __launch_bounds__(256) clip_to_u8_frames_kernel(const float* __r
 
 inline int grid_for(long long total, int block = 256) {
   long long g = (total + block - 1) / block;
-  const long long cap = 148LL * 16;
+  const long long cap = 132LL * 16;
   return (int)(g < 1 ? 1 : (g > cap ? cap : g));
 }
 
@@ -947,7 +947,7 @@ cudaError_t launch_layernorm(DType t, const void* x, const float* gamma, const f
   } else if (C == 128 || C == 256 || C == 512) {
     const long long per_block = (C == 128) ? 8 * 2 * 4 : (C == 256 ? 8 * 4 : 8 * 2);
     long long gb = (rows + per_block - 1) / per_block;
-    if (gb > 148 * 8) gb = 148 * 8;
+    if (gb > 132 * 8) gb = 132 * 8;
 #define VT_LN_BF(CC)                                                                                                  \
   do {                                                                                                                \
     if (silu) layernorm_bf16_kernel<CC, true><<<(unsigned)gb, 256, 0, s>>>((const bf16*)x, gamma, beta, (bf16*)y, rows); \
@@ -1097,7 +1097,7 @@ cudaError_t launch_tap_planes_gather(const bf16* P, const float* bias, float* ou
   if (total <= 0) return cudaSuccess;
   ProfScope _ps("tap_planes_gather", 2.0 * 27 * Co * total, (double)B * Ti * H * W * NP * 2.0 + (double)total * Co * 4.0, s);
   long long g = (total + 255) / 256;
-  if (g > 148LL * 32) g = 148LL * 32;
+  if (g > 132LL * 32) g = 132LL * 32;
   tap_planes_gather_kernel<<<(unsigned)g, 256, 0, s>>>(P, bias, out, B, Ti, H, W, NP, Co, to_off, pt);
   count_launch();
   return cudaGetLastError();

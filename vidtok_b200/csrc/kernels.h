@@ -42,7 +42,7 @@ cudaError_t launch_fsq_indices_to_codes(const int* indices, int d, const int* le
                                         float* codes, cudaStream_t s);
 // weight repacking: w [Co][Ci][taps] (reference OIDHW flattened) -> [K = tap*Ci + ci][Co] fp32
 cudaError_t launch_pack_w_kn(const float* w, float* out, int Co, int Ci, int taps, cudaStream_t s);
-// -> [Co][K = tap*Ci + ci] bf16 (K-major rows for the tcgen05 B operand)
+// -> [Co][K = tap*Ci + ci] bf16 (K-major rows for the wgmma B operand)
 // wscale != 0: split rows [hi(Kpad) | lo(Kpad)] (fp16 planes, DT_SPLIT operand format) of w * wscale (see split_weight_scale)
 cudaError_t launch_pack_w_nk_bf16(const float* w, bf16* out, int Co, int Co_pad, int Ci, int taps, int Kpad, cudaStream_t s,
                                   float wscale = 0.f);
@@ -81,8 +81,8 @@ cudaError_t launch_clip_to_u8_frames(const float* src, uint8_t* dst, int C, int 
 cudaError_t launch_split_to_f32(const bf16* x, float* y, long long rows, int C, cudaStream_t s);
 cudaError_t launch_f32_to_split(const float* x, bf16* y, long long rows, int C, cudaStream_t s);
 
-// conv_tc.cu (tcgen05 / TMA implicit GEMM)
-// LayerNorm(+SiLU) of the output row fused into the conv epilogue (the row is complete in TMEM when Cout <= 256):
+// conv_tc.cu (wgmma / TMA implicit GEMM)
+// LayerNorm(+SiLU) of the output row fused into the conv epilogue (the row is complete in one N tile when Cout <= 256):
 // mode 1: out := act(LN(v));  mode 2: out := v, out2 := act(LN(v))   (out2 uses the strides of out)
 struct TcLnFusion {
   int mode = 0;
@@ -120,10 +120,10 @@ cudaError_t launch_pack_w_tap_planes(const float* w, bf16* out, int Co, int Ci, 
 // x [batch][rows][cols] -> y [batch][cols][rows] (bf16), rows and cols multiples of 32
 cudaError_t launch_transpose_bf16(const bf16* x, bf16* y, int batch, int rows, int cols, cudaStream_t s, bool split = false);
 const char* conv_tc_last_error();
-void conv_tc_set_pair(bool on);
+// diagnostics: resident CTAs of the conv kernel per SM with `smem` dynamic bytes, plus its register / smem attributes
 int conv_tc_cluster_query(int smem, char* msg, int cap);
 
-// tblock_tc.cu: fused ResnetCausalBlock1D (k311 conv -> LayerNorm -> SiLU -> k311 conv + residual) for C = 128, v1.0 padding
+// tblock_tc.cu: ResnetCausalBlock1D (k311 conv -> LayerNorm -> SiLU -> k311 conv + residual) for C = 128, v1.0 padding
 bool tblock_tc_supported(int B, int T, int H, int W, int C, bool planning = false);
 cudaError_t launch_tblock_tc(const bf16* n1, const bf16* x, const bf16* w1, const float* bias1, const float* gamma2,
                              const float* beta2, const bf16* w2, const float* bias2, bf16* out, bf16* out2,
@@ -131,7 +131,7 @@ cudaError_t launch_tblock_tc(const bf16* n1, const bf16* x, const bf16* w1, cons
                              cudaStream_t s);
 const char* tblock_tc_last_error();
 
-// conv_stem.cu (thread-built im2col A tile + tcgen05 for the Cin=3 stem)
+// conv_stem.cu (thread-built im2col A tile + wgmma for the Cin=3 stem)
 bool conv_stem_supported(const ConvP& p);
 cudaError_t launch_conv_stem(const ConvP& p, const float* x, const bf16* wpk, bf16* out, cudaStream_t s);
 cudaError_t launch_stem_cache_update(const float* x, float* cache, int B, int Ci, int T, int t_rep, int H, int W, cudaStream_t s);

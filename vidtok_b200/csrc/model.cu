@@ -331,7 +331,7 @@ struct ConvOpt {
   bool force_simt = false;
   void* out_view = nullptr;       // write into an existing channels-last tensor through these element strides
   long long ov_sB = 0, ov_sT = 0, ov_sH = 0, ov_sW = 0;
-  // LayerNorm(+SiLU) fusion requests (BF16 tcgen05 path only; silently not honoured otherwise -> check fused1/fused2)
+  // LayerNorm(+SiLU) fusion requests (BF16 wgmma path only; silently not honoured otherwise -> check fused1/fused2)
   const NormW* ln1 = nullptr;     // replace the output by act(LN(out))           (conv1 -> norm2 of a ResBlock)
   bool ln1_silu = true;
   const NormW* ln2 = nullptr;     // additionally produce act(LN(out))            (stream producer -> next block's norm1)
@@ -339,7 +339,7 @@ struct ConvOpt {
   void* ln2_view = nullptr;       // with out_view: where the normalised copy goes (same strides)
   mutable bool fused1 = false, fused2 = false;
   mutable Act ln2_act;            // filled when fused2 and no view was given
-  // regularizer (KL / FSQ) fused into the epilogue of an fp32 head (encoder conv_out); honoured on the tcgen05 path only
+  // regularizer (KL / FSQ) fused into the epilogue of an fp32 head (encoder conv_out); honoured on the wgmma path only
   const TcRegFusion* reg = nullptr;
   bool reg_only = false;          // nobody reads the head's own output (h_pre): skip its stores when the regularizer is fused
   mutable bool fused_reg = false;
@@ -577,7 +577,7 @@ struct Exec {
       } else if (stem) {
         if (!cuda(launch_conv_stem(p, o.ext_in, wst, (bf16*)out.p, s), "conv_stem")) return out;
       } else if (!w.w_kn) {
-        rc = fail(VT_ERR_INVALID, "phase-collapsed conv rejected by the tcgen05 path: %s", conv_tc_last_error());
+        rc = fail(VT_ERR_INVALID, "phase-collapsed conv rejected by the wgmma path: %s", conv_tc_last_error());
         return out;
       } else {
         if (!cuda(launch_conv_simt(p, tin, tout, ta, o.ext_in ? (const void*)o.ext_in : in.p, w.w_kn, out.p, s), "conv_simt")) return out;
@@ -702,7 +702,7 @@ struct Exec {
     if (r.has_nin) free_act(skip);
     set_stream(st, out, o);
   }
-  // tcgen05 path of the attention core: S = scale * Q K^T (fp32), P = softmax(S) (bf16), O = P V.
+  // wgmma path of the attention core: S = scale * Q K^T (fp32), P = softmax(S) (bf16), O = P V.
   // Both products are the conv_tc GEMM with per-frame "weights": K of the frame for the scores, V^T for the output.
   bool attention_tc(const Act& q, const Act& k, const Act& v, Act& o) {
     const int frames = q.B * q.T, tokens = q.H * q.W, C = q.C;
@@ -745,7 +745,7 @@ struct Exec {
     }
     Act o = new_act(q.B, q.T, q.H, q.W, C);
     if (split) {
-      // shapes the tcgen05 path does not take (tiny test models): join hi|lo to fp32, fp32 FMA GEMMs, split the result
+      // shapes the wgmma path does not take (tiny test models): join hi|lo to fp32, fp32 FMA GEMMs, split the result
       const size_t nqc = (size_t)frames * tokens * C;
       float* S = (float*)alloc((size_t)frames * tokens * tokens * sizeof(float));
       float* P = (float*)alloc((size_t)frames * tokens * tokens * sizeof(float));
@@ -1021,7 +1021,7 @@ static void run_stages(Exec& ex, Exec::Stream& st, const std::vector<Stage>& sta
 }
 
 // x_ext: fp32 [B,Cin,T,H,W]; h_out: fp32 [B,Cz,Tz,Hz,Wz].  reg (optional): regularizer outputs; when conv_out runs on the
-// tcgen05 path it is applied in that kernel's epilogue (reg_done = true) and h_out is only written if want_h.
+// wgmma path it is applied in that kernel's epilogue (reg_done = true) and h_out is only written if want_h.
 static void run_encoder(Exec& ex, const float* x_ext, int B, int T, int H, int W, float* h_out, const TcRegFusion* reg = nullptr,
                         bool want_h = true, bool* reg_done = nullptr) {
   if (reg_done) *reg_done = false;
@@ -1986,7 +1986,7 @@ static int op_conv_impl(int precision, int force_simt, const vt_conv_desc* d, co
   TcLnFusion lf;
   if (e && e->ln_mode) {
     if (!gamma || !beta || (e->ln_mode == 2 && !out2)) return fail(VT_ERR_INVALID, "fused LayerNorm needs gamma, beta (and out2 for mode 2)");
-    if (precision == VT_PREC_FMA32 || force_simt) return fail(VT_ERR_INVALID, "the LayerNorm epilogue exists on the tcgen05 path only");
+    if (precision == VT_PREC_FMA32 || force_simt) return fail(VT_ERR_INVALID, "the LayerNorm epilogue exists on the wgmma path only");
     if (!conv_tc_can_fuse_ln(p)) return fail(VT_ERR_INVALID, "LayerNorm cannot be fused for this Cout");
     lf.mode = e->ln_mode; lf.silu = e->ln_silu != 0; lf.gamma = gamma; lf.beta = beta; lf.out2 = out2;
   }
@@ -1996,7 +1996,7 @@ static int op_conv_impl(int precision, int force_simt, const vt_conv_desc* d, co
   const bool want_tc = precision != VT_PREC_FMA32 && !force_simt;
   if (want_tc) {
     if (d->Ci % 64 != 0 || !conv_tc_supported(p, tout))
-      return fail(VT_ERR_INVALID, "tcgen05 conv does not support this geometry: %s", d->Ci % 64 ? "Cin % 64 != 0" : conv_tc_last_error());
+      return fail(VT_ERR_INVALID, "wgmma conv does not support this geometry: %s", d->Ci % 64 ? "Cin % 64 != 0" : conv_tc_last_error());
     const int Co_pad = (d->Co + 31) / 32 * 32;
     VT_CUDA(cudaMalloc(&wnk, (size_t)K * Co_pad * sizeof(bf16) * cw));
     float wsc = 0.f;
@@ -2038,7 +2038,7 @@ int32_t vt_op_conv_regularize(int32_t precision, const vt_conv_desc* d, const vo
                               int32_t reg_mode, int32_t zc, const int32_t* fsq_levels, const float* noise, float* h_out,
                               float* z, int32_t* indices, float* kl_loss, void* stream) {
   if (!d || !z) return fail(VT_ERR_INVALID, "null argument");
-  if (precision != VT_PREC_BF16 && precision != VT_PREC_EXACT_TC) return fail(VT_ERR_INVALID, "the regularizer epilogue exists on the tcgen05 path only");
+  if (precision != VT_PREC_BF16 && precision != VT_PREC_EXACT_TC) return fail(VT_ERR_INVALID, "the regularizer epilogue exists on the wgmma path only");
   cudaStream_t s = (cudaStream_t)stream;
   vt_conv_ex e;
   memset(&e, 0, sizeof(e));
@@ -2071,7 +2071,7 @@ int32_t vt_op_conv_regularize(int32_t precision, const vt_conv_desc* d, const vo
 int32_t vt_op_conv_stem(int32_t precision, const float* x, const float* w, const float* bias, void* out, int32_t B,
                         int32_t Ci, int32_t T, int32_t H, int32_t W, int32_t Co, int32_t t_rep, void* stream) {
   if (!x || !w || !out) return fail(VT_ERR_INVALID, "null argument");
-  if (precision != VT_PREC_BF16 && precision != VT_PREC_EXACT_TC) return fail(VT_ERR_INVALID, "the stem kernel is a tcgen05 kernel (BF16 / EXACT_TC)");
+  if (precision != VT_PREC_BF16 && precision != VT_PREC_EXACT_TC) return fail(VT_ERR_INVALID, "the stem kernel is a wgmma kernel (BF16 / EXACT_TC)");
   cudaStream_t s = (cudaStream_t)stream;
   const bool split = precision == VT_PREC_EXACT_TC;
   ConvP p;
@@ -2244,7 +2244,7 @@ int32_t vt_op_groupnorm(int32_t precision, const void* x, const float* gamma, co
                            (float*)workspace, (cudaStream_t)stream));
   return VT_OK;
 }
-// The attention core the model path runs for this precision and shape: tcgen05 GEMMs (per-frame K / V^T as the B
+// The attention core the model path runs for this precision and shape: wgmma GEMMs (per-frame K / V^T as the B
 // operand) when tokens and C are multiples of 64 in the tensor-core modes, fp32 FMA GEMMs otherwise.
 int32_t vt_op_attention(int32_t precision, const void* q, const void* k, const void* v, void* o, int32_t frames,
                         int32_t tokens, int32_t C, void* workspace, int64_t workspace_bytes, void* stream) {
@@ -2256,7 +2256,7 @@ int32_t vt_op_attention(int32_t precision, const void* q, const void* k, const v
   Exec ex(&dummy, precision, (cudaStream_t)stream, workspace, (size_t)workspace_bytes, false);
   Act aq, ak, av;
   aq.B = frames; aq.T = 1; aq.H = 1; aq.W = tokens; aq.C = C;
-  // the tcgen05 formulation tiles positions as (H, W) boxes: present the token axis as an 8-wide image when possible
+  // the wgmma formulation tiles positions as (H, W) boxes: present the token axis as an 8-wide image when possible
   if (tokens % 8 == 0) { aq.H = tokens / 8; aq.W = 8; }
   ak = aq; av = aq;
   aq.p = const_cast<void*>(q); ak.p = const_cast<void*>(k); av.p = const_cast<void*>(v);

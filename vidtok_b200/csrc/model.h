@@ -24,7 +24,7 @@ struct ConvW {
   int Co = 0, Ci = 0, kt = 1, kh = 1, kw = 1;
   int pw = -1, pb = -1;      // param indices (weight, bias)
   float* w_kn = nullptr;     // [K][Co] fp32
-  bf16* w_nk = nullptr;      // [Co_pad][Kpad] bf16 (tcgen05 B operand), may be null
+  bf16* w_nk = nullptr;      // [Co_pad][Kpad] bf16 (wgmma B operand), may be null
   bf16* w_nk3 = nullptr;     // [Co_pad][hi(Kpad) | lo(Kpad)] fp16 planes of w * wscale3: split operand of the EXACT_TC mode
   float wscale3 = 1.f;       // power of two (kernels.h: split_weight_scale); the epilogue multiplies the accumulator by 1/wscale3
   int Kpad = 0;
@@ -99,7 +99,7 @@ struct vt_model {
   int64_t pool_elems = 0;
   float* packed_kn = nullptr;   // all [K][Co] fp32 repacks
   vt::bf16* packed_nk = nullptr;
-  vt::bf16* packed_nk3 = nullptr;      // split (hi|lo) copies of every tcgen05 weight matrix
+  vt::bf16* packed_nk3 = nullptr;      // split (hi|lo) copies of every wgmma weight matrix
   vt::bf16* packed_stem = nullptr;     // [Co][128] followed by the split copy [Co][256]
   vt::bf16* packed_planes = nullptr;   // decoder conv_out as 27x4 tap planes: [128][Cin] bf16
   vt::ConvW head_planes;               // 1x1x1 pseudo-conv Cin -> 128 using packed_planes

@@ -1,22 +1,20 @@
-// Fused temporal residual block on tcgen05 (BF16 mode):
+// Fused temporal residual block on wgmma (BF16 mode):
 //   ResnetCausalBlock1D  (vidtok/modules/model_3dcausal.py:427-499)
 //     h   = conv1(n1)                      n1 = silu(LN1(x)) is produced by the previous stage's epilogue
 //     out = x + conv2(silu(LN2(h)))        both convs are causal k=3 temporal convolutions (CausalConv1d, :144-159)
-// as ONE kernel.  The two launches of conv_tc.cu it replaces move six full-resolution tensors per block through HBM
-// (n1 in, LN'd h out; LN'd h in, x in, out and LN'd out out) and run at ~0.35 of the HBM roofline (profiles/notes_r1.md);
-// a k=3 temporal convolution is point-wise in space, so a CTA that owns a strip of 128 positions and walks the frames in
-// order can keep LN2(h) in shared memory: HBM sees n1, x in and out (+ the next stage's LN'd copy) out.
+// as ONE kernel.  A k=3 temporal convolution is point-wise in space, so a CTA that owns a strip of 128 positions and walks
+// the frames in order keeps LN2(h) in shared memory: HBM sees n1 and x in and out (+ the next stage's LN'd copy) out, and the
+// intermediate h never leaves the SM.
 //
-// Per CTA (persistent over strips of BW x BH = 128 positions), for t = 0 .. T-1:
-//   G1(t): acc1 = sum_a W1[a] . n1[t-2+a]            A, B tiles by TMA (frames t-2.. are L2 hits), fp32 acc in TMEM
-//   E1(t): h = acc1 + b1;  H[t mod 3] = bf16(silu(LN2(h)))   written by 4 epilogue warps straight into the canonical
-//          K-major SWIZZLE_128B layout (the layout a TMA load would have produced), fence.proxy.async, mbarrier
-//   G2(t): acc2 = sum_a W2[a] . H[t-2+a]  +  I . x[t] A operand = the shared-memory ring, B by TMA; the residual rides the
-//          tensor pipe as extra K steps against an identity tile (as in conv_tc.cu)
-//   E2(t): out[t] = acc2 + b2 (TMA store); optionally out2[t] = act(LN_next(out[t])) for the next stage
-// Issue order G1(0) G1(1) G2(0) G1(2) G2(1) ...: while E1(t) normalises frame t the tensor pipe runs G1(t+1) and G2(t-1).
-// TMEM: acc1 and acc2 double-buffered = 4 x C = 512 columns for C = 128.  Causal zero padding = skipped taps.
-// Warp roles: 0 TMA producer, 1 MMA issuer, 2 TMEM allocator, 3-6 E1, 7-10 E2.
+// Per CTA (persistent over strips of BW x BH = 128 positions), for t = 0 .. T-1, each of the two consumer warpgroups on its
+// 64 rows of the strip:
+//   G1(t): acc = sum_a W1[a] . n1[t-2+a]          A (n1 frame) and B (W1 slice) tiles by TMA; fp32 accumulators in registers
+//   E1(t): H[t mod 3] = bf16(silu(LN2(acc + b1)))  written by the warpgroup straight into the canonical K-major SWIZZLE_128B
+//          layout (the layout a TMA load would have produced), then fence.proxy.async: the ring is the next A operand
+//   G2(t): acc = sum_a W2[a] . H[t-2+a]            A = the shared-memory ring, B (W2 slice) by TMA
+//   E2(t): out[t] = acc + b2 + x[t]; optionally out2[t] = act(LN_next(out[t])) for the next stage
+// Causal zero padding = skipped taps.  Warp roles: warps 0-7 = two consumer warpgroups, warp 8 = TMA producer (its warpgroup
+// hands its registers to the consumers through setmaxnreg).
 #include <cuda.h>
 
 #include <cstdio>
@@ -33,11 +31,14 @@ namespace vt {
 namespace {
 using namespace tcx;
 
+thread_local std::string g_tb_err;
 constexpr int kC = 128;                 // channels (Cin == Cout) this kernel is built for
 constexpr int kKc = kC / 64;            // 64-channel K chunks per tap
-constexpr int kTile = 128 * 128;        // one operand tile: 128 rows x 64 bf16
+constexpr uint32_t kTile = 128 * 128;   // one operand tile: 128 rows x 64 bf16
 constexpr int kHSlots = 3;
-constexpr int kThreadsTb = 11 * 32;
+constexpr int kConsumerWarps = 8;
+constexpr int kProducerWarp = kConsumerWarps;
+constexpr int kThreadsTb = (kConsumerWarps + 4) * 32;
 
 struct TbParams {
   int B, T, H, W;
@@ -52,14 +53,22 @@ struct TbParams {
   int ln_out, ln_out_silu;   // additionally write out2 = act(LN(out)) (the next stage's first norm)
   const float* g3;
   const float* b3;
-  int store_stream;
+  const bf16* x;
+  bf16* out;
+  bf16* out2;
 };
 struct TbMaps {
-  CUtensorMap n1, x, w1, w2, e, o, o2;
+  CUtensorMap n1, w1, w2;
 };
 
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  v += __shfl_xor_sync(0xffffffffu, v, 2);
+  return v;
+}
+
 // smem layout from the 1024-aligned base:
-//   [H ring: 3 slots x kKc tiles][stage ring: stages x (A tile | B tile)][store staging: 4 warps x 4 KB][barriers][constants]
+//   [H ring: 3 slots x kKc tiles][stage ring: stages x (A tile | B tile)][barriers][constants]
 __global__ void __launch_bounds__(kThreadsTb, 1) tblock_tc_kernel(const __grid_constant__ TbMaps maps, const TbParams p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -68,21 +77,10 @@ __global__ void __launch_bounds__(kThreadsTb, 1) tblock_tc_kernel(const __grid_c
   const uint32_t h_base = smem_base;
   const uint32_t ring_base = h_base + kHSlots * kKc * kTile;
   const uint32_t stage_bytes = 2u * kTile;
-  const uint32_t stg_base = ring_base + (uint32_t)p.stages * stage_bytes;
-  const uint32_t bar_base = stg_base + 4u * 4096u;
+  const uint32_t bar_base = ring_base + (uint32_t)p.stages * stage_bytes;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (p.stages + s); };
-  const uint32_t bar2 = bar_base + 16u * p.stages;
-  auto a1_full = [&](int s) { return bar2 + 8u * s; };
-  auto a1_empty = [&](int s) { return bar2 + 8u * (2 + s); };
-  auto a2_full = [&](int s) { return bar2 + 8u * (4 + s); };
-  auto a2_empty = [&](int s) { return bar2 + 8u * (6 + s); };
-  auto h_full = [&](int s) { return bar2 + 8u * (8 + s); };
-  auto h_empty = [&](int s) { return bar2 + 8u * (11 + s); };
-  const uint32_t tmem_slot = bar2 + 8u * 14;
-  const uint32_t const_base = tmem_slot + 16u;
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(smem_gen + (tmem_slot - smem_base));
-  float* cst = reinterpret_cast<float*>(smem_gen + (const_base - smem_base));   // bias1 | g2 | b2 | bias2 | g3 | b3 (kC each)
+  float* cst = reinterpret_cast<float*>(smem_gen + (bar_base - smem_base) + 16u * p.stages);   // bias1 | g2 | b2 | bias2 | g3 | b3
 
   for (int i = threadIdx.x; i < kC; i += kThreadsTb) {
     cst[i] = p.bias1 ? p.bias1[i] : 0.f;
@@ -94,867 +92,205 @@ __global__ void __launch_bounds__(kThreadsTb, 1) tblock_tc_kernel(const __grid_c
     cst[4 * kC + i] = p.ln_out ? sc * p.g3[i] : 0.f;
     cst[5 * kC + i] = p.ln_out ? sc * p.b3[i] : 0.f;
   }
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&maps.n1); prefetch_tmap(&maps.x); prefetch_tmap(&maps.w1); prefetch_tmap(&maps.w2);
-    prefetch_tmap(&maps.e); prefetch_tmap(&maps.o);
-    if (p.ln_out) prefetch_tmap(&maps.o2);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < p.stages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(a1_full(s), 1); mbar_init(a1_empty(s), 4);
-      mbar_init(a2_full(s), 1); mbar_init(a2_empty(s), 4);
-    }
-    for (int s = 0; s < kHSlots; ++s) { mbar_init(h_full(s), 4); mbar_init(h_empty(s), 1); }
+  if (threadIdx.x == 0) {
+    // a stage is released by every consumer warp once its own wait has seen the MMAs that read it complete
+    for (int s = 0; s < p.stages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), kConsumerWarps); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  constexpr uint32_t kTmemCols = 4 * kC;   // acc1[2] | acc2[2]
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(kTmemCols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
 
-  const long long strip0 = blockIdx.x, strip_step = gridDim.x;
-  auto decode = [&](long long strip, int& b, int& h0, int& w0) {
-    const int tw = (int)(strip % p.tilesW);
-    long long m = strip / p.tilesW;
-    const int th = (int)(m % p.tilesH);
-    b = (int)(m / p.tilesH);
-    h0 = th * p.BH;
-    w0 = tw * p.BW;
-  };
-  const int T = p.T, nstages = p.stages;
-
-  if (warp == 0) {
-    // ===================== TMA producer =====================
+  if (warp >= kProducerWarp) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+    if (warp != kProducerWarp) return;
+    // ===================== TMA producer: per frame the G1 steps (n1 tile + W1 slice), then the G2 steps (W2 slice) =====
     const bool el = elect_one();
+    if (el) { prefetch_tmap(&maps.n1); prefetch_tmap(&maps.w1); prefetch_tmap(&maps.w2); }
     int stage = 0;
     uint32_t phase = 0;
     auto acquire = [&](uint32_t bytes) {
       mbar_wait(empty_bar(stage), phase ^ 1u);
       if (el) mbar_expect_tx(full_bar(stage), bytes);
     };
-    auto advance = [&]() { if (++stage == nstages) { stage = 0; phase ^= 1u; } };
-    for (long long strip = strip0; strip < p.num_strips; strip += strip_step) {
-      int b, h0, w0;
-      decode(strip, b, h0, w0);
-      // the loads of G2(u): W2 tap tiles (A operand = the H ring), then the residual K steps (x tile, identity tile)
-      auto g2_loads = [&](int u) {
+    auto advance = [&]() { if (++stage == p.stages) { stage = 0; phase ^= 1u; } };
+    for (long long strip = blockIdx.x; strip < p.num_strips; strip += gridDim.x) {
+      const int tw = (int)(strip % p.tilesW);
+      const int th = (int)((strip / p.tilesW) % p.tilesH);
+      const int b = (int)(strip / ((long long)p.tilesW * p.tilesH));
+      const int w0 = tw * p.BW, h0 = th * p.BH;
+      for (int t = 0; t < p.T; ++t) {
         for (int a = 0; a < 3; ++a) {
-          if (u - 2 + a < 0) continue;
+          if (t - 2 + a < 0) continue;
+          for (int kc = 0; kc < kKc; ++kc) {
+            acquire(2u * kTile);
+            if (el) {
+              const uint32_t sa = ring_base + stage * stage_bytes;
+              tma_load_5d(sa, &maps.n1, full_bar(stage), kc * 64, w0, h0, t - 2 + a, b);
+              tma_load_3d(sa + kTile, &maps.w1, full_bar(stage), a * kC + kc * 64, 0, 0);
+            }
+            advance();
+          }
+        }
+        for (int a = 0; a < 3; ++a) {
+          if (t - 2 + a < 0) continue;
           for (int kc = 0; kc < kKc; ++kc) {
             acquire(kTile);
             if (el) tma_load_3d(ring_base + stage * stage_bytes + kTile, &maps.w2, full_bar(stage), a * kC + kc * 64, 0, 0);
             advance();
           }
         }
-        for (int g = 0; g < kKc; ++g) {
-          acquire(2u * kTile);
-          if (el) {
-            const uint32_t sa = ring_base + stage * stage_bytes;
-            tma_load_5d(sa, &maps.x, full_bar(stage), g * 64, w0, h0, u, b);
-            tma_load_3d(sa + kTile, &maps.e, full_bar(stage), g * 64, 0, 0);
-          }
-          advance();
-        }
-      };
-      for (int t = 0; t < T; ++t) {
-        for (int a = 0; a < 3; ++a) {
-          const int tv = t - 2 + a;
-          if (tv < 0) continue;
-          for (int kc = 0; kc < kKc; ++kc) {
-            acquire(2u * kTile);
-            if (el) {
-              const uint32_t sa = ring_base + stage * stage_bytes;
-              tma_load_5d(sa, &maps.n1, full_bar(stage), kc * 64, w0, h0, tv, b);
-              tma_load_3d(sa + kTile, &maps.w1, full_bar(stage), a * kC + kc * 64, 0, 0);
-            }
-            advance();
-          }
-        }
-        if (t >= 1) g2_loads(t - 1);
-      }
-      g2_loads(T - 1);
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    const bool el = elect_one();
-    const uint32_t idesc = make_idesc(kC, 128);
-    const uint32_t hi_d = 64u | (1u << 14) | (2u << 29);   // SBO 1024 B, version 1, SWIZZLE_128B
-    int stage = 0;
-    uint32_t phase = 0;
-    long long f1 = 0, f2 = 0;   // global frame counters of G1 / G2 (barrier phases run across strips)
-    auto desc_lo = [&](uint32_t addr) { return ((addr & 0x3FFFFu) >> 4) | 0x10000u; };
-    auto mma4 = [&](uint32_t d, uint32_t a_lo, uint32_t b_lo, uint32_t acc) {
-#pragma unroll
-      for (uint32_t j = 0; j < 8u; j += 2u) umma_f16_lohi(d, a_lo + j, hi_d, b_lo + j, hi_d, idesc, j == 0 ? acc : 1u);
-    };
-    auto next_stage = [&]() { if (++stage == nstages) { stage = 0; phase ^= 1u; } };
-    for (long long strip = strip0; strip < p.num_strips; strip += strip_step) {
-      auto g2 = [&](int u) {
-        const uint32_t as = (uint32_t)(f2 & 1), aph = (uint32_t)((f2 >> 1) & 1);
-        mbar_wait(h_full((int)(f2 % kHSlots)), (uint32_t)((f2 / kHSlots) & 1));   // E1 has written H[u]
-        mbar_wait(a2_empty(as), aph ^ 1u);
-        tc_fence_after();
-        const uint32_t d = tmem_base + 2u * kC + as * kC;
-        uint32_t accum = 0;
-        for (int a = 0; a < 3; ++a) {
-          if (u - 2 + a < 0) continue;
-          const long long fh = f2 - 2 + a;                 // global index of the H frame this tap reads
-          const uint32_t hs = h_base + (uint32_t)(fh % kHSlots) * (kKc * kTile);
-          for (int kc = 0; kc < kKc; ++kc) {
-            mbar_wait(full_bar(stage), phase);
-            tc_fence_after();
-            if (el) {
-              mma4(d, desc_lo(hs + kc * kTile), desc_lo(ring_base + stage * stage_bytes + kTile), accum);
-              umma_commit(empty_bar(stage));
-            }
-            accum = 1;
-            next_stage();
-          }
-        }
-        for (int g = 0; g < kKc; ++g) {   // + I * x[u]
-          mbar_wait(full_bar(stage), phase);
-          tc_fence_after();
-          if (el) {
-            const uint32_t sa = ring_base + stage * stage_bytes;
-            mma4(d, desc_lo(sa), desc_lo(sa + kTile), 1u);
-            umma_commit(empty_bar(stage));
-          }
-          next_stage();
-        }
-        if (el) {
-          umma_commit(a2_full(as));
-          if (f2 >= 2) umma_commit(h_empty((int)((f2 - 2) % kHSlots)));   // frame f2-2 is not read again
-        }
-        ++f2;
-      };
-      for (int t = 0; t < T; ++t) {
-        {
-          const uint32_t as = (uint32_t)(f1 & 1), aph = (uint32_t)((f1 >> 1) & 1);
-          mbar_wait(a1_empty(as), aph ^ 1u);
-          tc_fence_after();
-          const uint32_t d = tmem_base + as * kC;
-          uint32_t accum = 0;
-          for (int a = 0; a < 3; ++a) {
-            if (t - 2 + a < 0) continue;
-            for (int kc = 0; kc < kKc; ++kc) {
-              mbar_wait(full_bar(stage), phase);
-              tc_fence_after();
-              if (el) {
-                const uint32_t sa = ring_base + stage * stage_bytes;
-                mma4(d, desc_lo(sa), desc_lo(sa + kTile), accum);
-                umma_commit(empty_bar(stage));
-              }
-              accum = 1;
-              next_stage();
-            }
-          }
-          if (el) umma_commit(a1_full(as));
-          ++f1;
-        }
-        if (t >= 1) g2(t - 1);
-      }
-      g2(T - 1);
-    }
-  } else if (warp >= 3 && warp < 7) {
-    // ===================== E1: h = acc1 + b1 -> H[t] = bf16(silu(LN2(h))) =====================
-    const int q = warp & 3;
-    const int rr = q * 32 + lane;
-    const int swz = lane & 7;
-    const float* bias1 = cst;
-    const float* gam = cst + kC;
-    const float* bet = cst + 2 * kC;
-    long long f = 0;
-    for (long long strip = strip0; strip < p.num_strips; strip += strip_step) {
-      for (int t = 0; t < T; ++t, ++f) {
-        const uint32_t as = (uint32_t)(f & 1), aph = (uint32_t)((f >> 1) & 1);
-        mbar_wait(a1_full(as), aph);
-        tc_fence_after();
-        const uint32_t tb = tmem_base + ((uint32_t)(q * 32) << 16) + as * kC;
-        uint64_t lsum2 = 0ull, lsq2 = 0ull;
-        uint32_t keep[kC / 2];
-#pragma unroll
-        for (int c = 0; c < kC / 32; ++c) {
-          uint32_t v[32];
-          tmem_ld32(tb + (uint32_t)(c * 32), v);
-          tmem_ld_wait();
-#pragma unroll
-          for (int g = 0; g < 8; ++g) {
-            const ulonglong2 bv = *reinterpret_cast<const ulonglong2*>(bias1 + c * 32 + g * 4);
-            const uint64_t a0 = add2(pk2(__uint_as_float(v[g * 4 + 0]), __uint_as_float(v[g * 4 + 1])), bv.x);
-            const uint64_t a1 = add2(pk2(__uint_as_float(v[g * 4 + 2]), __uint_as_float(v[g * 4 + 3])), bv.y);
-            lsum2 = add2(lsum2, add2(a0, a1));
-            lsq2 = fma2(a0, a0, lsq2);
-            lsq2 = fma2(a1, a1, lsq2);
-            float f0, f1, f2_, f3;
-            upk2(a0, f0, f1);
-            upk2(a1, f2_, f3);
-            keep[c * 16 + g * 2] = pack_bf16x2(f0, f1);
-            keep[c * 16 + g * 2 + 1] = pack_bf16x2(f2_, f3);
-          }
-        }
-        // the accumulator has been read: hand it back before the normalisation pass
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(a1_empty(as));
-        float lsum, lsq;
-        {
-          float a, b;
-          upk2(lsum2, a, b); lsum = a + b;
-          upk2(lsq2, a, b); lsq = a + b;
-        }
-        const float mean = lsum * (1.0f / kC);
-        float var = fmaf(-mean, mean, lsq * (1.0f / kC));
-        var = var < 0.f ? 0.f : var;
-        const float rstd = rsqrtf(var + 1e-6f);
-        const float nmr = -mean * rstd;
-        const uint64_t rstd2 = pk2(rstd, rstd), nmr2 = pk2(nmr, nmr);
-        // the ring slot of frame f: free once G2(f-1) (the last reader of frame f-3) has completed
-        const int slot = (int)(f % kHSlots);
-        if (f >= kHSlots) mbar_wait(h_empty(slot), (uint32_t)(((f / kHSlots) - 1) & 1));
-        uint8_t* hrow = smem_gen + (h_base - smem_base) + (uint32_t)slot * (kKc * kTile) + (uint32_t)rr * 128u;
-#pragma unroll
-        for (int kc = 0; kc < kKc; ++kc) {
-#pragma unroll
-          for (int g = 0; g < 8; ++g) {
-            uint32_t o[4];
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              const int ci = kc * 64 + g * 8 + h * 4;
-              const ulonglong2 gv = *reinterpret_cast<const ulonglong2*>(gam + ci);
-              const ulonglong2 bv = *reinterpret_cast<const ulonglong2*>(bet + ci);
-              const uint32_t a2 = keep[ci / 2], b2 = keep[ci / 2 + 1];
-              uint64_t y0 = fma2(fma2(pk2(bf16_lo(a2), bf16_hi(a2)), rstd2, nmr2), gv.x, bv.x);
-              uint64_t y1 = fma2(fma2(pk2(bf16_lo(b2), bf16_hi(b2)), rstd2, nmr2), gv.y, bv.y);
-              float h0, h1, h2, h3;
-              upk2(y0, h0, h1);
-              upk2(y1, h2, h3);
-              y0 = fma2(y0, pk2(tanh_approx(h0), tanh_approx(h1)), y0);
-              y1 = fma2(y1, pk2(tanh_approx(h2), tanh_approx(h3)), y1);
-              float o0, o1, o2, o3;
-              upk2(y0, o0, o1);
-              upk2(y1, o2, o3);
-              o[2 * h] = pack_bf16x2(o0, o1);
-              o[2 * h + 1] = pack_bf16x2(o2, o3);
-            }
-            *reinterpret_cast<uint4*>(hrow + kc * kTile + ((g ^ swz) << 4)) = make_uint4(o[0], o[1], o[2], o[3]);
-          }
-        }
-        fence_async_smem();   // generic-proxy writes -> visible to the tensor core's (async proxy) reads
-        __syncwarp();
-        if (lane == 0) mbar_arrive(h_full(slot));
       }
     }
-  } else if (warp >= 7) {
-    // ===================== E2: out = acc2 + b2 (TMA store) [+ out2 = act(LN_next(out))] =====================
-    const int q = warp & 3;
-    const int rr = q * 32 + lane;
-    const int swz = lane & 7;
-    const float* bias2 = cst + 3 * kC;
-    const float* gam = cst + 4 * kC;
-    const float* bet = cst + 5 * kC;
-    const uint32_t wstg = stg_base + (uint32_t)(warp - 7) * 4096u;
-    uint8_t* wstg_gen = smem_gen + (stg_base - smem_base) + (uint32_t)(warp - 7) * 4096u;
-    const int row0 = q * 32;
-    const int qw0 = row0 % p.BW, qh0 = row0 / p.BW;
-    long long f = 0;
-    for (long long strip = strip0; strip < p.num_strips; strip += strip_step) {
-      int b, h0, w0;
-      decode(strip, b, h0, w0);
-      for (int t = 0; t < T; ++t, ++f) {
-        const uint32_t as = (uint32_t)(f & 1), aph = (uint32_t)((f >> 1) & 1);
-        auto put64 = [&](const uint32_t* pk, const CUtensorMap* m, int c0) {
-          if (lane == 0) tma_store_wait_read();   // the store that last used the staging buffer has read it
-          __syncwarp();
-          uint8_t* my = wstg_gen + (uint32_t)lane * 128u;
-#pragma unroll
-          for (int g = 0; g < 8; ++g)
-            *reinterpret_cast<uint4*>(my + ((g ^ swz) << 4)) = make_uint4(pk[4 * g], pk[4 * g + 1], pk[4 * g + 2], pk[4 * g + 3]);
-          fence_async_smem();
-          __syncwarp();
-          if (lane == 0) {
-            if (p.store_stream) tma_store_5d_stream(m, wstg, c0, w0 + qw0, h0 + qh0, t, b);
-            else tma_store_5d(m, wstg, c0, w0 + qw0, h0 + qh0, t, b);
-            tma_store_commit();
-          }
-        };
-        mbar_wait(a2_full(as), aph);
-        tc_fence_after();
-        const uint32_t tb = tmem_base + ((uint32_t)(q * 32) << 16) + 2u * kC + as * kC;
-        uint64_t lsum2 = 0ull, lsq2 = 0ull;
-        uint32_t keep[kC / 2];
-#pragma unroll
-        for (int i = 0; i < kKc; ++i) {
-#pragma unroll
-          for (int hc = 0; hc < 2; ++hc) {
-            uint32_t v[32];
-            tmem_ld32(tb + (uint32_t)(i * 64 + hc * 32), v);
-            tmem_ld_wait();
-#pragma unroll
-            for (int g = 0; g < 8; ++g) {
-              const ulonglong2 bv = *reinterpret_cast<const ulonglong2*>(bias2 + i * 64 + hc * 32 + g * 4);
-              const uint64_t a0 = add2(pk2(__uint_as_float(v[g * 4 + 0]), __uint_as_float(v[g * 4 + 1])), bv.x);
-              const uint64_t a1 = add2(pk2(__uint_as_float(v[g * 4 + 2]), __uint_as_float(v[g * 4 + 3])), bv.y);
-              if (p.ln_out) {
-                lsum2 = add2(lsum2, add2(a0, a1));
-                lsq2 = fma2(a0, a0, lsq2);
-                lsq2 = fma2(a1, a1, lsq2);
-              }
-              float f0, f1, f2_, f3;
-              upk2(a0, f0, f1);
-              upk2(a1, f2_, f3);
-              keep[i * 32 + hc * 16 + g * 2] = pack_bf16x2(f0, f1);
-              keep[i * 32 + hc * 16 + g * 2 + 1] = pack_bf16x2(f2_, f3);
-            }
-          }
-          put64(&keep[i * 32], &maps.o, i * 64);
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(a2_empty(as));
-        if (p.ln_out) {
-          float lsum, lsq;
-          {
-            float a, b2_;
-            upk2(lsum2, a, b2_); lsum = a + b2_;
-            upk2(lsq2, a, b2_); lsq = a + b2_;
-          }
-          const float mean = lsum * (1.0f / kC);
-          float var = fmaf(-mean, mean, lsq * (1.0f / kC));
-          var = var < 0.f ? 0.f : var;
-          const float rstd = rsqrtf(var + 1e-6f);
-          const float nmr = -mean * rstd;
-          const uint64_t rstd2 = pk2(rstd, rstd), nmr2 = pk2(nmr, nmr);
-#pragma unroll
-          for (int i = 0; i < kKc; ++i) {
-            uint32_t o[32];
-#pragma unroll
-            for (int g = 0; g < 16; ++g) {
-              const ulonglong2 gv = *reinterpret_cast<const ulonglong2*>(gam + i * 64 + g * 4);
-              const ulonglong2 bv = *reinterpret_cast<const ulonglong2*>(bet + i * 64 + g * 4);
-              const uint32_t a2 = keep[i * 32 + 2 * g], b2 = keep[i * 32 + 2 * g + 1];
-              uint64_t y0 = fma2(fma2(pk2(bf16_lo(a2), bf16_hi(a2)), rstd2, nmr2), gv.x, bv.x);
-              uint64_t y1 = fma2(fma2(pk2(bf16_lo(b2), bf16_hi(b2)), rstd2, nmr2), gv.y, bv.y);
-              if (p.ln_out_silu) {
-                float h0_, h1, h2, h3;
-                upk2(y0, h0_, h1);
-                upk2(y1, h2, h3);
-                y0 = fma2(y0, pk2(tanh_approx(h0_), tanh_approx(h1)), y0);
-                y1 = fma2(y1, pk2(tanh_approx(h2), tanh_approx(h3)), y1);
-              }
-              float o0, o1, o2, o3;
-              upk2(y0, o0, o1);
-              upk2(y1, o2, o3);
-              o[2 * g] = pack_bf16x2(o0, o1);
-              o[2 * g + 1] = pack_bf16x2(o2, o3);
-            }
-            put64(o, &maps.o2, i * 64);
-          }
-        }
-      }
-    }
-    if (lane == 0) tma_store_wait_all();
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kTmemCols) : "memory");
-  }
-}
-
-// ------------------------------------------------------------------------------------------------------------------
-// Version 2: CTA pairs (cta_group::2), weights resident in shared memory.
-// The first version streams both convolutions' weight tiles through the operand ring for every frame (352 KB of L2 -> SM
-// traffic per 128-position frame against 3.6k cycles of tensor work) and serialises its TMA stores on one staging buffer:
-// measured 3.0-4.7 ms per block, no better than the two conv_tc launches it replaces.  Here
-//   * two CTAs of a cluster share every MMA (M = 256: each CTA's own 128-position strip; N = 128 split across the pair),
-//     so each CTA keeps only its 64-row half of W1 and W2: 2 convs x 3 taps x 2 chunks x 8 KB = 96 KB, loaded ONCE;
-//   * G2 runs in scatter form -- H[t] is multiplied into the accumulators of frames t, t+1 and t+2 (taps 2, 1, 0) as soon
-//     as it exists -- so ONE 32 KB H tile replaces the three-frame ring (TMEM: acc1 + 3 x acc2 = 512 columns);
-//   * the residual x[t] is added by the epilogue from global memory (no identity tiles in shared memory);
-//   * E2 double-buffers its store staging.
-// Per frame the operand ring now carries only the three n1 frames of G1 (96 KB), and the tensor pipe is the bound:
-//   MMA  : G1(t)  G2s(t-1)  G1(t+1)  G2s(t) ...      E1(t) normalises frame t while G2s(t-1) / G1(t+1) run.
-// Warp roles: 0 producer, 1 G1 issuer (leader) / H forwarder (peer), 2 TMEM allocator + G2s issuer (leader), 3-10 E1, 11-18 E2.  Each epilogue group has
-// EIGHT warps -- lane quarter x 64-channel half -- because a group of four (one warp per scheduler) was the measured bound:
-// ncu showed ~65% of the frame period spent issuing the LayerNorm/SiLU arithmetic of one 128-channel row per thread.
-// ------------------------------------------------------------------------------------------------------------------
-constexpr int kWTile = 64 * 128;        // one resident weight tile: 64 rows (this CTA's half of N) x 64 bf16
-constexpr int kASlots = 3;
-constexpr int kEpi2 = 8;                     // warps per epilogue group (E1, E2): 4 lane quarters x 2 channel halves
-constexpr int kThreadsTb2 = (3 + 2 * kEpi2) * 32;
-
-struct Tb2Params {
-  int B, T, H, W;
-  int BW, BH;
-  int tilesW, tilesH;
-  long long num_strips;      // strips of 128 positions; a pair takes strips 2p and 2p+1
-  const float* bias1;
-  const float* bias2;
-  const float* g2;
-  const float* b2;
-  int ln_out, ln_out_silu;
-  const float* g3;
-  const float* b3;
-  int store_stream;
-  const bf16* x;             // residual, read by the epilogue: dense [B,T,H,W,128]
-};
-struct Tb2Maps {
-  CUtensorMap n1, w1, w2, o, o2;
-};
-
-// cluster-scope arrive / wait for the barrier that publishes the H tile of BOTH CTAs to the leader's MMA issuer
-__device__ __forceinline__ void mbar_arrive_remote_release(uint32_t bar, uint32_t rank) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\tmapa.shared::cluster.u32 ra, %0, %1;\n\tmbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}"
-      ::"r"(bar), "r"(rank) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity) {
-  const long long t0 = clock64();
-  for (;;) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
-    if (ok) return;
-    if (clock64() - t0 > 8000000000LL) __trap();
-  }
-}
-
-__global__ void __launch_bounds__(kThreadsTb2, 1) tblock2_tc_kernel(const __grid_constant__ Tb2Maps maps, const Tb2Params p) {
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int rank = (int)cluster_ctarank();                  // 0 = leader
-  // [resident W: 12 x 8 KB][H: kKc x 16 KB][A ring: kASlots x 16 KB][store staging: 8 warps x 4 KB][barriers][constants][LN partial sums]
-  const uint32_t w_base = smem_base;
-  const uint32_t h_base = w_base + 12u * kWTile;
-  const uint32_t a_base = h_base + kKc * kTile;
-  const uint32_t stg_base = a_base + kASlots * kTile;
-  const uint32_t bar_base = stg_base + (uint32_t)kEpi2 * 4096u;
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (kASlots + s); };
-  const uint32_t bar2 = bar_base + 16u * kASlots;
-  const uint32_t w_full = bar2;
-  const uint32_t a1_full = bar2 + 8, a1_empty = bar2 + 16, h_full = bar2 + 24, h_empty = bar2 + 32;
-  auto a2_full = [&](int s) { return bar2 + 40u + 8u * s; };
-  auto a2_empty = [&](int s) { return bar2 + 64u + 8u * s; };
-  const uint32_t tmem_slot = bar2 + 88u;
-  const uint32_t h_local = bar2 + 96u;
-  const uint32_t const_base = bar2 + 128u;
-  const uint32_t stat_base = const_base + 6u * kC * 4u;     // LayerNorm partial sums: [E1|E2][parity][half][128] float2
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(smem_gen + (tmem_slot - smem_base));
-  float* cst = reinterpret_cast<float*>(smem_gen + (const_base - smem_base));   // bias1 | g2 | b2 | bias2 | g3 | b3
-
-  for (int i = threadIdx.x; i < kC; i += kThreadsTb2) {
-    cst[i] = p.bias1 ? p.bias1[i] : 0.f;
-    cst[kC + i] = 0.5f * p.g2[i];          // SiLU in tanh form works on y/2
-    cst[2 * kC + i] = 0.5f * p.b2[i];
-    cst[3 * kC + i] = p.bias2 ? p.bias2[i] : 0.f;
-    const float sc = p.ln_out_silu ? 0.5f : 1.0f;
-    cst[4 * kC + i] = p.ln_out ? sc * p.g3[i] : 0.f;
-    cst[5 * kC + i] = p.ln_out ? sc * p.b3[i] : 0.f;
-  }
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&maps.n1); prefetch_tmap(&maps.w1); prefetch_tmap(&maps.w2); prefetch_tmap(&maps.o);
-    if (p.ln_out) prefetch_tmap(&maps.o2);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < kASlots; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-    mbar_init(w_full, 1);
-    mbar_init(a1_full, 1); mbar_init(a1_empty, 2 * kEpi2);     // E1 warps of both CTAs arrive on the leader's barrier
-    mbar_init(h_full, kEpi2 + 1); mbar_init(h_local, kEpi2); mbar_init(h_empty, 1);
-    for (int s = 0; s < 3; ++s) { mbar_init(a2_full(s), 1); mbar_init(a2_empty(s), 2 * kEpi2); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  constexpr uint32_t kTmemCols = 512;   // acc1 | acc2[3]
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(kTmemCols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
-
-  const long long pair0 = blockIdx.x >> 1, pair_step = gridDim.x >> 1;
-  const long long num_pairs = (p.num_strips + 1) / 2;
-  // strip of THIS CTA inside pair tile `pt`; a missing second strip (odd strip count) is placed at batch index B: its TMA
-  // boxes are out of bounds (zero fill on loads, nothing stored) and its epilogue rows are marked invalid
-  auto decode = [&](long long pt, int& b, int& h0, int& w0, bool& live) {
-    const long long strip = 2 * pt + rank;
-    live = strip < p.num_strips;
-    const long long sidx = live ? strip : 0;
-    const int tw = (int)(sidx % p.tilesW);
-    long long m = sidx / p.tilesW;
-    const int th = (int)(m % p.tilesH);
-    b = live ? (int)(m / p.tilesH) : p.B;
-    h0 = th * p.BH;
-    w0 = tw * p.BW;
+  // ===================== consumers =====================
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+  const int g = warp >> 2, wq = warp & 3;
+  const uint32_t hi = desc_hi(1024u);
+  float acc[kC / 2];
+  int stage = 0, pend_stage = -1;
+  uint32_t phase = 0;
+  auto release = [&]() {
+    if (lane == 0 && pend_stage >= 0) mbar_arrive(empty_bar(pend_stage));
+    pend_stage = -1;
   };
-  const int T = p.T;
+  // one K step (64 channels) of this warpgroup's 64 rows: A from the stage (G1) or from the H ring at h_addr (G2)
+  auto kstep = [&](bool a_from_stage, uint32_t h_addr, uint32_t scale) {
+    mbar_wait(full_bar(stage), phase);
+    const uint32_t sa = ring_base + stage * stage_bytes;
+    const uint32_t al = desc_lo(a_from_stage ? sa + (uint32_t)g * 64u * 128u : h_addr), bl = desc_lo(sa + kTile);
+    wgmma_fence();
+#pragma unroll
+    for (uint32_t j = 0; j < 4u; ++j) wgmma_k16<kC, false>(acc, desc(al + 2u * j, hi), desc(bl + 2u * j, hi), j == 0 ? scale : 1u);
+    wgmma_commit();
+    wgmma_wait<1>();
+    release();
+    pend_stage = stage;
+    if (++stage == p.stages) { stage = 0; phase ^= 1u; }
+  };
+  auto finish = [&]() {
+    wgmma_wait<0>();
+    acc_fence(acc);
+    release();
+  };
+  auto wg_sync = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(1 + g) : "memory"); };
+  const float* bias1 = cst;
+  const float* g2 = cst + kC;
+  const float* b2 = cst + 2 * kC;
+  const float* bias2 = cst + 3 * kC;
+  const float* g3 = cst + 4 * kC;
+  const float* b3 = cst + 5 * kC;
+  const int cq = 2 * (lane & 3);
+  const int rbase = 64 * g + 16 * wq + (lane >> 2);   // this thread's rows: rbase and rbase + 8
 
-  if (warp == 0) {
-    // ===================== TMA producer (both CTAs: own strip, own half of the weights) =====================
-    const bool el = elect_one();
-    if (el) {
-      if (rank == 0) mbar_expect_tx(w_full, 2u * 12u * kWTile);
-      for (int c = 0; c < 2; ++c)
-        for (int a = 0; a < 3; ++a)
-          for (int kc = 0; kc < kKc; ++kc)
-            tma_load_3d_2sm(w_base + (uint32_t)((c * 3 + a) * kKc + kc) * kWTile, c == 0 ? &maps.w1 : &maps.w2, w_full,
-                            a * kC + kc * 64, rank * 64, 0);
+  for (long long strip = blockIdx.x; strip < p.num_strips; strip += gridDim.x) {
+    const int tw = (int)(strip % p.tilesW);
+    const int th = (int)((strip / p.tilesW) % p.tilesH);
+    const int b = (int)(strip / ((long long)p.tilesW * p.tilesH));
+    long long pos0[2];   // position index (b, t = 0, h, w) of this thread's rows
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int row = rbase + 8 * r;
+      const int h = th * p.BH + row / p.BW, w = tw * p.BW + row % p.BW;
+      pos0[r] = (((long long)b * p.T) * p.H + h) * p.W + w;
     }
-    int slot = 0;
-    uint32_t phase = 0;
-    for (long long pt = pair0; pt < num_pairs; pt += pair_step) {
-      int b, h0, w0;
-      bool live;
-      decode(pt, b, h0, w0, live);
-      for (int t = 0; t < T; ++t) {
-        for (int a = 0; a < 3; ++a) {
-          const int tv = t - 2 + a;
-          if (tv < 0) continue;
-          for (int kc = 0; kc < kKc; ++kc) {
-            mbar_wait(empty_bar(slot), phase ^ 1u);
-            if (el) {
-              if (rank == 0) mbar_expect_tx(full_bar(slot), 2u * kTile);
-              tma_load_5d_2sm(a_base + slot * kTile, &maps.n1, full_bar(slot), kc * 64, w0, h0, tv, b);
-            }
-            if (++slot == kASlots) { slot = 0; phase ^= 1u; }
-          }
-        }
+    const long long frame = (long long)p.H * p.W;
+    for (int t = 0; t < p.T; ++t) {
+      // ---- G1(t)
+      uint32_t scale = 0;
+      for (int a = 0; a < 3; ++a) {
+        if (t - 2 + a < 0) continue;
+        for (int kc = 0; kc < kKc; ++kc) { kstep(true, 0u, scale); scale = 1; }
       }
-    }
-  } else if (warp == 1 || warp == 2) {
-    // ===================== MMA issuers (leader CTA): warp 1 = G1, warp 2 = G2s =====================
-    // Two issuing warps so that neither convolution's waits (operand ring for G1, the normalised H tile for G2s) sit in front
-    // of the other one's MMAs; the tensor pipe executes whatever has been issued, in order.
-    // In the peer CTA warp 1 forwards "my half of H is written" to the leader (see E1).
-    if (rank == 0) {
-      const bool el = elect_one();
-      const uint32_t idesc = make_idesc(kC, 256);
-      const uint32_t hi_d = 64u | (1u << 14) | (2u << 29);
-      auto desc_lo = [&](uint32_t addr) { return ((addr & 0x3FFFFu) >> 4) | 0x10000u; };
-      auto mma4 = [&](uint32_t d, uint32_t a_lo, uint32_t b_lo, uint32_t acc) {
+      finish();
+      // ---- E1(t): H[t mod 3] = bf16(silu(LN2(acc + b1))); statistics from fp32, normalisation of the bf16-rounded h
+      wg_sync();   // every warp of the group is past G2(t-1), which read the slot written here
+      const uint32_t slot = h_base + (uint32_t)(t % kHSlots) * kKc * kTile;
 #pragma unroll
-        for (uint32_t j = 0; j < 8u; j += 2u) umma_f16_2sm_lohi(d, a_lo + j, hi_d, b_lo + j, hi_d, idesc, j == 0 ? acc : 1u);
-      };
-      auto wres = [&](int c, int a, int kc) { return desc_lo(w_base + (uint32_t)((c * 3 + a) * kKc + kc) * kWTile); };
-      mbar_wait(w_full, 0);
-      tc_fence_after();
-      if (warp == 1) {
-        int slot = 0;
-        uint32_t phase = 0;
-        long long f1 = 0;            // global frame counter (barrier phases run across strips)
-        for (long long pt = pair0; pt < num_pairs; pt += pair_step) {
-          for (int t = 0; t < T; ++t, ++f1) {
-            mbar_wait(a1_empty, (uint32_t)((f1 & 1) ^ 1));
-            tc_fence_after();
-            uint32_t accum = 0;
-            for (int a = 0; a < 3; ++a) {
-              if (t - 2 + a < 0) continue;
-              for (int kc = 0; kc < kKc; ++kc) {
-                mbar_wait(full_bar(slot), phase);
-                tc_fence_after();
-                if (el) {
-                  mma4(tmem_base, desc_lo(a_base + slot * kTile), wres(0, a, kc), accum);
-                  umma_commit_2sm(empty_bar(slot));
-                }
-                accum = 1;
-                if (++slot == kASlots) { slot = 0; phase ^= 1u; }
-              }
-            }
-            if (el) umma_commit_2sm(a1_full);
-          }
-        }
-      } else {
-        long long f2 = 0;
-        for (long long pt = pair0; pt < num_pairs; pt += pair_step) {
-          // G2s(u): H[u] (just normalised) into the accumulators of frames u (tap 2), u+1 (tap 1), u+2 (tap 0)
-          for (int u = 0; u < T; ++u, ++f2) {
-            mbar_wait_cluster(h_full, (uint32_t)(f2 & 1));
-            tc_fence_after();
-            for (int j = 0; j < 3; ++j) {
-              if (u + j >= T) break;
-              const long long g = f2 + j;                       // global index of the target frame
-              const int as = (int)(g % 3);
-              const bool first = (j == 2) || (u == 0);          // first contribution to that frame's accumulator
-              if (first && g >= 3) {
-                mbar_wait(a2_empty(as), (uint32_t)(((g / 3) - 1) & 1));   // E2 has read the previous occupant (frame g-3)
-                tc_fence_after();
-              }
-              if (el) {
-                const uint32_t d = tmem_base + (uint32_t)kC + (uint32_t)as * kC;
-                for (int kc = 0; kc < kKc; ++kc) mma4(d, desc_lo(h_base + kc * kTile), wres(1, 2 - j, kc), (first && kc == 0) ? 0u : 1u);
-                if (j == 0) umma_commit_2sm(a2_full(as));       // frame u is complete
-              }
-            }
-            if (el) umma_commit_2sm(h_empty);
-          }
-        }
-      }
-    } else if (warp == 1) {
-      // peer CTA: its E1 warps arrive on the local h_local; ONE thread then publishes with cluster-scope release on the
-      // leader's h_full (eight release.cluster arrives straight from the E1 warps cost ~17% of the frame period each)
-      long long f = 0;
-      for (long long pt = pair0; pt < num_pairs; pt += pair_step)
-        for (int t = 0; t < T; ++t, ++f) {
-          mbar_wait(h_local, (uint32_t)(f & 1));
-          if (lane == 0) mbar_arrive_remote_release(h_full, 0);
-          __syncwarp();
-        }
-    }
-  } else if (warp >= 3 && warp < 3 + kEpi2) {
-    // ===================== E1: h = acc1 + b1 -> H = bf16(silu(LN2(h))) =====================
-    // 8 warps: warp & 3 picks the TMEM lane quarter (32 positions), hf the 64-channel half (= one K tile of H)
-    const int q = warp & 3;
-    const int hf = (warp - 3) >> 2;
-    const int rr = q * 32 + lane;
-    const int swz = lane & 7;
-    const float* bias1 = cst + hf * 64;
-    const float* gam = cst + kC + hf * 64;
-    const float* bet = cst + 2 * kC + hf * 64;
-    uint8_t* hrow = smem_gen + (h_base - smem_base) + (uint32_t)hf * kTile + (uint32_t)rr * 128u;
-    float2* st1 = reinterpret_cast<float2*>(smem_gen + (stat_base - smem_base));     // [parity][half][row]
-    long long f = 0;
-    for (long long pt = pair0; pt < num_pairs; pt += pair_step) {
-      for (int t = 0; t < T; ++t, ++f) {
-        mbar_wait(a1_full, (uint32_t)(f & 1));
-        tc_fence_after();
-        const uint32_t tb = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(hf * 64);
-        uint64_t lsum2 = 0ull, lsq2 = 0ull;
-        uint32_t keep[32];
+      for (int r = 0; r < 2; ++r) {
+        float s = 0.f, q = 0.f;
 #pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          uint32_t v[32];
-          tmem_ld32(tb + (uint32_t)(c * 32), v);
-          tmem_ld_wait();
-#pragma unroll
-          for (int g = 0; g < 8; ++g) {
-            const ulonglong2 bv = *reinterpret_cast<const ulonglong2*>(bias1 + c * 32 + g * 4);
-            const uint64_t a0 = add2(pk2(__uint_as_float(v[g * 4 + 0]), __uint_as_float(v[g * 4 + 1])), bv.x);
-            const uint64_t a1 = add2(pk2(__uint_as_float(v[g * 4 + 2]), __uint_as_float(v[g * 4 + 3])), bv.y);
-            lsum2 = add2(lsum2, add2(a0, a1));
-            lsq2 = fma2(a0, a0, lsq2);
-            lsq2 = fma2(a1, a1, lsq2);
-            float f0, f1, f2_, f3;
-            upk2(a0, f0, f1);
-            upk2(a1, f2_, f3);
-            keep[c * 16 + g * 2] = pack_bf16x2(f0, f1);
-            keep[c * 16 + g * 2 + 1] = pack_bf16x2(f2_, f3);
-          }
+        for (int j = 0; j < kC / 8; ++j) {
+          const int c = 8 * j + cq;
+          const float f0 = acc[4 * j + 2 * r] + bias1[c], f1 = acc[4 * j + 2 * r + 1] + bias1[c + 1];
+          s += f0 + f1;
+          q = fmaf(f0, f0, q);
+          q = fmaf(f1, f1, q);
+          const uint32_t kp = pack_bf16x2(f0, f1);
+          acc[4 * j + 2 * r] = bf16_lo(kp);
+          acc[4 * j + 2 * r + 1] = bf16_hi(kp);
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive_remote(a1_empty, 0);
-        float lsum, lsq;
-        {
-          float a, b;
-          upk2(lsum2, a, b); lsum = a + b;
-          upk2(lsq2, a, b); lsq = a + b;
-        }
-        // the other half of the row is held by the warp 4 above / below: exchange partial sums through shared memory
-        st1[((int)(f & 1) * 2 + hf) * 128 + rr] = make_float2(lsum, lsq);
-        asm volatile("bar.sync %0, 64;" ::"r"(1 + q) : "memory");    // the two warps of this lane quarter only
-        {
-          const float2 o2 = st1[((int)(f & 1) * 2 + (hf ^ 1)) * 128 + rr];
-          lsum += o2.x;
-          lsq += o2.y;
-        }
-        const float mean = lsum * (1.0f / kC);
-        float var = fmaf(-mean, mean, lsq * (1.0f / kC));
+        const float mean = quad_sum(s) * (1.0f / kC);
+        float var = fmaf(-mean, mean, quad_sum(q) * (1.0f / kC));
         var = var < 0.f ? 0.f : var;
         const float rstd = rsqrtf(var + 1e-6f);
         const float nmr = -mean * rstd;
-        const uint64_t rstd2 = pk2(rstd, rstd), nmr2 = pk2(nmr, nmr);
-        uint32_t o[32];
+        const int row = rbase + 8 * r;
+        uint8_t* hrow = smem_gen + (slot - smem_base) + row * 128;
 #pragma unroll
-        for (int w2 = 0; w2 < 16; ++w2) {   // 4 channels per step
-          const int ci = w2 * 4;
-          const ulonglong2 gv = *reinterpret_cast<const ulonglong2*>(gam + ci);
-          const ulonglong2 bv = *reinterpret_cast<const ulonglong2*>(bet + ci);
-          const uint32_t a2 = keep[ci / 2], b2 = keep[ci / 2 + 1];
-          uint64_t y0 = fma2(fma2(pk2(bf16_lo(a2), bf16_hi(a2)), rstd2, nmr2), gv.x, bv.x);
-          uint64_t y1 = fma2(fma2(pk2(bf16_lo(b2), bf16_hi(b2)), rstd2, nmr2), gv.y, bv.y);
-          float h0, h1, h2, h3;
-          upk2(y0, h0, h1);
-          upk2(y1, h2, h3);
-          y0 = fma2(y0, pk2(tanh_approx(h0), tanh_approx(h1)), y0);
-          y1 = fma2(y1, pk2(tanh_approx(h2), tanh_approx(h3)), y1);
-          float o0, o1, o2, o3;
-          upk2(y0, o0, o1);
-          upk2(y1, o2, o3);
-          o[ci / 2] = pack_bf16x2(o0, o1);
-          o[ci / 2 + 1] = pack_bf16x2(o2, o3);
+        for (int j = 0; j < kC / 8; ++j) {
+          const int c = 8 * j + cq;
+          float y0 = fmaf(fmaf(acc[4 * j + 2 * r], rstd, nmr), g2[c], b2[c]);
+          float y1 = fmaf(fmaf(acc[4 * j + 2 * r + 1], rstd, nmr), g2[c + 1], b2[c + 1]);
+          y0 = fmaf(y0, tanh_approx(y0), y0);
+          y1 = fmaf(y1, tanh_approx(y1), y1);
+          // canonical K-major SWIZZLE_128B: 16-byte unit u of row r lives at unit u ^ (r & 7)
+          const int cc = c & 63, u = cc >> 3;
+          *reinterpret_cast<uint32_t*>(hrow + (c >> 6) * kTile + ((u ^ (row & 7)) << 4) + (cc & 7) * 2) = pack_bf16x2(y0, y1);
         }
-        // the single H tile: free once G2s(f-1) has consumed the previous frame
-        if (f >= 1) mbar_wait(h_empty, (uint32_t)((f - 1) & 1));
-#pragma unroll
-        for (int g = 0; g < 8; ++g)
-          *reinterpret_cast<uint4*>(hrow + ((g ^ swz) << 4)) = make_uint4(o[g * 4], o[g * 4 + 1], o[g * 4 + 2], o[g * 4 + 3]);
-        fence_async_smem();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(rank == 0 ? h_full : h_local);
       }
-    }
-  } else if (warp >= 3 + kEpi2) {
-    // ===================== E2: out = acc2 + b2 + x (TMA store) [+ out2 = act(LN_next(out))] =====================
-    const int q = warp & 3;
-    const int hf = (warp - 3 - kEpi2) >> 2;
-    const int rr = q * 32 + lane;
-    const int swz = lane & 7;
-    const float* bias2 = cst + 3 * kC + hf * 64;
-    const float* gam = cst + 4 * kC + hf * 64;
-    const float* bet = cst + 5 * kC + hf * 64;
-    const uint32_t wstg = stg_base + (uint32_t)(warp - 3 - kEpi2) * 4096u;
-    uint8_t* wstg_gen = smem_gen + (wstg - smem_base);
-    float2* st2 = reinterpret_cast<float2*>(smem_gen + (stat_base - smem_base)) + 2 * 2 * 128;
-    const int row0 = q * 32;
-    const int qw0 = row0 % p.BW, qh0 = row0 / p.BW;
-    const int dw = rr % p.BW, dh = rr / p.BW;
-    long long f = 0;
-    for (long long pt = pair0; pt < num_pairs; pt += pair_step) {
-      int b, h0, w0;
-      bool live;
-      decode(pt, b, h0, w0, live);
-      const bf16* xrow0 = p.x + ((((long long)(live ? b : 0) * T) * p.H + (h0 + dh)) * p.W + (w0 + dw)) * kC + hf * 64;
-      const long long xframe = (long long)p.H * p.W * kC;
-      uint4 xv[8];
-      for (int t = 0; t < T; ++t, ++f) {
-        const int as = (int)(f % 3);
-        auto put64 = [&](const uint32_t* pk, const CUtensorMap* m) {
-          if (lane == 0) tma_store_wait_read();    // this warp's previous store has read the staging buffer
-          __syncwarp();
-          uint8_t* my = wstg_gen + (uint32_t)lane * 128u;
+      fence_async_smem();
+      wg_sync();
+      // ---- G2(t): A = this group's rows of the H ring
+      scale = 0;
+      for (int a = 0; a < 3; ++a) {
+        const int tv = t - 2 + a;
+        if (tv < 0) continue;
+        const uint32_t hs = h_base + (uint32_t)(tv % kHSlots) * kKc * kTile + (uint32_t)g * 64u * 128u;
+        for (int kc = 0; kc < kKc; ++kc) { kstep(false, hs + (uint32_t)kc * kTile, scale); scale = 1; }
+      }
+      finish();
+      // ---- E2(t): out = acc + b2 + x; out2 = act(LN_next(out)) from the bf16-rounded out
 #pragma unroll
-          for (int g = 0; g < 8; ++g)
-            *reinterpret_cast<uint4*>(my + ((g ^ swz) << 4)) = make_uint4(pk[4 * g], pk[4 * g + 1], pk[4 * g + 2], pk[4 * g + 3]);
-          fence_async_smem();
-          __syncwarp();
-          if (lane == 0) {
-            if (p.store_stream) tma_store_5d_stream(m, wstg, hf * 64, w0 + qw0, h0 + qh0, t, b);
-            else tma_store_5d(m, wstg, hf * 64, w0 + qw0, h0 + qh0, t, b);
-            tma_store_commit();
-          }
-        };
-        // residual (this thread's position, its 64 channels).  E2 is the slowest stage, so a load issued at the top of the
-        // frame is waited for in full (~2k cycles at 3 TB/s of DRAM traffic): the rows of frame t+1 are requested as soon as
-        // the registers of frame t are free (below), and only the first frame of a strip is loaded here
-        if (t == 0) {
+      for (int r = 0; r < 2; ++r) {
+        const long long off = (pos0[r] + (long long)t * frame) * kC;
+        const bf16* xr = p.x + off;
+        bf16* orow = p.out + off;
+        float s = 0.f, q = 0.f;
 #pragma unroll
-          for (int k = 0; k < 8; ++k) xv[k] = live ? __ldg(reinterpret_cast<const uint4*>(xrow0) + k) : make_uint4(0, 0, 0, 0);
+        for (int j = 0; j < kC / 8; ++j) {
+          const int c = 8 * j + cq;
+          const uint32_t xw = *reinterpret_cast<const uint32_t*>(xr + c);
+          const float f0 = acc[4 * j + 2 * r] + bias2[c] + bf16_lo(xw), f1 = acc[4 * j + 2 * r + 1] + bias2[c + 1] + bf16_hi(xw);
+          s += f0 + f1;
+          q = fmaf(f0, f0, q);
+          q = fmaf(f1, f1, q);
+          const uint32_t kp = pack_bf16x2(f0, f1);
+          *reinterpret_cast<uint32_t*>(orow + c) = kp;
+          acc[4 * j + 2 * r] = bf16_lo(kp);
+          acc[4 * j + 2 * r + 1] = bf16_hi(kp);
         }
-        mbar_wait(a2_full(as), (uint32_t)((f / 3) & 1));
-        tc_fence_after();
-        const uint32_t tb = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)kC + (uint32_t)as * kC + (uint32_t)(hf * 64);
-        uint64_t lsum2 = 0ull, lsq2 = 0ull;
-        uint32_t keep[32];
+        if (!p.ln_out) continue;
+        const float mean = quad_sum(s) * (1.0f / kC);
+        float var = fmaf(-mean, mean, quad_sum(q) * (1.0f / kC));
+        var = var < 0.f ? 0.f : var;
+        const float rstd = rsqrtf(var + 1e-6f);
+        const float nmr = -mean * rstd;
+        bf16* o2 = p.out2 + off;
 #pragma unroll
-        for (int hc = 0; hc < 2; ++hc) {
-          uint32_t v[32];
-          tmem_ld32(tb + (uint32_t)(hc * 32), v);
-          tmem_ld_wait();
-#pragma unroll
-          for (int g = 0; g < 4; ++g) {   // 8 channels per step: one 16-byte residual load
-            float rv[8];
-            unpack8(xv[hc * 4 + g], rv);
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              const ulonglong2 bv = *reinterpret_cast<const ulonglong2*>(bias2 + hc * 32 + g * 8 + h * 4);
-              uint64_t a0 = add2(pk2(__uint_as_float(v[g * 8 + h * 4 + 0]), __uint_as_float(v[g * 8 + h * 4 + 1])), bv.x);
-              uint64_t a1 = add2(pk2(__uint_as_float(v[g * 8 + h * 4 + 2]), __uint_as_float(v[g * 8 + h * 4 + 3])), bv.y);
-              a0 = add2(a0, pk2(rv[h * 4 + 0], rv[h * 4 + 1]));
-              a1 = add2(a1, pk2(rv[h * 4 + 2], rv[h * 4 + 3]));
-              if (p.ln_out) {
-                lsum2 = add2(lsum2, add2(a0, a1));
-                lsq2 = fma2(a0, a0, lsq2);
-                lsq2 = fma2(a1, a1, lsq2);
-              }
-              float f0, f1, f2_, f3;
-              upk2(a0, f0, f1);
-              upk2(a1, f2_, f3);
-              keep[hc * 16 + g * 4 + h * 2] = pack_bf16x2(f0, f1);
-              keep[hc * 16 + g * 4 + h * 2 + 1] = pack_bf16x2(f2_, f3);
-            }
+        for (int j = 0; j < kC / 8; ++j) {
+          const int c = 8 * j + cq;
+          float y0 = fmaf(fmaf(acc[4 * j + 2 * r], rstd, nmr), g3[c], b3[c]);
+          float y1 = fmaf(fmaf(acc[4 * j + 2 * r + 1], rstd, nmr), g3[c + 1], b3[c + 1]);
+          if (p.ln_out_silu) {
+            y0 = fmaf(y0, tanh_approx(y0), y0);
+            y1 = fmaf(y1, tanh_approx(y1), y1);
           }
-        }
-        tc_fence_before();     // the accumulator slice has been read completely
-        __syncwarp();
-        if (lane == 0) mbar_arrive_remote(a2_empty(as), 0);
-        float lsum = 0.f, lsq = 0.f;
-        if (p.ln_out) {   // partial sums out first: the partner's arrive at the barrier below hides behind the store of `out`
-          float a, b2_;
-          upk2(lsum2, a, b2_); lsum = a + b2_;
-          upk2(lsq2, a, b2_); lsq = a + b2_;
-          st2[((int)(f & 1) * 2 + hf) * 128 + rr] = make_float2(lsum, lsq);
-        }
-        if (t + 1 < T) {
-          const bf16* xr = xrow0 + (long long)(t + 1) * xframe;
-#pragma unroll
-          for (int k = 0; k < 8; ++k) xv[k] = live ? __ldg(reinterpret_cast<const uint4*>(xr) + k) : make_uint4(0, 0, 0, 0);
-        }
-        put64(keep, &maps.o);
-        if (p.ln_out) {
-          asm volatile("bar.sync %0, 64;" ::"r"(5 + q) : "memory");
-          {
-            const float2 o2 = st2[((int)(f & 1) * 2 + (hf ^ 1)) * 128 + rr];
-            lsum += o2.x;
-            lsq += o2.y;
-          }
-          const float mean = lsum * (1.0f / kC);
-          float var = fmaf(-mean, mean, lsq * (1.0f / kC));
-          var = var < 0.f ? 0.f : var;
-          const float rstd = rsqrtf(var + 1e-6f);
-          const float nmr = -mean * rstd;
-          const uint64_t rstd2 = pk2(rstd, rstd), nmr2 = pk2(nmr, nmr);
-          uint32_t o[32];
-#pragma unroll
-          for (int g = 0; g < 16; ++g) {
-            const ulonglong2 gv = *reinterpret_cast<const ulonglong2*>(gam + g * 4);
-            const ulonglong2 bv = *reinterpret_cast<const ulonglong2*>(bet + g * 4);
-            const uint32_t a2 = keep[2 * g], b2 = keep[2 * g + 1];
-            uint64_t y0 = fma2(fma2(pk2(bf16_lo(a2), bf16_hi(a2)), rstd2, nmr2), gv.x, bv.x);
-            uint64_t y1 = fma2(fma2(pk2(bf16_lo(b2), bf16_hi(b2)), rstd2, nmr2), gv.y, bv.y);
-            if (p.ln_out_silu) {
-              float h0_, h1, h2, h3;
-              upk2(y0, h0_, h1);
-              upk2(y1, h2, h3);
-              y0 = fma2(y0, pk2(tanh_approx(h0_), tanh_approx(h1)), y0);
-              y1 = fma2(y1, pk2(tanh_approx(h2), tanh_approx(h3)), y1);
-            }
-            float o0, o1, o2, o3;
-            upk2(y0, o0, o1);
-            upk2(y1, o2, o3);
-            o[2 * g] = pack_bf16x2(o0, o1);
-            o[2 * g + 1] = pack_bf16x2(o2, o3);
-          }
-          put64(o, &maps.o2);
+          *reinterpret_cast<uint32_t*>(o2 + c) = pack_bf16x2(y0, y1);
         }
       }
     }
-    if (lane == 0) tma_store_wait_all();
   }
-
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kTmemCols) : "memory");
-  }
-}
-
-__global__ void fill_identity256_kernel(bf16* e) {
-  const int r = blockIdx.x, c = threadIdx.x;
-  e[r * 256 + c] = __float2bfloat16_rn(r == c ? 1.0f : 0.0f);
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -965,119 +301,32 @@ EncodeTiledFn tb_get_encode() {
   static bool tried = false;
   if (!tried) {
     tried = true;
-    void* p = nullptr;
+    void* f = nullptr;
     cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-      fn = (EncodeTiledFn)p;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
+      fn = (EncodeTiledFn)f;
   }
   return fn;
 }
 
-thread_local std::string g_tb_err;
-
-// VT_TBLOCK: 0 = off (two conv_tc launches per block), 1 = version 1 (single CTA, streamed weights), 2 = version 2 (CTA
-// pairs, resident weights; default)
-int tblock_variant() {
-  static int env = -1;
-  if (env < 0) { const char* e = getenv("VT_TBLOCK"); env = e ? atoi(e) : 2; }
-  return env;
-}
-
+// strip box of 128 positions that tiles H x W exactly: the widest power-of-two BW <= 128 dividing W, BH = 128 / BW
 bool strip_box(int H, int W, int& BW, int& BH) {
-  BW = 128;
-  while (BW > 1 && (BW > W || W % BW != 0)) BW >>= 1;
-  if (BW < 8) return false;
-  BH = 128 / BW;
-  return H % BH == 0 && BH <= 256;
-}
-
-cudaError_t launch_tblock2(const bf16* n1, const bf16* x, const bf16* w1, const float* bias1, const float* gamma2, const float* beta2,
-                           const bf16* w2, const float* bias2, bf16* out, bf16* out2, const float* gamma_out, const float* beta_out,
-                           bool out_silu, int B, int T, int H, int W, cudaStream_t s) {
-  EncodeTiledFn enc = tb_get_encode();
-  if (!enc) { g_tb_err = "cuTensorMapEncodeTiled unavailable"; return cudaErrorNotSupported; }
-  Tb2Params p;
-  memset(&p, 0, sizeof(p));
-  if (!strip_box(H, W, p.BW, p.BH)) { g_tb_err = "H x W not tileable"; return cudaErrorInvalidValue; }
-  p.B = B; p.T = T; p.H = H; p.W = W;
-  p.tilesW = W / p.BW; p.tilesH = H / p.BH;
-  p.num_strips = (long long)B * p.tilesH * p.tilesW;
-  p.bias1 = bias1; p.bias2 = bias2; p.g2 = gamma2; p.b2 = beta2;
-  p.ln_out = (out2 && gamma_out && beta_out) ? 1 : 0;
-  p.ln_out_silu = out_silu ? 1 : 0;
-  p.g3 = gamma_out; p.b3 = beta_out;
-  p.store_stream = ((double)B * T * H * W * kC * 2.0 > 256e6) ? 1 : 0;
-  p.x = x;
-  const size_t smem = 1024 + 12 * (size_t)kWTile + (size_t)kKc * kTile + (size_t)kASlots * kTile + (size_t)kEpi2 * 4096 + 16 * kASlots + 128 + 6 * kC * 4 +
-                      2 * 2 * 2 * 128 * 8 + 256;
-  Tb2Maps maps;
-  auto enc_act = [&](CUtensorMap* m, const void* base, int bw, int bh) -> bool {
-    cuuint64_t dims[5] = {(cuuint64_t)kC, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)T, (cuuint64_t)B};
-    cuuint64_t strides[4] = {(cuuint64_t)kC * 2, (cuuint64_t)W * kC * 2, (cuuint64_t)H * W * kC * 2, (cuuint64_t)T * H * W * kC * 2};
-    cuuint32_t box[5] = {64, (cuuint32_t)bw, (cuuint32_t)bh, 1, 1};
-    cuuint32_t es[5] = {1, 1, 1, 1, 1};
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, const_cast<void*>(base), dims, strides, box, es,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { g_tb_err = "cuTensorMapEncodeTiled(activation) failed: " + std::to_string((int)r); return false; }
-    return true;
-  };
-  auto enc_w = [&](CUtensorMap* m, const void* base) -> bool {   // [128][3*128] bf16, box = 64 channels x 64 rows (one CTA's half of N)
-    cuuint64_t dims[3] = {(cuuint64_t)(3 * kC), (cuuint64_t)kC, 1};
-    cuuint64_t strides[2] = {(cuuint64_t)(3 * kC) * 2, (cuuint64_t)(3 * kC) * kC * 2};
-    cuuint32_t box[3] = {64, 64, 1};
-    cuuint32_t es[3] = {1, 1, 1};
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(base), dims, strides, box, es,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { g_tb_err = "cuTensorMapEncodeTiled(weights) failed: " + std::to_string((int)r); return false; }
-    return true;
-  };
-  static bool attr_set[64] = {false};
-  static int sms[64] = {0};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev < 0 || dev >= 64) { g_tb_err = "device index out of range"; return cudaErrorInvalidValue; }
-  if (!attr_set[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(tblock2_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
-    if (e != cudaSuccess) { g_tb_err = "cudaFuncSetAttribute(smem)"; return e; }
-    attr_set[dev] = true;
-    cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, dev);
-    if (sms[dev] <= 0) sms[dev] = 148;
+  for (int bw = 128; bw >= 1; bw >>= 1) {
+    if (W % bw != 0) continue;
+    const int bh = 128 / bw;
+    if (bh <= 256 && H % bh == 0) { BW = bw; BH = bh; return true; }
   }
-  const int qw = p.BW < 32 ? p.BW : 32, qh = 32 / qw;
-  if (!enc_act(&maps.n1, n1, p.BW, p.BH) || !enc_act(&maps.o, out, qw, qh)) return cudaErrorInvalidValue;
-  maps.o2 = maps.o;
-  if (p.ln_out && !enc_act(&maps.o2, out2, qw, qh)) return cudaErrorInvalidValue;
-  if (!enc_w(&maps.w1, w1) || !enc_w(&maps.w2, w2)) return cudaErrorInvalidValue;
-  const long long num_pairs = (p.num_strips + 1) / 2, max_pairs = sms[dev] / 2;
-  const unsigned grid = 2u * (unsigned)(num_pairs < max_pairs ? num_pairs : max_pairs);
-  const double M = (double)B * T * H * W;
-  char det[96] = "";
-  if (prof_enabled()) snprintf(det, sizeof(det), "2x k311 %d->%d @%dx%dx%d strip%dx%d pair%s", kC, kC, T, H, W, p.BH, p.BW, p.ln_out ? " ln" : "");
-  ProfScope _ps("tblock_tc", 2.0 * 2.0 * M * 3 * kC * kC, 2.0 * M * kC * (3.0 + (p.ln_out ? 1.0 : 0.0)), s, det);
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(kThreadsTb2);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, tblock2_tc_kernel, maps, p);
-  count_launch();
-  return e != cudaSuccess ? e : cudaGetLastError();
+  return false;
 }
-
 }  // namespace
 
 const char* tblock_tc_last_error() { return g_tb_err.c_str(); }
 
 bool tblock_tc_supported(int B, int T, int H, int W, int C, bool planning) {
   g_tb_err.clear();
-  if (!tblock_variant()) { g_tb_err = "disabled (VT_TBLOCK=0)"; return false; }
+  static int env = -1;   // VT_TBLOCK=0: the model runs the block as two conv_tc launches instead (measurement knob)
+  if (env < 0) { const char* e = getenv("VT_TBLOCK"); env = e ? atoi(e) : 1; }
+  if (!env) { g_tb_err = "disabled (VT_TBLOCK=0)"; return false; }
   if (C != kC) { g_tb_err = "C != 128"; return false; }
   if (B <= 0 || T <= 0) { g_tb_err = "empty"; return false; }
   int BW, BH;
@@ -1092,8 +341,7 @@ cudaError_t launch_tblock_tc(const bf16* n1, const bf16* x, const bf16* w1, cons
                              const float* beta2, const bf16* w2, const float* bias2, bf16* out, bf16* out2,
                              const float* gamma_out, const float* beta_out, bool out_silu, int B, int T, int H, int W,
                              cudaStream_t s) {
-  if (tblock_variant() >= 2)
-    return launch_tblock2(n1, x, w1, bias1, gamma2, beta2, w2, bias2, out, out2, gamma_out, beta_out, out_silu, B, T, H, W, s);
+  g_tb_err.clear();
   EncodeTiledFn enc = tb_get_encode();
   if (!enc) { g_tb_err = "cuTensorMapEncodeTiled unavailable"; return cudaErrorNotSupported; }
   TbParams p;
@@ -1106,65 +354,49 @@ cudaError_t launch_tblock_tc(const bf16* n1, const bf16* x, const bf16* w1, cons
   p.ln_out = (out2 && gamma_out && beta_out) ? 1 : 0;
   p.ln_out_silu = out_silu ? 1 : 0;
   p.g3 = gamma_out; p.b3 = beta_out;
-  p.store_stream = ((double)B * T * H * W * kC * 2.0 > 256e6) ? 1 : 0;
-  const size_t fixed = 1024 + (size_t)kHSlots * kKc * kTile + 4 * 4096 + 8 * 14 + 16 + 6 * kC * 4 + 256;
-  int stages = (int)((222 * 1024 - fixed) / (2 * kTile + 16));
-  if (stages > 6) stages = 6;
-  if (stages < 2) { g_tb_err = "not enough shared memory"; return cudaErrorInvalidValue; }
+  p.x = x; p.out = out; p.out2 = out2;
+  const size_t fixed = 1024 + (size_t)kHSlots * kKc * kTile + 6 * kC * 4;
+  const size_t budget = 225 * 1024;
+  int stages = (int)((budget - fixed) / (2 * kTile + 16));
+  if (stages > 4) stages = 4;
   p.stages = stages;
   const size_t smem = fixed + (size_t)stages * (2 * kTile + 16);
-
   TbMaps maps;
-  auto enc_act = [&](CUtensorMap* m, const void* base, int bw, int bh) -> bool {
+  {
     cuuint64_t dims[5] = {(cuuint64_t)kC, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)T, (cuuint64_t)B};
     cuuint64_t strides[4] = {(cuuint64_t)kC * 2, (cuuint64_t)W * kC * 2, (cuuint64_t)H * W * kC * 2, (cuuint64_t)T * H * W * kC * 2};
-    cuuint32_t box[5] = {64, (cuuint32_t)bw, (cuuint32_t)bh, 1, 1};
+    cuuint32_t box[5] = {64, (cuuint32_t)p.BW, (cuuint32_t)p.BH, 1, 1};
     cuuint32_t es[5] = {1, 1, 1, 1, 1};
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, const_cast<void*>(base), dims, strides, box, es,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { g_tb_err = "cuTensorMapEncodeTiled(activation) failed: " + std::to_string((int)r); return false; }
-    return true;
-  };
-  auto enc_w = [&](CUtensorMap* m, const void* base, int K, int rows) -> bool {
-    cuuint64_t dims[3] = {(cuuint64_t)K, (cuuint64_t)rows, 1};
-    cuuint64_t strides[2] = {(cuuint64_t)K * 2, (cuuint64_t)K * rows * 2};
+    CUresult r = enc(&maps.n1, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, const_cast<bf16*>(n1), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) { g_tb_err = "cuTensorMapEncodeTiled(n1) failed: " + std::to_string((int)r); return cudaErrorInvalidValue; }
+  }
+  for (int i = 0; i < 2; ++i) {
+    cuuint64_t dims[3] = {(cuuint64_t)(3 * kC), (cuuint64_t)kC, 1};
+    cuuint64_t strides[2] = {(cuuint64_t)(3 * kC) * 2, (cuuint64_t)(3 * kC) * kC * 2};
     cuuint32_t box[3] = {64, (cuuint32_t)kC, 1};
     cuuint32_t es[3] = {1, 1, 1};
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(base), dims, strides, box, es,
+    CUresult r = enc(i ? &maps.w2 : &maps.w1, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<bf16*>(i ? w2 : w1), dims, strides, box, es,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { g_tb_err = "cuTensorMapEncodeTiled(weights) failed: " + std::to_string((int)r); return false; }
-    return true;
-  };
-  static bf16* ident_dev[64] = {nullptr};   // 256 x 256 identity, built once per device on the launching stream
-  static bool attr_set[64] = {false};
+    if (r != CUDA_SUCCESS) { g_tb_err = "cuTensorMapEncodeTiled(weights) failed: " + std::to_string((int)r); return cudaErrorInvalidValue; }
+  }
+  static bool attr[64] = {false};
   static int sms[64] = {0};
   int dev = 0;
   cudaGetDevice(&dev);
-  if (dev < 0 || dev >= 64) { g_tb_err = "device index out of range"; return cudaErrorInvalidValue; }
-  if (!ident_dev[dev]) {
-    cudaError_t e = cudaMalloc(&ident_dev[dev], 256 * 256 * sizeof(bf16));
-    if (e != cudaSuccess) { g_tb_err = "cudaMalloc(identity)"; return e; }
-    fill_identity256_kernel<<<256, 256, 0, s>>>(ident_dev[dev]);
-  }
-  if (!attr_set[dev]) {
+  if (dev < 0 || dev >= 64) return cudaErrorInvalidDevice;
+  if (!attr[dev]) {
     cudaError_t e = cudaFuncSetAttribute(tblock_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
     if (e != cudaSuccess) { g_tb_err = "cudaFuncSetAttribute(smem)"; return e; }
-    attr_set[dev] = true;
+    attr[dev] = true;
     cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, dev);
-    if (sms[dev] <= 0) sms[dev] = 148;
+    if (sms[dev] <= 0) sms[dev] = 132;
   }
-  const int qw = p.BW < 32 ? p.BW : 32, qh = 32 / qw;
-  if (!enc_act(&maps.n1, n1, p.BW, p.BH) || !enc_act(&maps.x, x, p.BW, p.BH) || !enc_act(&maps.o, out, qw, qh)) return cudaErrorInvalidValue;
-  maps.o2 = maps.o;
-  if (p.ln_out && !enc_act(&maps.o2, out2, qw, qh)) return cudaErrorInvalidValue;
-  if (!enc_w(&maps.w1, w1, 3 * kC, kC) || !enc_w(&maps.w2, w2, 3 * kC, kC) || !enc_w(&maps.e, ident_dev[dev], 256, 256)) return cudaErrorInvalidValue;
-
   const unsigned grid = (unsigned)(p.num_strips < sms[dev] ? p.num_strips : sms[dev]);
   const double M = (double)B * T * H * W;
   char det[96] = "";
-  if (prof_enabled()) snprintf(det, sizeof(det), "2x k311 %d->%d @%dx%dx%d strip%dx%d st%d%s", kC, kC, T, H, W, p.BH, p.BW, stages, p.ln_out ? " ln" : "");
+  if (prof_enabled()) snprintf(det, sizeof(det), "strip %dx%d T%d ln_out%d", p.BH, p.BW, T, p.ln_out);
   ProfScope _ps("tblock_tc", 2.0 * 2.0 * M * 3 * kC * kC, 2.0 * M * kC * (3.0 + (p.ln_out ? 1.0 : 0.0)), s, det);
   tblock_tc_kernel<<<grid, kThreadsTb, smem, s>>>(maps, p);
   count_launch();

@@ -5,14 +5,14 @@ Same class names, constructor kwargs, attributes, state-dict keys and return con
   vidtok/models/autoencoder_v1_1.py:98-342       (AutoencodingEngine with temporal tiling, v1.1)
   vidtok/modules/model_3dcausal[_v1_1].py        (EncoderCausal3DPadding / DecoderCausal3DPadding)
   vidtok/modules/regularizers.py:74-268          (DiagonalGaussianRegularizer / FSQRegularizer)
-but every tensor operation runs in libvidtok_b200.so (hand-written sm_100a kernels) through the C ABI of
+but every tensor operation runs in libvidtok_b200.so (hand-written sm_90a kernels) through the C ABI of
 include/vidtok_b200.h.  There is no PyTorch/CPU fallback: a model that is not on a CUDA device raises.
 
 Precision: the reference scripts run fp32 by default and bf16/fp16 under `--precision autocast`
 (scripts/inference_evaluate.py:77-79,137).  Mirroring that, `model.precision = None` (default) selects
-  * "exact"  -- fp32-class results on the tcgen05 tensor cores (fp16 hi|lo split operands x 3 MMAs, fp32 LayerNorm/SiLU): the
+  * "exact"  -- fp32-class results on the tensor cores (wgmma) (fp16 hi|lo split operands x 3 MMAs, fp32 LayerNorm/SiLU): the
                 parity mode (1e-3 max-abs, FSQ codes equal), unless
-  * "bf16"   -- torch.autocast is active (bf16 activations/weights on tcgen05, fp32 accumulate: the throughput mode;
+  * "bf16"   -- torch.autocast is active (bf16 activations/weights on wgmma, fp32 accumulate: the throughput mode;
                 outputs are returned in the autocast dtype like the reference's; an fp16 autocast region also
                 computes in bf16).
 Explicit settings: "exact", "bf16", "mixed" (encoder exact, decoder bf16: bit-exact FSQ codes / 1e-3 latents with a
