@@ -1,53 +1,40 @@
-"""SASS evidence: per kernel of libvidtok_b200.so, the count of tensor-core / TMA / TMEM instructions (cuobjdump -sass).
-  python tools/sass_summary.py [round-tag]  ->  profiles/sass_<tag>.txt
-Mnemonics (B200_PROFILING.md): UTCHMMA = tcgen05.mma kind::f16, UTCBAR = tcgen05.commit, LDTM = tcgen05.ld, UTMALDG / UTMASTG =
-TMA tensor load / store (cp.async.bulk.tensor), UTCATOMSWS / ... = TMEM alloc, SYNCS = mbarrier ops."""
+"""SASS evidence: per kernel of libvidtok_b200.so (sm_90a), the count of tensor-core / TMA / barrier instructions.
+  python tools/sass_summary.py OUT_DIR [LIB]  ->  OUT_DIR/sass_summary.txt
+LIB defaults to the in-tree vidtok_b200/libvidtok_b200.so.  Mnemonics (vidtok_b200/sass.py): HGMMA = wgmma.mma_async,
+HGMMA_WAIT = those of them that carry the gsb0 scoreboard (a pipelined main loop has fewer of these than HGMMAs),
+WARPGROUP.ARRIVE / DEPBAR = wgmma.fence / wait_group, UTMALDG / UTMASTG = TMA tensor load / store, SYNCS = mbarrier."""
 import os
-import re
-import subprocess
 import sys
-from collections import OrderedDict
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-tag = sys.argv[1] if len(sys.argv) > 1 else "r2"
-lib = os.path.join(ROOT, "vidtok_b200", "libvidtok_b200.so")
-sass = subprocess.run(["cuobjdump", "-sass", lib], capture_output=True, text=True).stdout
-WATCH = ["UTCHMMA", "UTCQMMA", "UTCBAR", "LDTM", "STTM", "UTMALDG", "UTMASTG", "UTMAPF", "UTCATOMSWS", "SYNCS", "HMMA", "FFMA2", "FFMA", "MUFU", "LDG", "STG", "BAR"]
-kernels = OrderedDict()
-cur = None
-for line in sass.splitlines():
-    m = re.match(r"\s*Function : (\S+)", line)
-    if m:
-        cur = m.group(1)
-        kernels[cur] = {"n": 0, "first": {}}
-        continue
-    if cur is None:
-        continue
-    m = re.match(r"\s*/\*[0-9a-f]+\*/\s+(?:@!?U?P\d+\s+)?([A-Z0-9_.]+)", line)
-    if not m:
-        continue
-    op = m.group(1)
-    k = kernels[cur]
-    k["n"] += 1
-    base = op.split(".")[0]
-    for w in WATCH:
-        if base == w:
-            k[w] = k.get(w, 0) + 1
-            if w not in k["first"]:
-                k["first"][w] = line.strip()
-            break
-demangle = subprocess.run(["c++filt"], input="\n".join(kernels), capture_output=True, text=True).stdout.splitlines()
-out = os.path.join(ROOT, "profiles", f"sass_{tag}.txt")
-with open(out, "w") as f:
-    f.write(f"# cuobjdump -sass vidtok_b200/libvidtok_b200.so (sm_100a), instruction counts per kernel -- round {tag}\n")
-    f.write("# UTCHMMA = tcgen05.mma.kind::f16, UTCBAR = tcgen05.commit, LDTM = tcgen05.ld, UTMALDG/UTMASTG = TMA tensor load/store,\n# SYNCS = mbarrier, FFMA2 = packed fp32x2 FMA.\n\n")
-    for (mang, k), name in zip(kernels.items(), demangle):
-        name = re.sub(r"\(anonymous namespace\)::", "", name)
-        name = name.split("(")[0] if not name.startswith("void") else name[5:].split("(")[0]
-        counts = "  ".join(f"{w}={k[w]}" for w in WATCH if w in k)
-        f.write(f"{name}\n    {k['n']} instructions   {counts}\n")
-        for w in ("UTCHMMA", "UTMALDG", "UTMASTG", "LDTM"):
-            if w in k["first"]:
-                f.write(f"      e.g. {k['first'][w]}\n")
-        f.write("\n")
-print("wrote", out, len(kernels), "kernels")
+sys.path.insert(0, ROOT)
+from vidtok_b200 import sass  # noqa: E402
+
+
+def main():
+    if len(sys.argv) < 2:
+        sys.exit(__doc__)
+    out_dir = sys.argv[1]
+    lib = sys.argv[2] if len(sys.argv) > 2 else os.path.join(ROOT, "vidtok_b200", "libvidtok_b200.so")
+    kernels = sass.kernel_counts(sass.disassemble(lib))
+    serialized = set(sass.serialized_wgmma_kernels(kernels))
+    os.makedirs(out_dir, exist_ok=True)
+    out = os.path.join(out_dir, "sass_summary.txt")
+    with open(out, "w") as f:
+        f.write(f"# cuobjdump -sass {os.path.basename(lib)} (sm_90a), instruction counts per kernel\n")
+        f.write("# HGMMA = wgmma.mma_async, HGMMA_WAIT = HGMMA with the gsb0 scoreboard, WARPGROUP.ARRIVE/DEPBAR = wgmma fence / "
+                "wait_group,\n# UTMALDG/UTMASTG = TMA tensor load/store, SYNCS = mbarrier.\n\n")
+        for (mang, k), name in zip(kernels.items(), sass.demangle(kernels)):
+            counts = "  ".join(f"{w}={k[w]}" for w in sass.WATCH if w in k)
+            f.write(f"{name}\n    {k['n']} instructions   {counts}\n")
+            if mang in serialized:
+                f.write("    SERIALIZED: every HGMMA waits for the previous one\n")
+            for w in ("HGMMA", "UTMALDG", "UTMASTG"):
+                if w in k["first"]:
+                    f.write(f"      e.g. {k['first'][w]}\n")
+            f.write("\n")
+    print("wrote", out, len(kernels), "kernels,", len(serialized), "with serialized wgmma")
+
+
+if __name__ == "__main__":
+    main()

@@ -3,9 +3,15 @@
 from __future__ import annotations
 
 import os
+import re
 import shutil
 import subprocess
 from concurrent.futures import ThreadPoolExecutor
+
+try:
+    from . import sass
+except ImportError:   # run as a script: python vidtok_b200/build.py
+    import sass
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
@@ -14,8 +20,19 @@ LIB = os.path.join(HERE, "libvidtok_b200.so")
 SOURCES = ["conv_simt.cu", "conv_tc.cu", "conv_stem.cu", "tblock_tc.cu", "elementwise.cu", "model.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
-    "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
+    "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v",
 ]
+# ptxas's "Potential Performance Loss" notes of the C751x family: it had to wait for every wgmma.mma_async before issuing
+# the next one, so a kernel's main loop runs with a single MMA in flight.  That costs tensor-pipe throughput without
+# changing any result, so nothing else would notice it: the build refuses it instead.
+_WGMMA_SERIALIZED = re.compile(r"\((C75\d\d)\) Potential Performance Loss: wgmma\.mma_async instructions are serialized (.*?)"
+                               r"(?: in| for) the function '([^']+)'")
+
+
+def _serialized_wgmma(ptxas_log: str) -> list:
+    hits = _WGMMA_SERIALIZED.findall(ptxas_log)
+    names = sass.demangle(h[2] for h in hits)
+    return [f"{name}: {code} serialized {why.strip()}" for (code, why, _), name in zip(hits, names)]
 
 
 def _nvcc() -> str:
@@ -48,10 +65,17 @@ def build(force: bool = False, verbose: bool = False) -> str:
             raise RuntimeError(f"nvcc failed for {src}:\n{r.stdout}\n{r.stderr}")
         if verbose and r.stderr:
             print(r.stderr)
+        bad = _serialized_wgmma(r.stderr)
+        if bad:
+            os.remove(obj)   # an object that was refused must not pass the next build's freshness check
+            serialized.extend(f"{os.path.basename(src)}: {b}" for b in bad)
         return obj
 
+    serialized = []
     with ThreadPoolExecutor(max_workers=len(srcs)) as ex:
         objs = list(ex.map(compile_one, srcs))
+    if serialized:
+        raise RuntimeError("ptxas serialized the wgmma pipeline of:\n  " + "\n  ".join(serialized))
     cmd = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB] + objs
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:

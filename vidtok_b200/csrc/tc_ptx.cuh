@@ -315,8 +315,12 @@ __device__ __forceinline__ void unpack8h(const uint4& u, float (&f)[8]) {
     f[2 * i + 1] = v.y;
   }
 }
-__device__ __forceinline__ float bf16_lo(uint32_t w) { return __uint_as_float(w << 16); }
-__device__ __forceinline__ float bf16_hi(uint32_t w) { return __uint_as_float(w & 0xFFFF0000u); }
+// bf16 -> fp32 of the low / high half of a packed pair.  The bit move is done in PTX so that the result is an f32 register:
+// with __uint_as_float the optimizer carries the accumulator fragments that the bf16 epilogues overwrite with these values
+// as 32-bit integers across the tile loop, and the resulting moves between wgmma.mma_async and its commit make ptxas
+// serialize every MMA of the main loop (C7514 / C7511, which the build rejects).
+__device__ __forceinline__ float bf16_lo(uint32_t w) { float f; asm("mov.b32 %0, %1;" : "=f"(f) : "r"(w << 16)); return f; }
+__device__ __forceinline__ float bf16_hi(uint32_t w) { float f; asm("mov.b32 %0, %1;" : "=f"(f) : "r"(w & 0xFFFF0000u)); return f; }
 
 }  // namespace tcx
 }  // namespace vt
