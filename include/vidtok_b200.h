@@ -232,10 +232,15 @@ int32_t vt_op_conv_ex(int32_t precision, const vt_conv_ex* e, const void* x, con
                       void* stream);
 /* Encoder conv_out with the KL / FSQ regularizer applied in the convolution's epilogue (regularizers.py:82-92,153-178,
  * distributions.py:8-18): reg_mode 1 = KL (Co = 2*zc, zc in {4,8,16}; noise NULL = the mode), 2 = FSQ (Co = zc = len(levels)).
- * h_out (fp32 [B,Co,T,H,W]) may be NULL; z fp32 [B,zc,T,H,W]; indices int32 [B,T,H,W] (FSQ); kl_loss 1 float (KL). */
+ * h_out (fp32 [B,Co,T,H,W]) may be NULL; z fp32 [B,zc,T,H,W]; indices int32 [B,T,H,W] (FSQ); kl_loss 1 float (KL).
+ * vt_op_conv_regularize: v1.0 zero time padding.  vt_op_conv_regularize_ex: e carries the geometry (e->d) and the v1.1
+ * time padding (t_mode, cacheT, with `cache` as in vt_op_conv_ex); its other fields are ignored. */
 int32_t vt_op_conv_regularize(int32_t precision, const vt_conv_desc* d, const void* x, const float* w, const float* bias,
                               int32_t reg_mode, int32_t zc, const int32_t* fsq_levels, const float* noise, float* h_out,
                               float* z, int32_t* indices, float* kl_loss, void* stream);
+int32_t vt_op_conv_regularize_ex(int32_t precision, const vt_conv_ex* e, const void* x, const void* cache, const float* w,
+                                 const float* bias, int32_t reg_mode, int32_t zc, const int32_t* fsq_levels, const float* noise,
+                                 float* h_out, float* z, int32_t* indices, float* kl_loss, void* stream);
 /* Encoder stem from the caller's fp32 [B,Ci,T,H,W] (t_rep replicated leading frames); out channels-last
  * [B,T+t_rep,H,W,Co] in the precision's activation type (BF16 / EXACT_TC). */
 int32_t vt_op_conv_stem(int32_t precision, const float* x, const float* w, const float* bias, void* out, int32_t B,
@@ -261,11 +266,15 @@ int32_t vt_op_layernorm(int32_t precision, const void* x, const float* gamma, co
 int32_t vt_op_groupnorm(int32_t precision, const void* x, const float* gamma, const float* beta, void* y,
                         int64_t frames, int64_t positions_per_frame, int32_t C, int32_t per_position,
                         int32_t apply_silu, void* workspace, int64_t workspace_bytes, void* stream);
-/* per-frame single-head attention core: q,k,v,o channels-last [frames, tokens, C]; scale = C^-0.5.  Runs what the
- * model path runs: wgmma GEMMs in BF16 / EXACT_TC when tokens % 64 == 0 and C % 64 == 0, fp32 FMAs otherwise.
+/* per-frame single-head attention core: q,k,v,o channels-last [frames, H, W, C] (tokens = H*W positions of a frame);
+ * scale = C^-0.5.  vt_op_attention_hw runs what the model path runs for a frame of H x W: wgmma GEMMs in BF16 / EXACT_TC
+ * when tokens % 64 == 0 and C % 64 == 0, fp32 FMAs otherwise.  vt_op_attention takes a token count and lays the tokens
+ * out as an image 8 wide (one row if tokens % 8 != 0): the same arithmetic, not necessarily a model frame's tile plan.
  * workspace: frames*tokens*(8*tokens + 24*C) + 65536 bytes is always enough. */
 int32_t vt_op_attention(int32_t precision, const void* q, const void* k, const void* v, void* o, int32_t frames,
                         int32_t tokens, int32_t C, void* workspace, int64_t workspace_bytes, void* stream);
+int32_t vt_op_attention_hw(int32_t precision, const void* q, const void* k, const void* v, void* o, int32_t frames,
+                           int32_t H, int32_t W, int32_t C, void* workspace, int64_t workspace_bytes, void* stream);
 int32_t vt_op_fsq(const float* h, int32_t d, const int32_t* levels, int64_t positions_per_batch, int32_t B,
                   float* codes, int32_t* indices, void* stream);
 int32_t vt_op_fsq_indices_to_codes(const int32_t* indices, int32_t d, const int32_t* levels,

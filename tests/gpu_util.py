@@ -141,3 +141,24 @@ def op_conv_ex(x, w, b, *, precision, stride=(1, 1, 1), pads=None, res=None, res
 
 def bf16_round(x):
     return x.to(torch.bfloat16).float()
+
+
+# kernels whose launch plan (tile, N tile, halo windows, stages, kparts, residual path, ...) the detailed profiler names
+PLAN_KERNELS = ("conv_tc", "conv_tc3", "tblock_tc", "conv_stem", "conv_stem3")
+
+
+def plan_keys(fn):
+    """run fn() under the library's detailed profiler -> (fn's result, {plan key: launches}) for the PLAN_KERNELS launches.
+    A key is the kernel name and its detail string, e.g. 'conv_tc k333 s11 128->128 @17x256x256 tile1x16x8 bn128 halo ln1
+    r0 p1 t0 st8'."""
+    import json
+    lib = N.lib()
+    lib.vt_profile_start_detailed()
+    try:
+        out = fn()
+    finally:
+        buf = C.create_string_buffer(1 << 22)
+        n = lib.vt_profile_stop(buf, len(buf))
+    assert n > 0, "profile did not fit the buffer"
+    prof = json.loads(buf.value.decode())
+    return out, {k: v["launches"] for k, v in prof.items() if k.split(" ", 1)[0] in PLAN_KERNELS}

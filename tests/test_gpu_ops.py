@@ -237,9 +237,9 @@ TC_CASES = [
     ("tc_tstride_avgpool", 64, 64, (3, 3, 3), (2, 1, 1), (2, 6, 16, 16), 3),
     ("tc_many_tiles", 64, 64, (3, 3, 3), (1, 1, 1), (2, 4, 64, 64), 1),
     ("tc_k333_c512", 512, 512, (3, 3, 3), (1, 1, 1), (1, 3, 16, 16), 1),
-    # large enough for the shared-memory halo window with two M tiles per CTA / with CTA pairs
+    # halo windows (8 x 16 output tiles): with the residual through the MMA / at N tile 256 with two time taps
     ("tc_halo_mt2", 64, 128, (1, 3, 3), (1, 1, 1), (1, 5, 128, 128), 1),
-    ("tc_halo_pair", 128, 256, (2, 3, 3), (1, 1, 1), (1, 3, 128, 128), 0),
+    ("tc_halo_k233_n256", 128, 256, (2, 3, 3), (1, 1, 1), (1, 3, 128, 128), 0),
 ]
 
 

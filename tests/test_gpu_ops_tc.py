@@ -85,7 +85,7 @@ X3_CASES = [
     ("many_tiles_res", 64, 64, (3, 3, 3), (1, 1, 1), (2, 4, 64, 64), 1),
     ("k333_c512_res", 512, 512, (3, 3, 3), (1, 1, 1), (1, 3, 16, 16), 1),
     ("halo_res", 64, 128, (1, 3, 3), (1, 1, 1), (1, 5, 128, 128), 1),
-    ("halo_pair_k233", 128, 256, (2, 3, 3), (1, 1, 1), (1, 3, 128, 128), 0),
+    ("halo_k233_n256", 128, 256, (2, 3, 3), (1, 1, 1), (1, 3, 128, 128), 0),
 ]
 
 
@@ -132,7 +132,7 @@ LN_CASES = [
     ("ln2_c128_k133_res", 128, 128, (1, 3, 3), (1, 2, 32, 32), 2, True, True),  # conv2 + skip -> next block's norm1
     ("ln2_c256_k311_res", 256, 256, (3, 1, 1), (2, 3, 16, 16), 2, True, True),
     ("ln2_c256_nosilu", 128, 256, (1, 1, 1), (1, 2, 16, 16), 2, False, False),  # -> attention norm (no SiLU)
-    ("ln2_c128_halo_res", 128, 128, (1, 3, 3), (1, 3, 128, 128), 2, True, True),  # halo windows, 2 M tiles, CTA pairs
+    ("ln2_c128_halo_res", 128, 128, (1, 3, 3), (1, 3, 128, 128), 2, True, True),  # halo windows, residual through the MMA
     ("ln1_c64", 64, 64, (3, 3, 3), (1, 3, 16, 16), 1, True, False),
 ]
 
@@ -327,9 +327,12 @@ def test_time_upsample_conv_two_phases(precision, fuse_ln):
 # attention core on wgmma (per-frame K / V^T as the B operand), LayerNorm / GroupNorm on split rows
 # ---------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("precision", PRECS, ids=PIDS)
-def test_attention_core_tcgen05(precision):
+def test_attention_core_wgmma(precision):
+    """small frames (16 x 16 tokens, C = 128); the production size (32 x 32 tokens, C = 512) is in
+    tests/test_gpu_production_plans.py"""
     from gpu_util import _p, empty_act, from_act, stream, to_act
-    frames, tokens, C_ = 3, 256, 128
+    frames, H, W, C_ = 3, 16, 16, 128
+    tokens = H * W
     q, k, v = (prep(rnd(frames, tokens, C_, seed=s_), precision) for s_ in (1, 2, 3))
     ref = F.scaled_dot_product_attention(q.double().unsqueeze(0), k.double().unsqueeze(0), v.double().unsqueeze(0))[0]
     qd, kd, vd = (to_act(t, precision) for t in (q, k, v))
@@ -337,7 +340,7 @@ def test_attention_core_tcgen05(precision):
     ws = torch.empty(frames * tokens * (8 * tokens + 24 * C_) + 65536, dtype=torch.uint8, device="cuda")
     lib = N.lib()
     lib.vt_profile_start()
-    N.check(lib.vt_op_attention(precision, _p(qd), _p(kd), _p(vd), _p(o), frames, tokens, C_, _p(ws), ws.numel(), stream()))
+    N.check(lib.vt_op_attention_hw(precision, _p(qd), _p(kd), _p(vd), _p(o), frames, H, W, C_, _p(ws), ws.numel(), stream()))
     buf = C.create_string_buffer(1 << 14)
     lib.vt_profile_stop(buf, len(buf))
     assert b"conv_tc" in buf.value and b"gemm_simt" not in buf.value, buf.value   # the tensor-core formulation ran
@@ -443,9 +446,9 @@ def test_fused_temporal_resblock(geom, with_ln):
         check(ncdhw(o2.float().cpu()), out2, N.PREC_BF16, "tblock out2", slack=2.5)
 
 
-def test_fused_temporal_resblock_many_frames_per_cta_pair():
-    """Same block at a size where every CTA pair walks ~7 strips x 20 frames (barrier phases wrap many times, the H tile and
-    the three accumulators are recycled hundreds of times, the peer CTA publishes its half through the forwarder warp).
+def test_fused_temporal_resblock_many_frames_per_cta():
+    """Same block at a size where every persistent CTA walks ~7 strips x 20 frames (barrier phases wrap many times, the
+    3-frame shared-memory ring and the accumulators are recycled hundreds of times).
     The reference is plain PyTorch fp32 on the GPU (TF32 off) with h rounded to bf16 where the kernel rounds it."""
     from gpu_util import _p, stream
     import torch.nn.functional as F

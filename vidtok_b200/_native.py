@@ -73,6 +73,7 @@ _SIGS = {
     "vt_op_conv": (_I32, [_I32, _I32, C.POINTER(ConvDesc), _P, _P, _P, _P, _P, _P]),
     "vt_op_conv_ex": (_I32, [_I32, C.POINTER(ConvEx), _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "vt_op_conv_regularize": (_I32, [_I32, C.POINTER(ConvDesc), _P, _P, _P, _I32, _I32, C.POINTER(_I32), _P, _P, _P, _P, _P, _P]),
+    "vt_op_conv_regularize_ex": (_I32, [_I32, C.POINTER(ConvEx), _P, _P, _P, _P, _I32, _I32, C.POINTER(_I32), _P, _P, _P, _P, _P, _P]),
     "vt_op_conv_stem": (_I32, [_I32, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P]),
     "vt_op_head_planes": (_I32, [_P, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P]),
     "vt_op_upsample_conv": (_I32, [_I32, _I32, _P, _P, _P, C.c_float, _P, _P, _I32, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P]),
@@ -80,6 +81,7 @@ _SIGS = {
     "vt_op_layernorm": (_I32, [_I32, _P, _P, _P, _P, _I64, _I32, _I32, _P]),
     "vt_op_groupnorm": (_I32, [_I32, _P, _P, _P, _P, _I64, _I64, _I32, _I32, _I32, _P, _I64, _P]),
     "vt_op_attention": (_I32, [_I32, _P, _P, _P, _P, _I32, _I32, _I32, _P, _I64, _P]),
+    "vt_op_attention_hw": (_I32, [_I32, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _P, _I64, _P]),
     "vt_op_fsq": (_I32, [_P, _I32, C.POINTER(_I32), _I64, _I32, _P, _P, _P]),
     "vt_op_fsq_indices_to_codes": (_I32, [_P, _I32, C.POINTER(_I32), _I64, _I32, _P, _P]),
     "vt_op_kl": (_I32, [_P, _P, _I32, _I64, _I32, _I32, _P, _P, _P]),

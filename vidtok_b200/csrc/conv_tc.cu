@@ -785,7 +785,9 @@ int conv_tc_cluster_query(int smem, char* msg, int cap) {
   return n;
 }
 
-bool conv_tc_can_fuse_ln(const ConvP& p) { return p.Co <= 256 && choose_bn(p.Co) == p.Co; }
+bool conv_tc_can_fuse_ln(const ConvP& p) {
+  return p.Co <= 256 && choose_bn(p.Co) == p.Co && (!p.split || split_ln_fusion_keeps_kparts(p.Co, p.kt * p.kh * p.kw * (p.Ci / 64)));
+}
 
 bool conv_tc_supported(const ConvP& p, DType tout, bool planning) {
   g_tc_err.clear();
@@ -1014,8 +1016,10 @@ cudaError_t launch_conv_tc(const ConvP& p, const bf16* x, const bf16* w_nk, int 
   }
   const unsigned grid = (unsigned)(t.num_tiles < num_sms ? t.num_tiles : num_sms);
   const double Mrows = (double)p.B * p.To * p.Ho * p.Wo;
-  char det[128] = "";
-  if (prof_enabled()) snprintf(det, sizeof(det), "k%d%d%d s%d%d %d->%d @%dx%dx%d tile%dx%dx%d bn%d%s ln%d r%d%s p%d", p.kt, p.kh, p.kw, p.st, p.sh, p.Ci, p.Co, p.To, p.Ho, p.Wo, t.BT, t.BH, t.BW, t.BN, t.halo ? " halo" : "", t.ln_mode, p.res_mode, t.res_mma ? "m" : "", split ? t.kparts : 1);
+  // plan key of the launch (profiler detail): geometry, tile, N tile, halo windows, fused LayerNorm, residual mode (m: through
+  // the MMA), kparts, time padding (t0 zeros / t1 replicate / t2 cache) and pipeline stages
+  char det[160] = "";
+  if (prof_enabled()) snprintf(det, sizeof(det), "k%d%d%d s%d%d %d->%d @%dx%dx%d tile%dx%dx%d bn%d%s ln%d r%d%s p%d t%d st%d", p.kt, p.kh, p.kw, p.st, p.sh, p.Ci, p.Co, p.To, p.Ho, p.Wo, t.BT, t.BH, t.BW, t.BN, t.halo ? " halo" : "", t.ln_mode, p.res_mode, t.res_mma ? "m" : "", split ? t.kparts : 1, p.t_mode, t.stages);
   ProfScope _ps(split ? "conv_tc3" : "conv_tc", 2.0 * Mrows * p.kt * p.kh * p.kw * p.Ci * p.Co,
                 2.0 * cw * ((double)p.B * p.Ti * p.Hi * p.Wi * p.Ci) + Mrows * p.Co * (tout == DT_F32 ? 4.0 : 2.0 * cw), s, det);
   auto launch = [&](auto kern) { kern<<<grid, kThreads, smem, s>>>(maps, t); };

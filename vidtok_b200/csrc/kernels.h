@@ -57,6 +57,10 @@ inline float split_weight_scale(float maxabs, float headroom = 1.0f) {
   while (sc * maxabs * headroom >= 4096.0f && sc > 1.0e-30f) sc *= 0.5f;
   return sc;
 }
+// The headroom the model uses for every convolution (a phase-collapsed tap sums up to 4 original taps).  The single-operator
+// entry points use it too, so that they pick the same scale, and with it the same residual path (res_mma needs 2^s <= 2^15),
+// as the model does for the same weights.
+constexpr float kModelWeightHeadroom = 4.0f;
 // phase-collapsed weights of "nearest-2x upsample then conv": original taps (a,b,c) of a kt x kh x kw kernel are
 // summed into tap (mt[a], mh[b], mw[c]) of a kt2 x kh2 x kw2 kernel; output [Co_pad][kt2*kh2*kw2*Ci] bf16
 cudaError_t launch_pack_w_collapsed(const float* w, bf16* out, int Co, int Co_pad, int Ci, int kt, int kh, int kw,
@@ -105,6 +109,11 @@ struct TcRegFusion {
   int fsq_levels[VT_MAX_FSQ] = {0};
 };
 bool conv_tc_can_fuse_ln(const ConvP& p);
+// Split mode: a fused LayerNorm needs one N tile over Cout, and N tiles wider than 128 have no registers left for the
+// running sum of the kparts groups.  From 16 K steps on, where the plan sums in kparts, the tensor core's chained fp32
+// accumulation alone would exceed fp32-class error (measured 1.2-1.4x the 4e-5 (1 + |ref|) bound at 72-108 K steps,
+// 256 channels), so such a LayerNorm runs as its own kernel after a kparts convolution.
+inline bool split_ln_fusion_keeps_kparts(int Co, int k_steps) { return Co <= 128 || k_steps < 16; }
 // planning = true: geometry-only answer (workspace dry runs: no device pointers, possibly no driver)
 bool conv_tc_supported(const ConvP& p, DType tout, bool planning = false);
 // out may be null when a regularizer epilogue consumes the result (reg != nullptr)

@@ -802,8 +802,9 @@ struct Exec {
   }
   bool fold_upsample() const { return prec == VT_PREC_FMA32; }
 
-  bool phase_ln_ok(int Co) const {
-    return tcm && m->desc.norm_type == VT_NORM_LAYERNORM && Co % 32 == 0 && Co <= 256;
+  bool phase_ln_ok(const ConvW& ph) const {
+    return tcm && m->desc.norm_type == VT_NORM_LAYERNORM && ph.Co % 32 == 0 && ph.Co <= 256 &&
+           (!split || split_ln_fusion_keeps_kparts(ph.Co, ph.taps() * (ph.Ci / 64)));
   }
   // Downsample: pad (0,1,0,1) + conv3x3 stride 2 (model_3dcausal.py:223-227)
   void down(const LevelW& lv, Stream& st, const NormW* next, bool next_silu) {
@@ -832,7 +833,7 @@ struct Exec {
     } else if (lv.has_up_phase && tcm) {
       // four parity classes of the 2x-upsampled output, each a 1x2x2 conv on the low-resolution input
       Act y = new_act(h.B, h.T, 2 * h.H, 2 * h.W, lv.resample.Co);
-      const bool fuse = next && phase_ln_ok(lv.resample.Co);
+      const bool fuse = next && phase_ln_ok(lv.up_ph[0]);
       Act n;
       if (fuse) n = new_act(h.B, h.T, 2 * h.H, 2 * h.W, lv.resample.Co);
       const long long C = lv.resample.Co, Wo2 = 2 * h.W, Ho2 = 2 * h.H;
@@ -878,7 +879,7 @@ struct Exec {
       if (lv.has_tup_phase && tcm) {
         // even / odd output frames: 2x3x3 convs on the un-upsampled input, mixed with x[t/2] in the epilogue
         Act out = new_act(x.B, 2 * x.T, x.H, x.W, lv.tconv.Co);
-        const bool fuse = next && phase_ln_ok(lv.tconv.Co);
+        const bool fuse = next && phase_ln_ok(lv.tup_ph[0]);
         Act n;
         if (fuse) n = new_act(x.B, 2 * x.T, x.H, x.W, lv.tconv.Co);
         const long long fr = (long long)x.H * x.W * lv.tconv.Co;
@@ -1369,7 +1370,7 @@ int32_t vt_model_finalize(vt_model* m, void* stream) {
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
     cudaFree(d_max);
     if (e != cudaSuccess) return fail(VT_ERR_CUDA, "weight scale readback: %s", cudaGetErrorString(e));
-    for (size_t i = 0; i < m->convs.size(); ++i) m->convs[i]->wscale3 = split_weight_scale(h_max[i], 4.0f);   // headroom: collapsed taps
+    for (size_t i = 0; i < m->convs.size(); ++i) m->convs[i]->wscale3 = split_weight_scale(h_max[i], kModelWeightHeadroom);
   }
   size_t okn = 0, onk = 0;
   for (ConvW* c : m->convs) {
@@ -2001,7 +2002,7 @@ static int op_conv_impl(int precision, int force_simt, const vt_conv_desc* d, co
     VT_CUDA(cudaMalloc(&wnk, (size_t)K * Co_pad * sizeof(bf16) * cw));
     float wsc = 0.f;
     if (ta == DT_SPLIT) {
-      int rc = op_weight_scale(w, (long long)d->Co * K, 1.0f, s, &wsc);
+      int rc = op_weight_scale(w, (long long)d->Co * K, kModelWeightHeadroom, s, &wsc);
       if (rc) { cudaFree(wnk); return rc; }
       p.acc_scale = 1.0f / wsc;
     }
@@ -2033,16 +2034,20 @@ int32_t vt_op_conv_ex(int32_t precision, const vt_conv_ex* e, const void* x, con
 
 // Encoder conv_out with the regularizer in its epilogue, as the model path runs it: x channels-last activation,
 // h_out (optional) fp32 [B,Co,T,H,W]; KL: Co = 2*zc, noise/z fp32 [B,zc,T,H,W], kl_loss = 0.5 * sum / B;
-// FSQ: Co = zc = number of levels, z = codes, indices int32 [B,T,H,W].
-int32_t vt_op_conv_regularize(int32_t precision, const vt_conv_desc* d, const void* x, const float* w, const float* bias,
-                              int32_t reg_mode, int32_t zc, const int32_t* fsq_levels, const float* noise, float* h_out,
-                              float* z, int32_t* indices, float* kl_loss, void* stream) {
-  if (!d || !z) return fail(VT_ERR_INVALID, "null argument");
+// FSQ: Co = zc = number of levels, z = codes, indices int32 [B,T,H,W].  ex carries the geometry and the v1.1 time
+// padding (t_mode, cacheT with `cache`); its output fields are ignored (the head output is always fp32 [B,C,T,H,W]).
+int32_t vt_op_conv_regularize_ex(int32_t precision, const vt_conv_ex* ex, const void* x, const void* cache, const float* w,
+                                 const float* bias, int32_t reg_mode, int32_t zc, const int32_t* fsq_levels, const float* noise,
+                                 float* h_out, float* z, int32_t* indices, float* kl_loss, void* stream) {
+  if (!ex || !z) return fail(VT_ERR_INVALID, "null argument");
   if (precision != VT_PREC_BF16 && precision != VT_PREC_EXACT_TC) return fail(VT_ERR_INVALID, "the regularizer epilogue exists on the wgmma path only");
   cudaStream_t s = (cudaStream_t)stream;
+  const vt_conv_desc* d = &ex->d;
   vt_conv_ex e;
   memset(&e, 0, sizeof(e));
   e.d = *d;
+  e.t_mode = ex->t_mode;
+  e.cacheT = ex->cacheT;
   e.out_f32_ncdhw = 1;
   TcRegFusion rf;
   rf.mode = reg_mode; rf.zc = zc; rf.z = z; rf.noise = noise; rf.indices = indices; rf.sample = noise ? 1 : 0;
@@ -2057,7 +2062,7 @@ int32_t vt_op_conv_regularize(int32_t precision, const vt_conv_desc* d, const vo
   } else {
     return fail(VT_ERR_INVALID, "reg_mode must be 1 (KL) or 2 (FSQ)");
   }
-  int rc = op_conv_impl(precision, 0, d, &e, x, nullptr, w, bias, nullptr, nullptr, nullptr, h_out, nullptr, s, &rf);
+  int rc = op_conv_impl(precision, 0, d, &e, x, cache, w, bias, nullptr, nullptr, nullptr, h_out, nullptr, s, &rf);
   if (rc == VT_OK && reg_mode == 1 && kl_loss) {
     cudaError_t er = launch_kl_finish(acc, d->B, kl_loss, s);
     if (er == cudaSuccess) er = cudaStreamSynchronize(s);
@@ -2065,6 +2070,16 @@ int32_t vt_op_conv_regularize(int32_t precision, const vt_conv_desc* d, const vo
   }
   if (acc) cudaFree(acc);
   return rc;
+}
+// the same with v1.0 zero time padding
+int32_t vt_op_conv_regularize(int32_t precision, const vt_conv_desc* d, const void* x, const float* w, const float* bias,
+                              int32_t reg_mode, int32_t zc, const int32_t* fsq_levels, const float* noise, float* h_out,
+                              float* z, int32_t* indices, float* kl_loss, void* stream) {
+  if (!d) return fail(VT_ERR_INVALID, "null argument");
+  vt_conv_ex e;
+  memset(&e, 0, sizeof(e));
+  e.d = *d;
+  return vt_op_conv_regularize_ex(precision, &e, x, nullptr, w, bias, reg_mode, zc, fsq_levels, noise, h_out, z, indices, kl_loss, stream);
 }
 
 // Encoder stem (conv_in from the caller's fp32 [B,Ci,T,H,W] tensor) on the conv_stem kernel.
@@ -2088,7 +2103,7 @@ int32_t vt_op_conv_stem(int32_t precision, const float* x, const float* w, const
   bf16* wpk = nullptr;
   float wsc = 0.f;
   if (split) {
-    int rc = op_weight_scale(w, (long long)Co * Ci * 27, 1.0f, s, &wsc);
+    int rc = op_weight_scale(w, (long long)Co * Ci * 27, kModelWeightHeadroom, s, &wsc);
     if (rc) return rc;
     p.acc_scale = 1.0f / wsc;
   }
@@ -2156,7 +2171,7 @@ int32_t vt_op_upsample_conv(int32_t precision, int32_t kind, const void* x, cons
   const int lo[3] = {0, 1, 1}, hi[3] = {0, 0, 1};
   float wsc = 0.f;
   if (split) {
-    int rcw = op_weight_scale(w, (long long)Co * Ci * (kind == 0 ? 9 : 27), 4.0f, s, &wsc);
+    int rcw = op_weight_scale(w, (long long)Co * Ci * (kind == 0 ? 9 : 27), kModelWeightHeadroom, s, &wsc);
     if (rcw) { cudaFree(wp); return rcw; }
   }
   for (int i = 0; i < nph; ++i) {
@@ -2245,24 +2260,32 @@ int32_t vt_op_groupnorm(int32_t precision, const void* x, const float* gamma, co
   return VT_OK;
 }
 // The attention core the model path runs for this precision and shape: wgmma GEMMs (per-frame K / V^T as the B
-// operand) when tokens and C are multiples of 64 in the tensor-core modes, fp32 FMA GEMMs otherwise.
-int32_t vt_op_attention(int32_t precision, const void* q, const void* k, const void* v, void* o, int32_t frames,
-                        int32_t tokens, int32_t C, void* workspace, int64_t workspace_bytes, void* stream) {
+// operand) when tokens = H * W and C are multiples of 64 in the tensor-core modes, fp32 FMA GEMMs otherwise.  The
+// tokens of a frame are its H x W positions, as in the model, so the launches get the model's tile plan.
+int32_t vt_op_attention_hw(int32_t precision, const void* q, const void* k, const void* v, void* o, int32_t frames,
+                           int32_t H, int32_t W, int32_t C, void* workspace, int64_t workspace_bytes, void* stream) {
   if (!q || !k || !v || !o || !workspace) return fail(VT_ERR_INVALID, "null argument");
   if (precision != VT_PREC_FMA32 && precision != VT_PREC_BF16 && precision != VT_PREC_EXACT_TC)
     return fail(VT_ERR_INVALID, "operator precision must be FMA32, BF16 or EXACT_TC");
+  if (frames <= 0 || H <= 0 || W <= 0 || C <= 0) return fail(VT_ERR_INVALID, "attention: empty shape");
+  const long long tokens = (long long)H * W;
   vt_model dummy;
   memset(&dummy.desc, 0, sizeof(dummy.desc));
   Exec ex(&dummy, precision, (cudaStream_t)stream, workspace, (size_t)workspace_bytes, false);
   Act aq, ak, av;
-  aq.B = frames; aq.T = 1; aq.H = 1; aq.W = tokens; aq.C = C;
-  // the wgmma formulation tiles positions as (H, W) boxes: present the token axis as an 8-wide image when possible
-  if (tokens % 8 == 0) { aq.H = tokens / 8; aq.W = 8; }
+  aq.B = frames; aq.T = 1; aq.H = H; aq.W = W; aq.C = C;
   ak = aq; av = aq;
   aq.p = const_cast<void*>(q); ak.p = const_cast<void*>(k); av.p = const_cast<void*>(v);
   Act ao = ex.attention_core(aq, ak, av);
   if (ex.ok()) ex.cuda(cudaMemcpyAsync(o, ao.p, (size_t)frames * tokens * C * dtype_size(ex.ta), cudaMemcpyDeviceToDevice, ex.s), "copy out");
   return ex.rc;
+}
+// The same for a token count without a frame geometry: the tokens are laid out as an image 8 wide when tokens % 8 == 0
+// (one row otherwise), which is not the tile plan of a model frame of H x W (vt_op_attention_hw).
+int32_t vt_op_attention(int32_t precision, const void* q, const void* k, const void* v, void* o, int32_t frames,
+                        int32_t tokens, int32_t C, void* workspace, int64_t workspace_bytes, void* stream) {
+  const bool w8 = tokens > 0 && tokens % 8 == 0;
+  return vt_op_attention_hw(precision, q, k, v, o, frames, w8 ? tokens / 8 : 1, w8 ? 8 : tokens, C, workspace, workspace_bytes, stream);
 }
 // ---- video I/O adjacent steps ---------------------------------------------------------------------------
 int32_t vt_video_u8_to_clip(const uint8_t* frames, float* clip, int32_t T, int32_t Hs, int32_t Ws, int32_t C, int32_t h0,
