@@ -192,6 +192,13 @@ int32_t vt_decode_video(vt_model* m, int32_t precision, const float* z, int32_t 
  * of the crop window at (h0, w0) (CenterCrop; the optional Resize is not part of this entry point). */
 int32_t vt_video_u8_to_clip(const uint8_t* frames, float* clip, int32_t T, int32_t Hs, int32_t Ws, int32_t C, int32_t h0,
                             int32_t w0, int32_t H, int32_t W, void* stream);
+/* frames: device uint8 [N,Hs,Ws,C]; clip: device fp32 [N/Tc,C,Tc,H,W], frame n -> clip n/Tc, time n%Tc.  The reference's
+ * Resize(antialias=True) -> CenterCrop -> Normalize(.5,.5) of frames/255: torch's antialiased bilinear resize to Hr x Wr
+ * (align_corners=False), then the crop window at (h0, w0), in one launch without workspace.  N % Tc == 0 and the window
+ * must lie inside Hr x Wr.  VT_ERR_INVALID when the downscale is so large that the source window of one output pixel
+ * does not fit in shared memory (about 130x for C = 3). */
+int32_t vt_video_u8_to_clip_resized(const uint8_t* frames, float* clip, int32_t N, int32_t Hs, int32_t Ws, int32_t C, int32_t Hr,
+                                    int32_t Wr, int32_t h0, int32_t w0, int32_t H, int32_t W, int32_t Tc, void* stream);
 /* clip: device fp32 [C,T,H,W]; frames: device uint8 [T,H,W,C] = uint8(255 * (clamp(clip,-1,1) + 1) / 2) (tensor_to_uint8). */
 int32_t vt_clip_to_video_u8(const float* clip, uint8_t* frames, int32_t C, int32_t T, int32_t H, int32_t W, void* stream);
 

@@ -69,6 +69,7 @@ _SIGS = {
     "vt_decode_video_frames": (_I32, [_P, _I32, _I32, _I32]),
     "vt_decode_video": (_I32, [_P, _I32, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _I32, _P, _I64, _P]),
     "vt_video_u8_to_clip": (_I32, [_P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P]),
+    "vt_video_u8_to_clip_resized": (_I32, [_P, _P] + [_I32] * 11 + [_P]),
     "vt_clip_to_video_u8": (_I32, [_P, _P, _I32, _I32, _I32, _I32, _P]),
     "vt_op_conv": (_I32, [_I32, _I32, C.POINTER(ConvDesc), _P, _P, _P, _P, _P, _P]),
     "vt_op_conv_ex": (_I32, [_I32, C.POINTER(ConvEx), _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),

@@ -81,6 +81,12 @@ cudaError_t launch_copy_frames(DType t, const void* src, void* dst, int B, long 
 cudaError_t launch_u8_frames_to_clip(const uint8_t* src, float* dst, int T, int Hs, int Ws, int C, int h0, int w0, int H, int W,
                                     cudaStream_t s);
 cudaError_t launch_clip_to_u8_frames(const float* src, uint8_t* dst, int C, int T, int H, int W, cudaStream_t s);
+// video_io.cu: uint8 frames [N,Hs,Ws,C] -> antialiased bilinear resize to Hr x Wr -> crop (h0,w0,H,W) -> Normalize(.5,.5)
+// -> clips fp32 [N/Tc,C,Tc,H,W].  _fits is false when the source window of one output pixel exceeds shared memory (the
+// launcher then returns cudaErrorInvalidValue).
+bool u8_frames_resize_fits(int Hs, int Ws, int C, int Hr, int Wr, int h0, int w0, int H, int W);
+cudaError_t launch_u8_frames_resize_to_clip(const uint8_t* src, float* dst, int N, int Hs, int Ws, int C, int Hr, int Wr, int h0,
+                                            int w0, int H, int W, int Tc, cudaStream_t s);
 // hi|lo split rows [rows][hi(C) | lo(C)] <-> fp32 rows [rows][C]
 cudaError_t launch_split_to_f32(const bf16* x, float* y, long long rows, int C, cudaStream_t s);
 cudaError_t launch_f32_to_split(const float* x, bf16* y, long long rows, int C, cudaStream_t s);

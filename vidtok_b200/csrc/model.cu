@@ -2295,6 +2295,18 @@ int32_t vt_video_u8_to_clip(const uint8_t* frames, float* clip, int32_t T, int32
   VT_CUDA(launch_u8_frames_to_clip(frames, clip, T, Hs, Ws, C, h0, w0, H, W, (cudaStream_t)stream));
   return VT_OK;
 }
+int32_t vt_video_u8_to_clip_resized(const uint8_t* frames, float* clip, int32_t N, int32_t Hs, int32_t Ws, int32_t C, int32_t Hr,
+                                    int32_t Wr, int32_t h0, int32_t w0, int32_t H, int32_t W, int32_t Tc, void* stream) {
+  if (!frames || !clip) return fail(VT_ERR_INVALID, "null argument");
+  if (N <= 0 || C <= 0 || Hs <= 0 || Ws <= 0 || Hr <= 0 || Wr <= 0 || Tc <= 0 || N % Tc != 0)
+    return fail(VT_ERR_INVALID, "bad shape: N=%d Tc=%d (N must be a positive multiple of Tc)", N, Tc);
+  if (H <= 0 || W <= 0 || h0 < 0 || w0 < 0 || h0 + H > Hr || w0 + W > Wr) return fail(VT_ERR_INVALID, "crop window outside the resized frame");
+  if (!u8_frames_resize_fits(Hs, Ws, C, Hr, Wr, h0, w0, H, W))
+    return fail(VT_ERR_INVALID, "resize %dx%d -> %dx%d: scale too large, the source window of one output pixel does not fit in "
+                "shared memory", Hs, Ws, Hr, Wr);
+  VT_CUDA(launch_u8_frames_resize_to_clip(frames, clip, N, Hs, Ws, C, Hr, Wr, h0, w0, H, W, Tc, (cudaStream_t)stream));
+  return VT_OK;
+}
 int32_t vt_clip_to_video_u8(const float* clip, uint8_t* frames, int32_t C, int32_t T, int32_t H, int32_t W, void* stream) {
   if (!frames || !clip) return fail(VT_ERR_INVALID, "null argument");
   if (T <= 0 || C <= 0 || H <= 0 || W <= 0) return fail(VT_ERR_INVALID, "bad shape");
