@@ -177,6 +177,15 @@ int64_t vt_encode_video_workspace_bytes(const vt_model* m, int32_t precision, in
 int32_t vt_encode_video(vt_model* m, int32_t precision, const float* x, int32_t x_on_host, int32_t B, int32_t C, int32_t T,
                         int32_t H, int32_t W, int32_t t_chunk_enc, const float* noise, float* z, int32_t* indices,
                         float* kl_loss, void* workspace, int64_t workspace_bytes, void* stream);
+/* vt_encode_video of an FSQ model that also writes the per-chunk partials of the FSQ aux loss (see vt_fsq_aux_partials):
+ * chunk i of the schedule (first frame alone, then t_chunk_enc frames each) writes aux_stats[2i..2i+1] and
+ * aux_avg_prob[i*J .. (i+1)*J), J = prod(levels).  z / indices as vt_encode_video; host-staged and device inputs give the
+ * same bits.  The workspace is larger than vt_encode_video's. */
+int64_t vt_encode_video_fsq_aux_workspace_bytes(const vt_model* m, int32_t precision, int32_t B, int32_t T, int32_t H, int32_t W,
+                                                int32_t t_chunk_enc);
+int32_t vt_encode_video_fsq_aux(vt_model* m, int32_t precision, const float* x, int32_t x_on_host, int32_t B, int32_t C, int32_t T,
+                                int32_t H, int32_t W, int32_t t_chunk_enc, float* z, int32_t* indices, float inv_temperature,
+                                float* aux_stats, float* aux_avg_prob, void* workspace, int64_t workspace_bytes, void* stream);
 int64_t vt_decode_video_workspace_bytes(const vt_model* m, int32_t precision, int32_t B, int32_t Tz, int32_t Hz, int32_t Wz,
                                         int32_t t_chunk_dec, int32_t use_overlap);
 /* frames vt_decode_video writes (look-ahead tails dropped; the v1.1 forward then keeps the last T_in frames) */
@@ -288,6 +297,29 @@ int32_t vt_op_fsq_indices_to_codes(const int32_t* indices, int32_t d, const int3
                                    int64_t positions_per_batch, int32_t B, float* codes, void* stream);
 int32_t vt_op_kl(const float* h, const float* noise, int32_t zc, int64_t positions_per_batch, int32_t B, int32_t sample,
                  float* z, float* kl_loss, void* stream);
+
+/* ---- FSQ auxiliary loss (FSQRegularizer.forward, regularizers.py:232-245): the clamped per-sample entropy, the codebook
+ *      entropy of the batch-mean code distribution and the commitment MSE, computed from one small softmax per latent
+ *      channel instead of the tokens x codebook distance matrix.  Two steps so that a caller can all-reduce the per-segment
+ *      avg_prob between them (regularizers.py:49-59,240).  A segment is one untiled batch or one chunk of a tiled video.
+ *      Supported: 1 <= d <= 8, every level >= 2, sum of the levels <= 256, codebook <= 2^22 codes (else VT_ERR_INVALID).
+ *      Every reduction runs in a fixed order: repeated calls give the same bits. ---- */
+/* workspace of vt_fsq_aux_partials for `tokens` = B * positions_per_batch tokens (-1 when unsupported) */
+int64_t vt_fsq_aux_workspace_bytes(int32_t d, const int32_t* levels, int64_t tokens);
+/* h: device fp32 [B,d,positions] (the encoder output before the FSQ bound; tokens in (b, t, h, w) order).  Outputs (device):
+ * stats fp32 [2] = (per_sample_entropy, commit_loss), avg_prob fp32 [prod(levels)] = mean over the tokens of
+ * softmax_j(2 * inv_temperature * <z, code_j>). */
+int32_t vt_fsq_aux_partials(const float* h, int32_t d, const int32_t* levels, int64_t positions_per_batch, int32_t B,
+                            float inv_temperature, float* stats, float* avg_prob, void* workspace, int64_t workspace_bytes,
+                            void* stream);
+/* stats [n_segments][2] and avg_prob [n_segments][J] as vt_fsq_aux_partials wrote them, avg_prob summed over world_size ranks
+ * by the caller (world_size 1: not distributed).  Per segment: codebook_entropy over all J codes of avg_prob / world_size,
+ * aux = (per_sample_entropy - diversity_gamma * codebook_entropy) * entropy_weight + commit_loss * commitment_weight.
+ * aux_loss (1 float, device) = mean of the segments' aux; components (device, may be NULL) [n_segments][4] =
+ * (per_sample_entropy, codebook_entropy, commit_loss, aux).  entropy_weight is calculate_entropy_loss_weight(n_steps). */
+int32_t vt_fsq_aux_finalize(const float* stats, const float* avg_prob, int32_t n_segments, int32_t d, const int32_t* levels,
+                            int32_t world_size, float entropy_weight, float diversity_gamma, float commitment_weight,
+                            float* aux_loss, float* components, void* stream);
 
 #ifdef __cplusplus
 }

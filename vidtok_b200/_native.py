@@ -65,6 +65,8 @@ _SIGS = {
     "vt_decode_chunk": (_I32, [_P, _I32, _P, _I32, _I32, _P, _P, _I64, _P]),
     "vt_encode_video_workspace_bytes": (_I64, [_P, _I32, _I32, _I32, _I32, _I32, _I32]),
     "vt_encode_video": (_I32, [_P, _I32, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _I64, _P]),
+    "vt_encode_video_fsq_aux_workspace_bytes": (_I64, [_P, _I32, _I32, _I32, _I32, _I32, _I32]),
+    "vt_encode_video_fsq_aux": (_I32, [_P, _I32, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P, C.c_float, _P, _P, _P, _I64, _P]),
     "vt_decode_video_workspace_bytes": (_I64, [_P, _I32, _I32, _I32, _I32, _I32, _I32, _I32]),
     "vt_decode_video_frames": (_I32, [_P, _I32, _I32, _I32]),
     "vt_decode_video": (_I32, [_P, _I32, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _I32, _P, _I64, _P]),
@@ -86,6 +88,9 @@ _SIGS = {
     "vt_op_fsq": (_I32, [_P, _I32, C.POINTER(_I32), _I64, _I32, _P, _P, _P]),
     "vt_op_fsq_indices_to_codes": (_I32, [_P, _I32, C.POINTER(_I32), _I64, _I32, _P, _P]),
     "vt_op_kl": (_I32, [_P, _P, _I32, _I64, _I32, _I32, _P, _P, _P]),
+    "vt_fsq_aux_workspace_bytes": (_I64, [_I32, C.POINTER(_I32), _I64]),
+    "vt_fsq_aux_partials": (_I32, [_P, _I32, C.POINTER(_I32), _I64, _I32, C.c_float, _P, _P, _P, _I64, _P]),
+    "vt_fsq_aux_finalize": (_I32, [_P, _P, _I32, _I32, C.POINTER(_I32), _I32, C.c_float, C.c_float, C.c_float, _P, _P, _P]),
 }
 EXPORTS = tuple(_SIGS.keys())
 

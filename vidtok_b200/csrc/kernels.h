@@ -40,6 +40,27 @@ cudaError_t launch_fsq(const float* h, int d, const int* levels_host, long long 
                        cudaStream_t s);
 cudaError_t launch_fsq_indices_to_codes(const int* indices, int d, const int* levels_host, long long P, int B,
                                         float* codes, cudaStream_t s);
+// fsq_aux.cu: the FSQ auxiliary loss (regularizers.py:232-245) from the per-channel softmax factors.  One segment (an
+// untiled batch or one chunk of a tiled video) gives partials stats [2] = (per_sample_entropy, commit_loss) and
+// avg_prob [J]; the finish step combines n segments (avg_prob summed over `world` ranks by the caller, then divided here).
+#define VT_FSQ_AUX_MAX_CODEBOOK (1LL << 22)
+#define VT_FSQ_AUX_MAX_SUM_LEVELS 256
+struct FsqAuxGeom {
+  int d = 0, a = 0;                            // digits; the low group is digits [0, a)
+  int L[VT_MAX_FSQ] = {0}, off[VT_MAX_FSQ] = {0};   // levels; offset of channel i's table in a token's factor row
+  int SL = 0;                                  // sum of the levels (factor row length)
+  int J = 0, Jlo = 0, Jhi = 0;                 // codebook = Jlo * Jhi, code j = j_lo + Jlo * j_hi
+  int ksplit = 1;                              // token slices of the avg_prob contraction
+  long long N = 0, kchunk = 0;                 // tokens; tokens per slice
+};
+// nullptr, or why the level list / token count is not supported
+const char* fsq_aux_geometry(int d, const int* levels, long long N, FsqAuxGeom* g);
+size_t fsq_aux_workspace(const FsqAuxGeom& g);
+// h fp32 [B, d, P] (tokens n = b * P + p); stats / avg_prob device outputs of this segment
+cudaError_t launch_fsq_aux_partials(const float* h, const FsqAuxGeom& g, const int* levels, long long P, float inv_t, float* stats,
+                                    float* avg_prob, void* ws, cudaStream_t s);
+cudaError_t launch_fsq_aux_finalize(const float* stats, const float* avg_prob, int nseg, int J, int world, float w_ent, float gamma,
+                                    float w_commit, float* aux, float* comp, cudaStream_t s);
 // weight repacking: w [Co][Ci][taps] (reference OIDHW flattened) -> [K = tap*Ci + ci][Co] fp32
 cudaError_t launch_pack_w_kn(const float* w, float* out, int Co, int Ci, int taps, cudaStream_t s);
 // -> [Co][K = tap*Ci + ci] bf16 (K-major rows for the wgmma B operand)

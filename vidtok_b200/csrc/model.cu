@@ -1615,8 +1615,9 @@ int64_t vt_chunk_workspace_bytes(const vt_chunk_state* cs, int32_t Tc) {
   return (int64_t)(peak + 4096);
 }
 
-int32_t vt_encode_chunk(vt_chunk_state* cs, int32_t is_first, const float* x_chunk, int32_t C, int32_t Tc, const float* noise,
-                        float* z, int32_t* indices, float* kl_loss, void* workspace, int64_t workspace_bytes,
+// h_out (optional): the chunk's encoder output before the regularizer, fp32 [B,Cz,Tz,Hz,Wz] (the FSQ aux loss reads it)
+static int encode_chunk(vt_chunk_state* cs, int32_t is_first, const float* x_chunk, int32_t C, int32_t Tc, const float* noise,
+                        float* z, int32_t* indices, float* kl_loss, float* h_out, void* workspace, int64_t workspace_bytes,
                         void* stream) {
   if (!cs || !x_chunk || !z) return fail(VT_ERR_INVALID, "null argument");
   if (cs->is_decoder) return fail(VT_ERR_INVALID, "decoder state passed to vt_encode_chunk");
@@ -1630,16 +1631,21 @@ int32_t vt_encode_chunk(vt_chunk_state* cs, int32_t is_first, const float* x_chu
   latent_shape(m, Tc, cs->H, cs->W, &Tz, &Hz, &Wz);
   Exec ex(m, stack_prec(cs->prec, false), s, workspace, (size_t)workspace_bytes, false);
   ex.ck = cs;
-  float* hp = (float*)ex.alloc((size_t)cs->B * (m->desc.double_z ? 2 : 1) * m->desc.z_channels * Tz * Hz * Wz * sizeof(float));
+  float* hp = h_out ? h_out : (float*)ex.alloc((size_t)cs->B * (m->desc.double_z ? 2 : 1) * m->desc.z_channels * Tz * Hz * Wz * sizeof(float));
   if (!ex.ok()) return ex.rc;
   TcRegFusion rf;
   int rc = make_reg_fusion(m, noise, z, indices, s, &rf);
   if (rc) return rc;
   bool reg_done = false;
-  run_encoder(ex, x_chunk, cs->B, Tc, cs->H, cs->W, hp, &rf, false, &reg_done);
+  run_encoder(ex, x_chunk, cs->B, Tc, cs->H, cs->W, hp, &rf, h_out != nullptr, &reg_done);
   if (!ex.ok()) return ex.rc;
   if (reg_done) return finish_reg_fusion(m, cs->B, kl_loss, s);
   return regularize(m, hp, noise, cs->B, Tz, Hz, Wz, z, indices, kl_loss, s);
+}
+int32_t vt_encode_chunk(vt_chunk_state* cs, int32_t is_first, const float* x_chunk, int32_t C, int32_t Tc, const float* noise,
+                        float* z, int32_t* indices, float* kl_loss, void* workspace, int64_t workspace_bytes,
+                        void* stream) {
+  return encode_chunk(cs, is_first, x_chunk, C, Tc, noise, z, indices, kl_loss, nullptr, workspace, workspace_bytes, stream);
 }
 
 int32_t vt_decode_chunk(vt_chunk_state* cs, int32_t is_first, const float* z_chunk, int32_t Cz, int32_t Tzc, float* x_out,
@@ -1762,9 +1768,28 @@ int32_t vt_decode_video_frames(const vt_model* m, int32_t Tz, int32_t t_chunk_de
   return total;
 }
 
-int32_t vt_encode_video(vt_model* m, int32_t precision, const float* x, int32_t x_on_host, int32_t B, int32_t C, int32_t T,
+// FSQ aux-loss partials of every chunk (vt_encode_video_fsq_aux): chunk i writes stats[2i..2i+1] and avg_prob[i*J ..)
+namespace {
+struct VideoAux {
+  float inv_t;
+  float* stats;
+  float* avg_prob;
+};
+// latent tokens of the longest chunk (the aux workspace is sized for it)
+long long video_max_chunk_tokens(const vt_model* m, int B, int T, int H, int W, int t_chunk) {
+  long long best = 0;
+  for (const ChunkSpan& c : chunk_schedule(T, t_chunk)) {
+    int Tz, Hz, Wz;
+    latent_shape(m, c.e - c.s, H, W, &Tz, &Hz, &Wz);
+    best = std::max(best, (long long)B * Tz * Hz * Wz);
+  }
+  return best;
+}
+}  // namespace
+
+static int encode_video(vt_model* m, int32_t precision, const float* x, int32_t x_on_host, int32_t B, int32_t C, int32_t T,
                         int32_t H, int32_t W, int32_t t_chunk_enc, const float* noise, float* z, int32_t* indices,
-                        float* kl_loss, void* workspace, int64_t workspace_bytes, void* stream) {
+                        float* kl_loss, const VideoAux* aux, void* workspace, int64_t workspace_bytes, void* stream) {
   if (!m || !x || !z || !workspace) return fail(VT_ERR_INVALID, "null argument");
   if (m->desc.version != 1) return fail(VT_ERR_INVALID, "temporal tiling exists only in the v1.1 model family");
   if (!m->finalized) return fail(VT_ERR_NOT_READY, "vt_model_finalize has not been called");
@@ -1800,6 +1825,16 @@ int32_t vt_encode_video(vt_model* m, int32_t precision, const float* x, int32_t 
   float* z_c = (float*)w; w += lat_b;
   int32_t* idx_c = (int32_t*)w; w += up1k((size_t)B * TzMax * Hz * Wz * 4);
   float* kl_c = (float*)w; w += up1k(4096);
+  float* h_c = nullptr;
+  void* aux_ws = nullptr;
+  FsqAuxGeom ag;
+  if (aux) {
+    if (d.regularizer != VT_REG_FSQ) return fail(VT_ERR_INVALID, "the FSQ aux loss needs an FSQ model");
+    const char* why = fsq_aux_geometry(d.z_channels, d.fsq_levels, video_max_chunk_tokens(m, B, T, H, W, t_chunk_enc), &ag);
+    if (why) return fail(VT_ERR_INVALID, "%s", why);
+    h_c = (float*)w; w += lat_b;
+    aux_ws = w; w += up1k(fsq_aux_workspace(ag));
+  }
   const int64_t ws_left = workspace_bytes - (w - (char*)workspace);
   if (ws_left <= 0) return fail(VT_ERR_WORKSPACE, "workspace too small for the chunk staging buffers");
   const size_t fr_in = (size_t)H * W * 4, fr_z = (size_t)Hz * Wz * 4;
@@ -1828,9 +1863,16 @@ int32_t vt_encode_video(vt_model* m, int32_t precision, const float* x, int32_t 
     if (ce == cudaSuccess && noise)
       ce = copy_frames_2d(noise_c, tzc, 0, noise, TzTot, tz0, (size_t)B * d.z_channels, tzc, fr_z, cudaMemcpyDeviceToDevice, s);
     if (ce != cudaSuccess) break;
-    rc = vt_encode_chunk(st, i == 0, stage[cur], C, n, noise ? noise_c : nullptr, z_c, indices ? idx_c : nullptr,
-                         d.regularizer == VT_REG_KL ? kl_c + i : nullptr, w, ws_left, stream);
+    rc = encode_chunk(st, i == 0, stage[cur], C, n, noise ? noise_c : nullptr, z_c, indices ? idx_c : nullptr,
+                      d.regularizer == VT_REG_KL ? kl_c + i : nullptr, h_c, w, ws_left, stream);
     if (rc) break;
+    if (aux) {
+      const char* why = fsq_aux_geometry(d.z_channels, d.fsq_levels, (long long)B * tzc * Hz * Wz, &ag);
+      if (why) { rc = fail(VT_ERR_INVALID, "%s", why); break; }
+      ce = launch_fsq_aux_partials(h_c, ag, d.fsq_levels, (long long)tzc * Hz * Wz, aux->inv_t, aux->stats + 2 * i,
+                                   aux->avg_prob + (size_t)i * ag.J, aux_ws, s);
+      if (ce != cudaSuccess) break;
+    }
     ce = cudaEventRecord(m->ev_free[cur], s);
     if (ce == cudaSuccess) ce = copy_frames_2d(z, TzTot, tz0, z_c, tzc, 0, (size_t)B * d.z_channels, tzc, fr_z, cudaMemcpyDeviceToDevice, s);
     if (ce == cudaSuccess && indices)
@@ -1849,6 +1891,38 @@ int32_t vt_encode_video(vt_model* m, int32_t precision, const float* x, int32_t 
   if (rc) return rc;
   if (ce != cudaSuccess) return fail(VT_ERR_CUDA, "vt_encode_video: %s", cudaGetErrorString(ce));
   return VT_OK;
+}
+
+int32_t vt_encode_video(vt_model* m, int32_t precision, const float* x, int32_t x_on_host, int32_t B, int32_t C, int32_t T,
+                        int32_t H, int32_t W, int32_t t_chunk_enc, const float* noise, float* z, int32_t* indices,
+                        float* kl_loss, void* workspace, int64_t workspace_bytes, void* stream) {
+  return encode_video(m, precision, x, x_on_host, B, C, T, H, W, t_chunk_enc, noise, z, indices, kl_loss, nullptr, workspace,
+                      workspace_bytes, stream);
+}
+
+int64_t vt_encode_video_fsq_aux_workspace_bytes(const vt_model* m, int32_t precision, int32_t B, int32_t T, int32_t H, int32_t W,
+                                                int32_t t_chunk_enc) {
+  const int64_t base = vt_encode_video_workspace_bytes(m, precision, B, T, H, W, t_chunk_enc);
+  if (base < 0) return -1;
+  const vt_model_desc& d = m->desc;
+  if (d.regularizer != VT_REG_FSQ) { fail(VT_ERR_INVALID, "the FSQ aux loss needs an FSQ model"); return -1; }
+  int max_len = 0;
+  for (const ChunkSpan& c : chunk_schedule(T, t_chunk_enc)) max_len = std::max(max_len, c.e - c.s);
+  int TzMax, Hz, Wz;
+  latent_shape(m, max_len, H, W, &TzMax, &Hz, &Wz);
+  FsqAuxGeom ag;
+  const char* why = fsq_aux_geometry(d.z_channels, d.fsq_levels, video_max_chunk_tokens(m, B, T, H, W, t_chunk_enc), &ag);
+  if (why) { fail(VT_ERR_INVALID, "%s", why); return -1; }
+  return base + (int64_t)up1k((size_t)B * d.z_channels * TzMax * Hz * Wz * 4) + (int64_t)up1k(fsq_aux_workspace(ag));
+}
+
+int32_t vt_encode_video_fsq_aux(vt_model* m, int32_t precision, const float* x, int32_t x_on_host, int32_t B, int32_t C, int32_t T,
+                                int32_t H, int32_t W, int32_t t_chunk_enc, float* z, int32_t* indices, float inv_temperature,
+                                float* aux_stats, float* aux_avg_prob, void* workspace, int64_t workspace_bytes, void* stream) {
+  if (!aux_stats || !aux_avg_prob) return fail(VT_ERR_INVALID, "null argument");
+  const VideoAux aux{inv_temperature, aux_stats, aux_avg_prob};
+  return encode_video(m, precision, x, x_on_host, B, C, T, H, W, t_chunk_enc, nullptr, z, indices, nullptr, &aux, workspace,
+                      workspace_bytes, stream);
 }
 
 int32_t vt_decode_video(vt_model* m, int32_t precision, const float* z, int32_t B, int32_t Cz, int32_t Tz, int32_t Hz, int32_t Wz,
@@ -2322,6 +2396,36 @@ int32_t vt_op_fsq(const float* h, int32_t d, const int32_t* levels, int64_t P, i
 int32_t vt_op_fsq_indices_to_codes(const int32_t* indices, int32_t d, const int32_t* levels, int64_t P, int32_t B,
                                    float* codes, void* stream) {
   VT_CUDA(launch_fsq_indices_to_codes(indices, d, levels, P, B, codes, (cudaStream_t)stream));
+  return VT_OK;
+}
+int64_t vt_fsq_aux_workspace_bytes(int32_t d, const int32_t* levels, int64_t tokens) {
+  if (!levels) { fail(VT_ERR_INVALID, "null argument"); return -1; }
+  FsqAuxGeom g;
+  const char* why = fsq_aux_geometry(d, levels, tokens, &g);
+  if (why) { fail(VT_ERR_INVALID, "%s", why); return -1; }
+  return (int64_t)fsq_aux_workspace(g);
+}
+int32_t vt_fsq_aux_partials(const float* h, int32_t d, const int32_t* levels, int64_t P, int32_t B, float inv_temperature,
+                            float* stats, float* avg_prob, void* workspace, int64_t workspace_bytes, void* stream) {
+  if (!h || !levels || !stats || !avg_prob || !workspace) return fail(VT_ERR_INVALID, "null argument");
+  if (B <= 0 || P <= 0) return fail(VT_ERR_INVALID, "bad shape");
+  FsqAuxGeom g;
+  const char* why = fsq_aux_geometry(d, levels, (long long)B * P, &g);
+  if (why) return fail(VT_ERR_INVALID, "%s", why);
+  if ((size_t)workspace_bytes < fsq_aux_workspace(g)) return fail(VT_ERR_WORKSPACE, "workspace too small for the FSQ aux loss");
+  VT_CUDA(launch_fsq_aux_partials(h, g, levels, P, inv_temperature, stats, avg_prob, workspace, (cudaStream_t)stream));
+  return VT_OK;
+}
+int32_t vt_fsq_aux_finalize(const float* stats, const float* avg_prob, int32_t n_segments, int32_t d, const int32_t* levels,
+                            int32_t world_size, float entropy_weight, float diversity_gamma, float commitment_weight,
+                            float* aux_loss, float* components, void* stream) {
+  if (!stats || !avg_prob || !levels || !aux_loss) return fail(VT_ERR_INVALID, "null argument");
+  if (n_segments <= 0 || world_size <= 0) return fail(VT_ERR_INVALID, "n_segments and world_size must be positive");
+  FsqAuxGeom g;
+  const char* why = fsq_aux_geometry(d, levels, 1, &g);
+  if (why) return fail(VT_ERR_INVALID, "%s", why);
+  VT_CUDA(launch_fsq_aux_finalize(stats, avg_prob, n_segments, g.J, world_size, entropy_weight, diversity_gamma, commitment_weight,
+                                  aux_loss, components, (cudaStream_t)stream));
   return VT_OK;
 }
 int32_t vt_op_kl(const float* h, const float* noise, int32_t zc, int64_t P, int32_t B, int32_t sample, float* z,

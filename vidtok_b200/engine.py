@@ -464,10 +464,21 @@ class DiagonalGaussianRegularizer(nn.Module):
         return out, {"kl_loss": kl}
 
 
+def _world_size() -> int:
+    """regularizers.py:49-64: avg_prob is all-reduced when torch.distributed runs with more than one rank."""
+    import torch.distributed as dist
+    if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+        return dist.get_world_size()
+    return 1
+
+
 class FSQRegularizer(nn.Module):
-    """vidtok.modules.regularizers.FSQRegularizer (regularizers.py:95-268), inference outputs only: `z` (codes) and
-    `reg_log['indices']`.  The entropy/commitment auxiliary loss (:232-245) is a training quantity that no inference
-    consumer reads (SURVEY.md section 0.7); `aux_loss` is returned as 0."""
+    """vidtok.modules.regularizers.FSQRegularizer (regularizers.py:95-268): `z` (codes), `reg_log['indices']` and
+    `reg_log['aux_loss']`.  The auxiliary loss (:232-245: clamped per-sample entropy, codebook entropy of the batch-mean
+    code distribution, commitment MSE) is computed on the device from one small softmax per latent channel
+    (csrc/fsq_aux.cu) instead of the tokens x codebook matrix; it is a device scalar (no host synchronisation).  As in the
+    reference it is computed whenever entropy_loss_weight or commitment_loss_weight is positive, in eval too, and avg_prob
+    is all-reduced over the ranks of an initialised torch.distributed group.  No gradient flows through it."""
 
     def __init__(self, levels: List[int], dim: Optional[int] = None, num_codebooks=1,
                  keep_num_codebooks_dim: Optional[bool] = None, scale: Optional[float] = None,
@@ -490,14 +501,72 @@ class FSQRegularizer(nn.Module):
         self.project_in = nn.Identity()
         self.project_out = nn.Identity()
         self.codebook_size = int(math.prod(self.levels))
+        self.scale = scale
         self.entropy_loss_weight = entropy_loss_weight
+        self.entropy_loss_annealing_steps = entropy_loss_annealing_steps
+        self.entropy_loss_annealing_factor = entropy_loss_annealing_factor
         self.commitment_loss_weight = commitment_loss_weight
+        self.diversity_gamma = diversity_gamma
 
     def get_trainable_parameters(self):
         return self.parameters()
 
     def _levels_c(self):
         return (C.c_int32 * len(self.levels))(*self.levels)
+
+    def calculate_entropy_loss_weight(self, n_steps):
+        """regularizers.py:200-204"""
+        if n_steps >= self.entropy_loss_annealing_steps:
+            return self.entropy_loss_weight
+        start = self.entropy_loss_annealing_factor * self.entropy_loss_weight
+        return start - (n_steps / self.entropy_loss_annealing_steps) * (start - self.entropy_loss_weight)
+
+    def aux_enabled(self) -> bool:
+        """regularizers.py:232: the auxiliary branch runs iff one of its weights is positive."""
+        return self.entropy_loss_weight > 0 or self.commitment_loss_weight > 0
+
+    def aux_partials(self, h: torch.Tensor, inv_temperature: float = 100.0) -> Tuple[torch.Tensor, torch.Tensor]:
+        """Per-segment partials of the auxiliary loss of one pre-bound latent h [B,d,...]: stats [1,2] = (per-sample
+        entropy, commitment MSE) and avg_prob [1,codebook_size]."""
+        hf = h.detach().float().contiguous()
+        B, P = hf.shape[0], hf[0, 0].numel()
+        lib = N.lib()
+        nbytes = int(lib.vt_fsq_aux_workspace_bytes(self.dim, self._levels_c(), B * P))
+        if nbytes < 0:
+            raise RuntimeError(f"vidtok_b200: {lib.vt_last_error().decode()}")
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=hf.device)
+        stats = torch.empty((1, 2), dtype=torch.float32, device=hf.device)
+        avg = torch.empty((1, self.codebook_size), dtype=torch.float32, device=hf.device)
+        N.check(lib.vt_fsq_aux_partials(_ptr(hf), self.dim, self._levels_c(), P, B, float(inv_temperature), _ptr(stats), _ptr(avg),
+                                        _ptr(ws), nbytes, _stream_ptr(hf.device)))
+        return stats, avg
+
+    def aux_finalize(self, stats: torch.Tensor, avg_prob: torch.Tensor, n_steps: int = 0, world_size: Optional[int] = None,
+                     components: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """aux_loss (a device scalar) from the partials of n segments (stats [n,2], avg_prob [n,codebook_size]): the mean
+        over the segments of (per_sample_entropy - diversity_gamma * codebook_entropy) * w(n_steps) + commit *
+        commitment_loss_weight.  world_size None: all-reduce avg_prob over the torch.distributed group when there is
+        one (in place, regularizers.py:49-59); an explicit world_size means avg_prob already holds the sum over the ranks.
+        components (optional, fp32 [n,4] on the device) receives each segment's (per_sample_entropy, codebook_entropy,
+        commit_loss, aux)."""
+        if world_size is None:
+            world_size = _world_size()
+            if world_size > 1:
+                import torch.distributed as dist
+                dist.all_reduce(avg_prob)
+        aux = torch.empty((), dtype=torch.float32, device=avg_prob.device)
+        N.check(N.lib().vt_fsq_aux_finalize(_ptr(stats), _ptr(avg_prob), int(stats.shape[0]), self.dim, self._levels_c(),
+                                            int(world_size), float(self.calculate_entropy_loss_weight(n_steps)),
+                                            float(self.diversity_gamma), float(self.commitment_loss_weight), _ptr(aux),
+                                            _ptr(components), _stream_ptr(avg_prob.device)))
+        return aux
+
+    def aux_loss(self, h: torch.Tensor, inv_temperature: float = 100.0, n_steps: int = 0) -> torch.Tensor:
+        """reg_log['aux_loss'] of one regularizer call on the pre-bound latent h (0 when both weights are 0)."""
+        if not self.aux_enabled():
+            return torch.zeros((), device=h.device)
+        stats, avg = self.aux_partials(h, inv_temperature)
+        return self.aux_finalize(stats, avg, n_steps)
 
     def indices_to_codes(self, indices: torch.Tensor, project_out=True) -> torch.Tensor:
         """regularizers.py:180-198: [B, ...] int -> [B, d, ...] for image/video shaped input, [..., d] otherwise."""
@@ -524,7 +593,7 @@ class FSQRegularizer(nn.Module):
         codes = torch.empty_like(zf)
         idx = torch.empty((B, *z.shape[2:]), dtype=torch.int32, device=z.device)
         N.check(N.lib().vt_op_fsq(_ptr(zf), self.dim, self._levels_c(), P, B, _ptr(codes), _ptr(idx), _stream_ptr(z.device)))
-        return codes.to(z.dtype), {"indices": idx, "aux_loss": torch.zeros((), device=z.device)}
+        return codes.to(z.dtype), {"indices": idx, "aux_loss": self.aux_loss(zf, inv_temperature, n_steps)}
 
 
 # --------------------------------------------------------------------------------------------------
@@ -704,9 +773,15 @@ class _EngineBase(nn.Module):
     def get_last_layer(self):
         return self.decoder.get_last_layer()
 
-    def _reg_log(self, idx, kl):
+    def _wants_aux(self, return_reg_log: bool) -> bool:
+        return return_reg_log and self.spec.regularizer == "fsq" and self.regularization.aux_enabled()
+
+    def _reg_log(self, idx, kl, h=None):
         if self.spec.regularizer == "fsq":
-            return {"indices": idx, "aux_loss": torch.zeros((), device=idx.device)}
+            # autoencoder.py:199 / autoencoder_v1_1.py:238: regularization(z, n_steps=self.global_step // 2)
+            aux = (self.regularization.aux_loss(h, n_steps=self.global_step // 2) if h is not None
+                   else torch.zeros((), device=idx.device))
+            return {"indices": idx, "aux_loss": aux}
         return {"kl_loss": kl}
 
     def indices_to_latent(self, token_indices: torch.Tensor) -> torch.Tensor:
@@ -720,10 +795,10 @@ class AutoencodingEngine(_EngineBase):
     _version = 0
 
     def encode(self, x: Any, return_reg_log: bool = False) -> Any:
-        z, idx, kl, _ = self._rt.encode_raw(x)
+        z, idx, kl, h = self._rt.encode_raw(x, want_h=self._wants_aux(return_reg_log))
         z = z.to(self._rt.out_dtype())
         if return_reg_log:
-            return z, self._reg_log(idx, kl)
+            return z, self._reg_log(idx, kl, h)
         return z
 
     def decode(self, z: Any, decode_from_indices: bool = False) -> torch.Tensor:
@@ -762,8 +837,8 @@ class AutoencodingEngineV11(_EngineBase):
         if self.use_tiling:
             z, reg_log = self.tile_encode(x)
         else:
-            z, idx, kl, _ = self._rt.encode_raw(x)
-            reg_log = self._reg_log(idx, kl)
+            z, idx, kl, h = self._rt.encode_raw(x, want_h=self._wants_aux(return_reg_log))
+            reg_log = self._reg_log(idx, kl, h)
         z = z.to(self._rt.out_dtype())
         if return_reg_log:
             return z, reg_log
@@ -797,6 +872,18 @@ class AutoencodingEngineV11(_EngineBase):
         z = torch.empty((B, self.spec.z_channels, Tz, Hz, Wz), dtype=torch.float32, device=dev)
         idx = torch.empty((B, Tz, Hz, Wz), dtype=torch.int32, device=dev) if self.spec.regularizer == "fsq" else None
         kl = torch.empty((), dtype=torch.float32, device=dev) if self.spec.regularizer == "kl" else None
+        reg = self.regularization
+        if self.spec.regularizer == "fsq" and reg.aux_enabled():
+            # one regularizer call per chunk (autoencoder_v1_1.py:253): the chunk loop writes each chunk's aux partials
+            stats = torch.empty((len(chunks), 2), dtype=torch.float32, device=dev)
+            avg = torch.empty((len(chunks), reg.codebook_size), dtype=torch.float32, device=dev)
+            ws = nat._workspace(int(lib.vt_encode_video_fsq_aux_workspace_bytes(nat.handle, prec, B, T, H, W, int(self.t_chunk_enc))))
+            N.check(lib.vt_encode_video_fsq_aux(nat.handle, prec, _ptr(x), int(on_host), B, Cin, T, H, W, int(self.t_chunk_enc), _ptr(z),
+                                                _ptr(idx), 100.0, _ptr(stats), _ptr(avg), _ptr(ws), ws.numel(), _stream_ptr(dev)))
+            if on_host:
+                torch.cuda.current_stream(dev).synchronize()
+            # per-chunk all-reduce of the reference = one all-reduce of all chunks' avg_prob; mean over the chunks (:261-264)
+            return z, {"aux_loss": reg.aux_finalize(stats, avg, n_steps=self.global_step // 2), "indices": idx}
         ws = nat._workspace(int(lib.vt_encode_video_workspace_bytes(nat.handle, prec, B, T, H, W, int(self.t_chunk_enc))))
         N.check(lib.vt_encode_video(nat.handle, prec, _ptr(x), int(on_host), B, Cin, T, H, W, int(self.t_chunk_enc), _ptr(noise), _ptr(z),
                                     _ptr(idx), _ptr(kl), _ptr(ws), ws.numel(), _stream_ptr(dev)))
