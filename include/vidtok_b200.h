@@ -148,7 +148,13 @@ int32_t vt_decode(vt_model* m, int32_t precision, const void* z, int32_t from_in
 
 /* ---- temporal tiling with causal caches (v1.1: tile_encode / tile_decode,
  *      autoencoder_v1_1.py:244-264,302-331; per-layer caches model_3dcausal_v1_1.py:159-178,216-236,
- *      289-302,325-343).  One state object per in-flight video. ---- */
+ *      289-302,325-343).  One state object per in-flight video.
+ *      Causal v1.0 models stream through the same calls: the first chunk has 1 (mod tdf) frames (it gets the tdf-1
+ *      replicated front frames and zero time padding, model_3dcausal.py:680-688), later chunks whole multiples of tdf;
+ *      decoding drops tdf-1 frames of the first chunk only (:883-885).  Every v1.0 norm and attention works within one
+ *      frame, so the concatenated chunk outputs equal the whole-clip encode / decode (bit for bit in VT_PREC_BF16 and
+ *      VT_PREC_FMA32; to fp32 rounding in the split-operand mode).  use_overlap is v1.1
+ *      only; non-causal models are rejected (a frame depends on later frames).  A v1.0 decoder state takes latents. ---- */
 typedef struct vt_chunk_state vt_chunk_state;
 int32_t vt_chunk_state_create(vt_model* m, int32_t precision, int32_t B, int32_t H, int32_t W, int32_t is_decoder,
                               int32_t use_overlap, vt_chunk_state** out);
@@ -276,6 +282,14 @@ int32_t vt_op_upsample_conv(int32_t precision, int32_t kind, const void* x, cons
 int32_t vt_op_tblock(const void* n1, const void* x, const float* w1, const float* b1, const float* g2, const float* be2,
                      const float* w2, const float* b2, const float* g3, const float* be3, int32_t out_silu, void* out,
                      void* out2, int32_t B, int32_t T, int32_t H, int32_t W, int32_t C, void* stream);
+/* vt_op_tblock continuing a video streamed chunk by chunk.  Caches: bf16 [B,2,H,W,C] (the layout the executor keeps for a
+ * temporal block's conv1 / conv2): n1_cache = the block input frames t-2, t-1 before this chunk, h_cache = its
+ * silu(LN2(conv1)) frames t-2, t-1.  Both inputs NULL: the video's first chunk (zero padding in front).  The outputs receive
+ * the same two frames after this chunk and must not alias the inputs. */
+int32_t vt_op_tblock_cached(const void* n1, const void* x, const float* w1, const float* b1, const float* g2, const float* be2,
+                            const float* w2, const float* b2, const float* g3, const float* be3, int32_t out_silu, void* out,
+                            void* out2, const void* n1_cache_in, const void* h_cache_in, void* n1_cache_out, void* h_cache_out,
+                            int32_t B, int32_t T, int32_t H, int32_t W, int32_t C, void* stream);
 /* y = silu?(norm(x)) over channels-last x [rows, C]; groupnorm variants take frame geometry. */
 int32_t vt_op_layernorm(int32_t precision, const void* x, const float* gamma, const float* beta, void* y,
                         int64_t rows, int32_t C, int32_t apply_silu, void* stream);

@@ -81,6 +81,7 @@ _SIGS = {
     "vt_op_head_planes": (_I32, [_P, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P]),
     "vt_op_upsample_conv": (_I32, [_I32, _I32, _P, _P, _P, C.c_float, _P, _P, _I32, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P]),
     "vt_op_tblock": (_I32, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I32, _P, _P, _I32, _I32, _I32, _I32, _I32, _P]),
+    "vt_op_tblock_cached": (_I32, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I32, _P, _P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _P]),
     "vt_op_layernorm": (_I32, [_I32, _P, _P, _P, _P, _I64, _I32, _I32, _P]),
     "vt_op_groupnorm": (_I32, [_I32, _P, _P, _P, _P, _I64, _I64, _I32, _I32, _I32, _P, _I64, _P]),
     "vt_op_attention": (_I32, [_I32, _P, _P, _P, _P, _I32, _I32, _I32, _P, _I64, _P]),

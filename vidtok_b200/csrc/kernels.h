@@ -161,10 +161,19 @@ int conv_tc_cluster_query(int smem, char* msg, int cap);
 
 // tblock_tc.cu: ResnetCausalBlock1D (k311 conv -> LayerNorm -> SiLU -> k311 conv + residual) for C = 128, v1.0 padding
 bool tblock_tc_supported(int B, int T, int H, int W, int C, bool planning = false);
+// Causal caches of a streamed video, bf16 [B,2,H,W,128] each: n1 = the block's input frames t-2, t-1, h = its LN2(h) frames
+// (conv2's input).  *_in null: the first chunk (zero padding in front); *_out receive the chunk's last two frames and must
+// not alias the inputs.
+struct TbCache {
+  const bf16* n1_in = nullptr;
+  const bf16* h_in = nullptr;
+  bf16* n1_out = nullptr;
+  bf16* h_out = nullptr;
+};
 cudaError_t launch_tblock_tc(const bf16* n1, const bf16* x, const bf16* w1, const float* bias1, const float* gamma2,
                              const float* beta2, const bf16* w2, const float* bias2, bf16* out, bf16* out2,
                              const float* gamma_out, const float* beta_out, bool out_silu, int B, int T, int H, int W,
-                             cudaStream_t s);
+                             cudaStream_t s, const TbCache* cache = nullptr);
 const char* tblock_tc_last_error();
 
 // conv_stem.cu (thread-built im2col A tile + wgmma for the Cin=3 stem)

@@ -1,7 +1,9 @@
 // Model construction (parameter manifest with the reference's checkpoint keys), weight repacking, and the
 // executor that walks the encoder/decoder stacks launching the kernels.  Host-side C++; the layer order follows
 // EncoderCausal3D.forward / DecoderCausal3D.forward (vidtok/modules/model_3dcausal.py:631-671,828-870) and the
-// chunked v1.1 variants (vidtok/modules/model_3dcausal_v1_1.py).
+// chunked v1.1 variants (vidtok/modules/model_3dcausal_v1_1.py).  Causal v1.0 models stream through the same chunk states:
+// per-layer caches replace the zero front padding, and since every v1.0 norm and attention works within one frame, a
+// streamed video computes the whole-clip function (bit for bit in BF16 / FMA32; see streaming.py for the split mode).
 #include "model.h"
 
 #include <algorithm>
@@ -299,6 +301,7 @@ struct vt_chunk_state {
   bool use_overlap = false;
   bool first = true;
   bool persist = true;           // false: one-shot "first chunk" context (untiled v1.1 forward)
+  // (v1.0 streams: a persistent state; the first chunk has zero padding in front, later chunks read the caches)
   std::map<std::string, vt::CacheBuf> caches;
   ~vt_chunk_state() {
     for (auto& kv : caches)
@@ -362,7 +365,7 @@ struct Exec {
   cudaStream_t s;
   Arena ar;
   bool dry;
-  vt_chunk_state* ck = nullptr;   // v1.1 chunk context (null for v1.0)
+  vt_chunk_state* ck = nullptr;   // v1.1 chunk context; for v1.0 only set while streaming (null: whole clip)
   int rc = VT_OK;
 
   Exec(vt_model* m_, int prec_, cudaStream_t s_, void* ws, size_t ws_bytes, bool dry_)
@@ -443,6 +446,63 @@ struct Exec {
     }
     return &c;
   }
+  // streaming: caches live across chunks (v1.1 tiling, v1.0 streams)
+  bool streaming() const { return ck && ck->persist; }
+  // dst [rows][2][fe] := the last two frames of [front (2 frames) | x (T frames)], rows of x T * fe apart; null front: zero
+  // frames (the causal padding in front of a first chunk)
+  void tail2(DType t, const void* x, const void* front, void* dst, long long rows, int T, long long fe) {
+    const size_t es = dtype_size(t);
+    for (int j = 0; j < 2 && ok(); ++j) {
+      char* d = (char*)dst + (size_t)j * fe * es;
+      if (T - 2 + j >= 0) cuda(launch_copy_frames(t, (const char*)x + (size_t)(T - 2 + j) * fe * es, d, (int)rows, (long long)T * fe, 2 * fe, fe, s), "cache tail");
+      else if (front) cuda(launch_copy_frames(t, (const char*)front + (size_t)(T + j) * fe * es, d, (int)rows, 2 * fe, 2 * fe, fe, s), "cache tail");
+      else cuda(cudaMemset2DAsync(d, 2 * fe * es, 0, fe * es, (size_t)rows, s), "cache tail");
+    }
+  }
+  // dst [rows][2 + T][fe] := [front (2 frames) | x (T frames)]
+  void cat2(DType t, const void* front, const void* x, void* dst, long long rows, int T, long long fe) {
+    const size_t es = dtype_size(t);
+    cuda(launch_copy_frames(t, front, dst, (int)rows, 2 * fe, (2 + T) * fe, 2 * fe, s), "cache cat");
+    cuda(launch_copy_frames(t, x, (char*)dst + 2 * fe * es, (int)rows, (long long)T * fe, (2 + T) * fe, (long long)T * fe, s), "cache cat");
+  }
+  // v1.0 stream, a conv whose input is the caller's fp32 NCDHW tensor (k = 3 in time): the cache holds the last two padded
+  // input frames in that layout; later chunks run over [cache | chunk] and drop the two cached output frames, so the conv
+  // kernel and its summation order are the whole clip's.
+  Act conv_ext_stream(const ConvW& w, const float* x, int B, int C, int T, int H, int W, int t_rep, const std::string& key, ConvOpt o) {
+    Act out;
+    const long long rows = (long long)B * C, fe = (long long)H * W;
+    CacheBuf* cb = get_cache(key, 2, (size_t)rows * 2 * fe * sizeof(float));
+    if (!ok()) return out;
+    Act in;
+    in.B = B; in.C = C; in.H = H; in.W = W;
+    if (ck->first) {
+      in.p = (void*)x; in.T = T;
+      o.ext_in = x; o.t_rep = t_rep;
+      out = conv(w, in, o);
+      if (ok() && !dry) {
+        if (t_rep > 0 && T == 1) {   // padded input [x0 ... x0]
+          for (int j = 0; j < 2; ++j)
+            cuda(launch_copy_frames(DT_F32, x, (float*)cb->buf[cb->cur ^ 1] + j * fe, (int)rows, fe, 2 * fe, fe, s), "cache tail");
+        } else {
+          tail2(DT_F32, x, nullptr, cb->buf[cb->cur ^ 1], rows, T, fe);
+        }
+      }
+    } else {
+      float* xc = (float*)alloc((size_t)rows * (2 + T) * fe * sizeof(float));
+      if (!ok()) return out;
+      if (!dry) {
+        if (!cb->valid) { rc = fail(VT_ERR_NOT_READY, "cache %s empty on a non-first chunk", key.c_str()); return out; }
+        cat2(DT_F32, cb->buf[cb->cur], x, xc, rows, T, fe);
+        tail2(DT_F32, x, cb->buf[cb->cur], cb->buf[cb->cur ^ 1], rows, T, fe);
+      }
+      in.p = xc; in.T = 2 + T;
+      o.ext_in = xc; o.to_off = 2;
+      out = conv(w, in, o);
+      ar.release(xc);
+    }
+    if (!dry) { cb->cur ^= 1; cb->valid = true; }
+    return out;
+  }
 
   // ---- convolution ----------------------------------------------------------------------------
   Act conv(const ConvW& w, const Act& in, const ConvOpt& o) {
@@ -504,8 +564,8 @@ struct Exec {
     p.t_mode = 0;
     CacheBuf* cb = nullptr;
     int cache_off = 0;
-    if (v11 && w.kt > 1) {
-      p.t_mode = 1;
+    if (v11 && w.kt > 1) p.t_mode = 1;
+    if (w.kt > 1 && (v11 || streaming())) {
       if (ck && o.cache_key && ck->persist) {
         cache_off = cache_offset_for(o.cache_key);
         cb = get_cache(o.cache_key, p.pt, (size_t)in.B * p.pt * in.frame() * dtype_size(o.ext_in ? DT_F32 : ta));
@@ -514,7 +574,7 @@ struct Exec {
           if (!dry && !cb->valid) { rc = fail(VT_ERR_NOT_READY, "causal cache %s empty on a non-first chunk", o.cache_key); return out; }
           p.t_mode = 2;
           p.cache = cb->buf[cb->cur];
-          p.cacheT = p.pt;
+          p.cacheT = p.pt;   // (folded 2x time upsampling: frames of the upsampled axis)
         }
       }
     }
@@ -530,14 +590,12 @@ struct Exec {
       if (o.res_mode == 3) {
         p.res_t_mode = 0;
         p.res_pool_off = o.res_pool_off;
-        if (v11) {
-          p.res_t_mode = 1;   // replicate (model_3dcausal_v1_1.py:293-294)
-          if (ck && ck->persist && o.cache_key) {
-            const std::string pk = std::string(o.cache_key) + "#pool";
-            CacheBuf* pc = get_cache(pk, 1, (size_t)r.B * r.frame() * dtype_size(ta));
-            if (!ok()) return out;
-            if (!ck->first) { p.res_t_mode = 2; p.res_cache = pc->buf[pc->cur]; }
-          }
+        if (v11) p.res_t_mode = 1;   // replicate (model_3dcausal_v1_1.py:293-294)
+        if (streaming() && o.cache_key) {
+          const std::string pk = std::string(o.cache_key) + "#pool";
+          CacheBuf* pc = get_cache(pk, 1, (size_t)r.B * r.frame() * dtype_size(ta));
+          if (!ok()) return out;
+          if (!ck->first) { p.res_t_mode = 2; p.res_cache = pc->buf[pc->cur]; }
         }
       }
     }
@@ -582,15 +640,27 @@ struct Exec {
       } else {
         if (!cuda(launch_conv_simt(p, tin, tout, ta, o.ext_in ? (const void*)o.ext_in : in.p, w.w_kn, out.p, s), "conv_simt")) return out;
       }
-      // v1.1: cache := tail of the padded input (after the conv consumed the old cache)
+      // cache := tail of the padded input (after the conv consumed the old cache)
       if (cb) {
         const int nxt = cb->cur ^ 1;
-        if (!cuda(launch_cache_update(tin, o.ext_in ? (const void*)o.ext_in : in.p, cb->buf[cb->cur], cb->buf[nxt], in.B, in.T,
-                                      p.pt, cache_off, ck->first, in.frame(), o.ext_in ? p.isB : p.isB / cw, s), "cache_update")) return out;
+        if (o.ut == 2) {
+          // v1.0 folded 2x time upsampling: the last two upsampled frames are the last input frame twice
+          const char* last = (const char*)in.p + (size_t)(in.T - 1) * in.frame() * dtype_size(tin);
+          for (int j = 0; j < 2 && ok(); ++j)
+            cuda(launch_copy_frames(tin, last, (char*)cb->buf[nxt] + (size_t)j * in.frame() * dtype_size(tin), in.B, (long long)in.T * in.frame(),
+                                    2 * in.frame(), in.frame(), s), "cache_update");
+          if (!ok()) return out;
+        } else {
+          // v1.0: zero frames in front of the first chunk (v1.1 replicates frame 0)
+          const bool zero_front = !v11 && ck->first;
+          if (zero_front && !cuda(cudaMemsetAsync(cb->buf[cb->cur], 0, cb->bytes, s), "cache_update")) return out;
+          if (!cuda(launch_cache_update(tin, o.ext_in ? (const void*)o.ext_in : in.p, cb->buf[cb->cur], cb->buf[nxt], in.B, in.T,
+                                        p.pt, cache_off, ck->first && !zero_front, in.frame(), o.ext_in ? p.isB : p.isB / cw, s), "cache_update")) return out;
+        }
         cb->cur = nxt;
         cb->valid = true;
       }
-      if (o.res_mode == 3 && v11 && ck && ck->persist && o.cache_key) {
+      if (o.res_mode == 3 && streaming() && o.cache_key) {
         // avg-pool branch cache = last frame of the padded input (model_3dcausal_v1_1.py:298)
         CacheBuf& pc = ck->caches[std::string(o.cache_key) + "#pool"];
         const Act& r = *o.res;
@@ -660,14 +730,31 @@ struct Exec {
     if (prec != VT_PREC_BF16 || m->desc.version != 0 || m->desc.noncausal || m->desc.norm_type != VT_NORM_LAYERNORM) return false;
     if (r.c1.Ci != 128 || r.c1.Co != 128 || r.c2.Co != 128 || !r.c1.w_nk || !r.c2.w_nk || r.c1.kt != 3 || r.c1.kh != 1) return false;
     if (!tblock_tc_supported(st.x.B, st.x.T, st.x.H, st.x.W, st.x.C, dry)) return false;
+    // streaming: the conv1 / conv2 caches of the two-launch path (n1 and LN2(h) frames t-2, t-1), read and written in-kernel
+    CacheBuf* cc[2] = {nullptr, nullptr};
+    TbCache tc;
+    if (streaming()) {
+      const size_t cbytes = (size_t)st.x.B * 2 * st.x.frame() * sizeof(bf16);
+      cc[0] = get_cache(r.key + ".conv1", 2, cbytes);
+      if (ok()) cc[1] = get_cache(r.key + ".conv2", 2, cbytes);
+      if (!ok()) return true;
+      if (!ck->first) {
+        if (!dry && (!cc[0]->valid || !cc[1]->valid)) { rc = fail(VT_ERR_NOT_READY, "causal cache %s empty on a non-first chunk", r.key.c_str()); return true; }
+        tc.n1_in = (const bf16*)cc[0]->buf[cc[0]->cur]; tc.h_in = (const bf16*)cc[1]->buf[cc[1]->cur];
+      }
+      tc.n1_out = (bf16*)cc[0]->buf[cc[0]->cur ^ 1]; tc.h_out = (bf16*)cc[1]->buf[cc[1]->cur ^ 1];
+    }
     Act n1 = take_norm(st, r.n1, true, true);
     Act out = new_act(st.x.B, st.x.T, st.x.H, st.x.W, 128);
     Act out2;
     if (next) out2 = new_act(st.x.B, st.x.T, st.x.H, st.x.W, 128);
-    if (ok() && !dry)
+    if (ok() && !dry) {
       cuda(launch_tblock_tc((const bf16*)n1.p, (const bf16*)st.x.p, r.c1.w_nk, r.c1.bias, r.n2.gamma, r.n2.beta, r.c2.w_nk, r.c2.bias,
                             (bf16*)out.p, next ? (bf16*)out2.p : nullptr, next ? next->gamma : nullptr, next ? next->beta : nullptr,
-                            next_silu, st.x.B, st.x.T, st.x.H, st.x.W, s), tblock_tc_last_error());
+                            next_silu, st.x.B, st.x.T, st.x.H, st.x.W, s, cc[0] ? &tc : nullptr), tblock_tc_last_error());
+      for (CacheBuf* c : cc)
+        if (c) { c->cur ^= 1; c->valid = true; }
+    }
     free_act(n1);
     if (st.n.p) free_act(st.n);
     free_act(st.x);
@@ -887,6 +974,8 @@ struct Exec {
           ConvOpt op;
           op.ra = lv.alpha; op.rb = 1.f - lv.alpha; op.res_mode = 1; op.res = &x;
           if (m->desc.noncausal) { op.pt_front = pt == 0 ? 1 : 0; op.pt_back = pt == 0 ? 0 : 1; }   // frames (i-1, i) / (i, i+1)
+          const std::string pk = ckey + (pt ? "#ph1" : "#ph0");   // streaming: each parity keeps its own copy of x[-1]
+          op.cache_key = pk.c_str();
           const size_t off = (size_t)(pt * fr) * dtype_size(ta);
           op.out_view = dry ? out.p : (void*)((char*)out.p + off);
           op.ov_sW = (long long)lv.tconv.Co * cw; op.ov_sH = (long long)x.W * lv.tconv.Co * cw; op.ov_sT = 2 * fr * cw; op.ov_sB = 2 * fr * x.T * cw;
@@ -1036,10 +1125,9 @@ static void run_encoder(Exec& ex, const float* x_ext, int B, int T, int H, int W
   xin.p = (void*)x_ext; xin.B = B; xin.T = T; xin.H = H; xin.W = W; xin.C = d.in_channels;
   Exec::Stream st;
   const bf16* stem_w = ex.split ? e.conv_in.w_stem3 : e.conv_in.w_stem;
-  if (d.version == 1 && ex.ck && ex.ck->persist && ex.tcm && stem_w && T + t_rep >= 2 &&
-      e.conv_in.Ci * 27 <= 128) {
-    // chunked v1.1 on the stem kernel: the causal cache (last two padded input frames, model_3dcausal_v1_1.py:230-233)
-    // is kept in the caller's layout (fp32 [B,C,2,H,W]) and read by the kernel's patch loader
+  if (ex.streaming() && ex.tcm && stem_w && T + t_rep >= 2 && e.conv_in.Ci * 27 <= 128) {
+    // chunked v1.1 / streamed v1.0 on the stem kernel: the causal cache (last two padded input frames,
+    // model_3dcausal_v1_1.py:230-233) is kept in the caller's layout (fp32 [B,C,2,H,W]) and read by the kernel's patch loader
     CacheBuf* cb = ex.get_cache("encoder.conv_in#stem", 2, (size_t)B * d.in_channels * 2 * H * W * sizeof(float));
     st.x = ex.new_act(B, T + t_rep, H, W, e.conv_in.Co);
     if (ex.ok() && !ex.dry) {
@@ -1054,7 +1142,7 @@ static void run_encoder(Exec& ex, const float* x_ext, int B, int T, int H, int W
       p.osC = 1; p.osW = (long long)p.Co * ex.cw; p.osH = (long long)W * p.osW; p.osT = p.osH * H; p.osB = p.osT * p.To;
       p.kt = p.kh = p.kw = 3; p.st = p.sh = p.sw = 1; p.ut = p.uh = p.uw = 1;
       p.pt = 2; p.ph = 1; p.pw = 1; p.t_rep = t_rep;
-      p.t_mode = ex.ck->first ? 1 : 2;
+      p.t_mode = ex.ck->first ? (d.version == 1 ? 1 : 0) : 2;   // first chunk: replicate (v1.1) / zero (v1.0) padding
       p.cache = cb->buf[cb->cur]; p.cacheT = 2;
       p.bias = e.conv_in.bias;
       if (!conv_stem_supported(p)) { ex.rc = fail(VT_ERR_INVALID, "stem kernel rejected the chunk geometry"); return; }
@@ -1072,6 +1160,8 @@ static void run_encoder(Exec& ex, const float* x_ext, int B, int T, int H, int W
     ConvOpt o; o.cache_key = "encoder.conv_in";
     st.x = ex.conv(e.conv_in, xp, o);
     ex.free_act(xp);
+  } else if (ex.streaming()) {
+    st.x = ex.conv_ext_stream(e.conv_in, x_ext, B, d.in_channels, T, H, W, t_rep, "encoder.conv_in", ConvOpt());
   } else {
     ConvOpt o; o.ext_in = x_ext; o.t_rep = t_rep;
     st.x = ex.conv(e.conv_in, xin, o);
@@ -1116,6 +1206,9 @@ static void run_decoder(Exec& ex, const float* z_ext, int B, int Tz, int Hz, int
     ConvOpt o; o.cache_key = "decoder.conv_in";
     st.x = ex.conv(g.conv_in, zp, o);
     ex.free_act(zp);
+  } else if (ex.streaming()) {
+    if (z_is_indices) { ex.rc = fail(VT_ERR_INVALID, "a decoder stream takes latents, not token indices"); return; }
+    st.x = ex.conv_ext_stream(g.conv_in, z_ext, B, d.z_channels, Tz, Hz, Wz, 0, "decoder.conv_in", ConvOpt());
   } else {
     ConvOpt o; o.ext_in = z_ext; o.ext_in_indices = z_is_indices;
     st.x = ex.conv(g.conv_in, zin, o);
@@ -1143,14 +1236,38 @@ static void run_decoder(Exec& ex, const float* z_ext, int B, int Tz, int Hz, int
     // 27 x 4 per-tap partial outputs by one GEMM over the input, then a gather-add of the shifted partials
     Act P = ex.conv(m->head_planes, n, ConvOpt());
     ex.free_act(n);
-    if (ex.ok() && !ex.dry)
+    if (ex.ok() && ex.streaming()) {
+      // streamed v1.0: the cache holds the planes of the last two input frames; later chunks gather over [cache | planes]
+      const long long fe = (long long)P.H * P.W * 128;
+      CacheBuf* cb = ex.get_cache("decoder.conv_out#planes", 2, (size_t)P.B * 2 * fe * sizeof(bf16));
+      if (!ex.ok()) return;
+      if (ex.ck->first) {
+        if (!ex.dry) {
+          ex.cuda(launch_tap_planes_gather((const bf16*)P.p, g.conv_out.bias, x_out, P.B, P.T, P.H, P.W, 128, g.conv_out.Co,
+                                           d.time_downsample_factor - 1, ex.s), "tap_planes_gather");
+          ex.tail2(DT_BF16, P.p, nullptr, cb->buf[cb->cur ^ 1], P.B, P.T, fe);
+        }
+      } else {
+        bf16* Pc = (bf16*)ex.alloc((size_t)P.B * (2 + P.T) * fe * sizeof(bf16));
+        if (ex.ok() && !ex.dry) {
+          if (!cb->valid) { ex.rc = fail(VT_ERR_NOT_READY, "decoder head cache empty on a non-first chunk"); return; }
+          ex.cat2(DT_BF16, cb->buf[cb->cur], P.p, Pc, P.B, P.T, fe);
+          ex.tail2(DT_BF16, P.p, cb->buf[cb->cur], cb->buf[cb->cur ^ 1], P.B, P.T, fe);
+          ex.cuda(launch_tap_planes_gather(Pc, g.conv_out.bias, x_out, P.B, 2 + P.T, P.H, P.W, 128, g.conv_out.Co, 2, ex.s), "tap_planes_gather");
+        }
+        ex.ar.release(Pc);
+      }
+      if (!ex.dry) { cb->cur ^= 1; cb->valid = true; }
+    } else if (ex.ok() && !ex.dry) {
       ex.cuda(launch_tap_planes_gather((const bf16*)P.p, g.conv_out.bias, x_out, P.B, P.T, P.H, P.W, 128, g.conv_out.Co,
                                        d.noncausal ? 0 : d.time_downsample_factor - 1, ex.s, d.noncausal ? 1 : 2), "tap_planes_gather");
+    }
     ex.free_act(P);
     return;
   }
   ConvOpt o; o.ext_out = x_out; o.cache_key = "decoder.conv_out";
-  if (d.version == 0 && !d.noncausal) o.to_off = d.time_downsample_factor - 1;  // model_3dcausal.py:883-885
+  // model_3dcausal.py:883-885 (a stream drops the frames once, in its first chunk)
+  if (d.version == 0 && !d.noncausal && (!ex.streaming() || ex.ck->first)) o.to_off = d.time_downsample_factor - 1;
   ex.conv(g.conv_out, n, o);
   ex.free_act(n);
 }
@@ -1480,6 +1597,23 @@ static int check_hw(const vt_model* m, int H, int W) {
   return VT_OK;
 }
 
+static int spatial_factor(const vt_model* m) {
+  int f = 1;
+  for (int l = 0; l < m->desc.num_levels; ++l)
+    if (contains(m->spatial_ds, l)) f *= 2;
+  return f;
+}
+// v1.0 streams: the whole clip's time padding is replicated tdf-1 frames, then stride-2 resampling, so the first chunk
+// must have 1 (mod tdf) frames and later chunks whole groups of tdf frames
+static int check_stream_chunk(const vt_model* m, bool first, int Tc) {
+  if (m->desc.version != 0) return VT_OK;
+  const int tdf = m->desc.time_downsample_factor;
+  if (first ? (Tc % tdf != 1 % tdf) : (Tc % tdf != 0))
+    return fail(VT_ERR_INVALID, "a v1.0 stream takes 1 (mod %d) frames in its first chunk and multiples of %d after it, got %d", tdf, tdf, Tc);
+  if (first && Tc + (tdf - 1) < 2) return fail(VT_ERR_INVALID, "the first chunk of a v1.0 stream needs two padded frames");
+  return VT_OK;
+}
+
 static int check_precision(int precision) {
   if (precision < 0 || precision > VT_PREC_MIXED) return fail(VT_ERR_INVALID, "unknown precision mode %d", precision);
   return VT_OK;
@@ -1580,8 +1714,12 @@ int32_t vt_decode(vt_model* m, int32_t precision, const void* z, int32_t from_in
 int32_t vt_chunk_state_create(vt_model* m, int32_t precision, int32_t B, int32_t H, int32_t W, int32_t is_decoder,
                               int32_t use_overlap, vt_chunk_state** out) {
   if (!m || !out) return fail(VT_ERR_INVALID, "null argument");
-  if (m->desc.version != 1) return fail(VT_ERR_INVALID, "temporal tiling exists only in the v1.1 model family");
+  if (m->desc.noncausal)
+    return fail(VT_ERR_INVALID, "non-causal models cannot stream: their time padding is symmetric, so a frame depends on later frames");
+  if (m->desc.version == 0 && use_overlap) return fail(VT_ERR_INVALID, "overlap look-ahead exists only in the v1.1 model family");
   if (check_precision(precision)) return VT_ERR_INVALID;
+  if (B <= 0 || H <= 0 || W <= 0) return fail(VT_ERR_INVALID, "bad shape");
+  if (check_hw(m, H * (is_decoder ? spatial_factor(m) : 1), W * (is_decoder ? spatial_factor(m) : 1))) return VT_ERR_INVALID;
   vt_chunk_state* st = new vt_chunk_state();
   st->m = m; st->prec = precision; st->B = B; st->H = H; st->W = W;
   st->is_decoder = is_decoder != 0; st->use_overlap = use_overlap != 0;
@@ -1626,6 +1764,9 @@ static int encode_chunk(vt_chunk_state* cs, int32_t is_first, const float* x_chu
   if (!m->finalized) return fail(VT_ERR_NOT_READY, "vt_model_finalize has not been called");
   VT_CUDA(cudaSetDevice(m->device));
   cudaStream_t s = (cudaStream_t)stream;
+  if (Tc <= 0) return fail(VT_ERR_INVALID, "bad shape");
+  int rc0 = check_stream_chunk(m, is_first != 0, Tc);
+  if (rc0) return rc0;
   cs->first = is_first != 0;
   int Tz, Hz, Wz;
   latent_shape(m, Tc, cs->H, cs->W, &Tz, &Hz, &Wz);
@@ -1655,6 +1796,7 @@ int32_t vt_decode_chunk(vt_chunk_state* cs, int32_t is_first, const float* z_chu
   vt_model* m = cs->m;
   if (Cz != m->desc.z_channels) return fail(VT_ERR_INVALID, "latent has %d channels, the model expects z_channels = %d", Cz, m->desc.z_channels);
   if (!m->finalized) return fail(VT_ERR_NOT_READY, "vt_model_finalize has not been called");
+  if (Tzc <= 0) return fail(VT_ERR_INVALID, "bad shape");
   VT_CUDA(cudaSetDevice(m->device));
   cs->first = is_first != 0;
   Exec ex(m, stack_prec(cs->prec, true), (cudaStream_t)stream, workspace, (size_t)workspace_bytes, false);
@@ -2301,9 +2443,9 @@ int32_t vt_op_upsample_conv(int32_t precision, int32_t kind, const void* x, cons
 }
 
 // Fused temporal residual block (BF16, C = 128) exactly as the model path launches it.
-int32_t vt_op_tblock(const void* n1, const void* x, const float* w1, const float* b1, const float* g2, const float* be2,
-                     const float* w2, const float* b2, const float* g3, const float* be3, int32_t out_silu, void* out,
-                     void* out2, int32_t B, int32_t T, int32_t H, int32_t W, int32_t C, void* stream) {
+static int32_t op_tblock(const void* n1, const void* x, const float* w1, const float* b1, const float* g2, const float* be2,
+                         const float* w2, const float* b2, const float* g3, const float* be3, int32_t out_silu, void* out,
+                         void* out2, int32_t B, int32_t T, int32_t H, int32_t W, int32_t C, void* stream, const TbCache* cache) {
   if (!n1 || !x || !w1 || !b1 || !g2 || !be2 || !w2 || !b2 || !out) return fail(VT_ERR_INVALID, "null argument");
   if (!tblock_tc_supported(B, T, H, W, C)) return fail(VT_ERR_INVALID, "fused temporal block does not take this geometry: %s", tblock_tc_last_error());
   cudaStream_t s = (cudaStream_t)stream;
@@ -2313,11 +2455,26 @@ int32_t vt_op_tblock(const void* n1, const void* x, const float* w1, const float
   VT_CUDA(launch_pack_w_nk_bf16(w1, wp, C, C, C, 3, 3 * C, s));
   VT_CUDA(launch_pack_w_nk_bf16(w2, wp + per, C, C, C, 3, 3 * C, s));
   cudaError_t er = launch_tblock_tc((const bf16*)n1, (const bf16*)x, wp, b1, g2, be2, wp + per, b2, (bf16*)out, (bf16*)out2,
-                                    out2 ? g3 : nullptr, out2 ? be3 : nullptr, out_silu != 0, B, T, H, W, s);
+                                    out2 ? g3 : nullptr, out2 ? be3 : nullptr, out_silu != 0, B, T, H, W, s, cache);
   cudaError_t e2 = cudaStreamSynchronize(s);
   cudaFree(wp);
   if (er != cudaSuccess || e2 != cudaSuccess) return fail(VT_ERR_CUDA, "tblock: %s %s", cudaGetErrorString(er != cudaSuccess ? er : e2), tblock_tc_last_error());
   return VT_OK;
+}
+int32_t vt_op_tblock(const void* n1, const void* x, const float* w1, const float* b1, const float* g2, const float* be2,
+                     const float* w2, const float* b2, const float* g3, const float* be3, int32_t out_silu, void* out,
+                     void* out2, int32_t B, int32_t T, int32_t H, int32_t W, int32_t C, void* stream) {
+  return op_tblock(n1, x, w1, b1, g2, be2, w2, b2, g3, be3, out_silu, out, out2, B, T, H, W, C, stream, nullptr);
+}
+int32_t vt_op_tblock_cached(const void* n1, const void* x, const float* w1, const float* b1, const float* g2, const float* be2,
+                            const float* w2, const float* b2, const float* g3, const float* be3, int32_t out_silu, void* out,
+                            void* out2, const void* n1_cache_in, const void* h_cache_in, void* n1_cache_out, void* h_cache_out,
+                            int32_t B, int32_t T, int32_t H, int32_t W, int32_t C, void* stream) {
+  if (!n1_cache_out || !h_cache_out) return fail(VT_ERR_INVALID, "null cache output");
+  if (!n1_cache_in != !h_cache_in) return fail(VT_ERR_INVALID, "pass both input caches (a continued video) or neither (its first chunk)");
+  TbCache c;
+  c.n1_in = (const bf16*)n1_cache_in; c.h_in = (const bf16*)h_cache_in; c.n1_out = (bf16*)n1_cache_out; c.h_out = (bf16*)h_cache_out;
+  return op_tblock(n1, x, w1, b1, g2, be2, w2, b2, g3, be3, out_silu, out, out2, B, T, H, W, C, stream, &c);
 }
 
 int32_t vt_op_layernorm(int32_t precision, const void* x, const float* gamma, const float* beta, void* y, int64_t rows,

@@ -13,7 +13,14 @@
 //          layout (the layout a TMA load would have produced), then fence.proxy.async: the ring is the next A operand
 //   G2(t): acc = sum_a W2[a] . H[t-2+a]            A = the shared-memory ring, B (W2 slice) by TMA
 //   E2(t): out[t] = acc + b2 + x[t]; optionally out2[t] = act(LN_next(out[t])) for the next stage
-// Causal zero padding = skipped taps.  Warp roles: warps 0-7 = two consumer warpgroups, warp 8 = TMA producer (its warpgroup
+// Causal zero padding = skipped taps.
+//
+// Cached variant (kCache, a video streamed chunk by chunk): the taps in front of frame 0 read the previous chunk's last two
+// n1 frames (G1) and the ring slots of frames -2, -1 are preloaded from its last two LN2(h) frames (G2), so a chunk computes
+// exactly what the whole clip computes for those frames.  After its last frame each strip writes the chunk's last two n1 and
+// LN2(h) frames as the next caches (for a one-frame chunk, part old cache and part new frame).  Without input caches (the
+// first chunk) the taps in front of frame 0 are zero padding, as in the uncached kernel.  Cache layout: bf16 [B,2,H,W,128],
+// the buffers the two-launch path keeps for conv1 / conv2.  Warp roles: warps 0-7 = two consumer warpgroups, warp 8 = TMA producer (its warpgroup
 // hands its registers to the consumers through setmaxnreg).
 #include <cuda.h>
 
@@ -56,9 +63,16 @@ struct TbParams {
   const bf16* x;
   bf16* out;
   bf16* out2;
+  // kCache only
+  const bf16* n1;
+  int cached_in;             // cn1_in / ch_in hold frames -2, -1 (else zero padding: the first chunk)
+  const bf16* cn1_in;
+  const bf16* ch_in;
+  bf16* cn1_out;
+  bf16* ch_out;
 };
 struct TbMaps {
-  CUtensorMap n1, w1, w2;
+  CUtensorMap n1, w1, w2, cn1;
 };
 
 __device__ __forceinline__ float quad_sum(float v) {
@@ -69,6 +83,7 @@ __device__ __forceinline__ float quad_sum(float v) {
 
 // smem layout from the 1024-aligned base:
 //   [H ring: 3 slots x kKc tiles][stage ring: stages x (A tile | B tile)][barriers][constants]
+template <bool kCache>
 __global__ void __launch_bounds__(kThreadsTb, 1) tblock_tc_kernel(const __grid_constant__ TbMaps maps, const TbParams p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -105,6 +120,7 @@ __global__ void __launch_bounds__(kThreadsTb, 1) tblock_tc_kernel(const __grid_c
     // ===================== TMA producer: per frame the G1 steps (n1 tile + W1 slice), then the G2 steps (W2 slice) =====
     const bool el = elect_one();
     if (el) { prefetch_tmap(&maps.n1); prefetch_tmap(&maps.w1); prefetch_tmap(&maps.w2); }
+    const bool front = kCache && p.cached_in;   // taps in front of frame 0 read the caches
     int stage = 0;
     uint32_t phase = 0;
     auto acquire = [&](uint32_t bytes) {
@@ -119,19 +135,21 @@ __global__ void __launch_bounds__(kThreadsTb, 1) tblock_tc_kernel(const __grid_c
       const int w0 = tw * p.BW, h0 = th * p.BH;
       for (int t = 0; t < p.T; ++t) {
         for (int a = 0; a < 3; ++a) {
-          if (t - 2 + a < 0) continue;
+          const int tv = t - 2 + a;
+          if (tv < 0 && !front) continue;
           for (int kc = 0; kc < kKc; ++kc) {
             acquire(2u * kTile);
             if (el) {
               const uint32_t sa = ring_base + stage * stage_bytes;
-              tma_load_5d(sa, &maps.n1, full_bar(stage), kc * 64, w0, h0, t - 2 + a, b);
+              if (kCache && tv < 0) tma_load_5d(sa, &maps.cn1, full_bar(stage), kc * 64, w0, h0, tv + 2, b);
+              else tma_load_5d(sa, &maps.n1, full_bar(stage), kc * 64, w0, h0, tv, b);
               tma_load_3d(sa + kTile, &maps.w1, full_bar(stage), a * kC + kc * 64, 0, 0);
             }
             advance();
           }
         }
         for (int a = 0; a < 3; ++a) {
-          if (t - 2 + a < 0) continue;
+          if (t - 2 + a < 0 && !front) continue;
           for (int kc = 0; kc < kKc; ++kc) {
             acquire(kTile);
             if (el) tma_load_3d(ring_base + stage * stage_bytes + kTile, &maps.w2, full_bar(stage), a * kC + kc * 64, 0, 0);
@@ -182,6 +200,14 @@ __global__ void __launch_bounds__(kThreadsTb, 1) tblock_tc_kernel(const __grid_c
   const float* b3 = cst + 5 * kC;
   const int cq = 2 * (lane & 3);
   const int rbase = 64 * g + 16 * wq + (lane >> 2);   // this thread's rows: rbase and rbase + 8
+  const bool front = kCache && p.cached_in;
+  const int gtid = threadIdx.x & 127;
+  // ring slot of frame tv >= -2
+  auto slot_of = [&](int tv) { return h_base + (uint32_t)((tv + kHSlots) % kHSlots) * kKc * kTile; };
+  // 16-byte unit (8 channels from c) of ring row `row` in the canonical K-major SWIZZLE_128B layout
+  auto ring_unit = [&](uint32_t slot, int row, int c) {
+    return reinterpret_cast<uint4*>(smem_gen + (slot - smem_base) + (c >> 6) * kTile + row * 128 + ((((c & 63) >> 3) ^ (row & 7)) << 4));
+  };
 
   for (long long strip = blockIdx.x; strip < p.num_strips; strip += gridDim.x) {
     const int tw = (int)(strip % p.tilesW);
@@ -195,11 +221,29 @@ __global__ void __launch_bounds__(kThreadsTb, 1) tblock_tc_kernel(const __grid_c
       pos0[r] = (((long long)b * p.T) * p.H + h) * p.W + w;
     }
     const long long frame = (long long)p.H * p.W;
+    // position (b, h, w) of unit i of this warpgroup's 64 rows (16 units of 8 channels per row) in a [B,2,H,W,128] cache
+    auto cache_pos = [&](int i, int j, int& row) {
+      row = 64 * g + (i >> 4);
+      const int h = th * p.BH + row / p.BW, w = tw * p.BW + row % p.BW;
+      return ((((long long)b * 2 + j) * p.H + h) * p.W + w) * kC + (i & 15) * 8;
+    };
+    if (front) {
+      // ring slots of frames -2, -1 := the LN2(h) cache
+      wg_sync();   // every warp of the group is done with the previous strip's ring
+      for (int j = 0; j < 2; ++j)
+        for (int i = gtid; i < 64 * 16; i += 128) {
+          int row;
+          const long long off = cache_pos(i, j, row);
+          *ring_unit(slot_of(j - 2), row, (i & 15) * 8) = *reinterpret_cast<const uint4*>(p.ch_in + off);
+        }
+      fence_async_smem();
+      wg_sync();
+    }
     for (int t = 0; t < p.T; ++t) {
       // ---- G1(t)
       uint32_t scale = 0;
       for (int a = 0; a < 3; ++a) {
-        if (t - 2 + a < 0) continue;
+        if (t - 2 + a < 0 && !front) continue;
         for (int kc = 0; kc < kKc; ++kc) { kstep(true, 0u, scale); scale = 1; }
       }
       finish();
@@ -245,8 +289,8 @@ __global__ void __launch_bounds__(kThreadsTb, 1) tblock_tc_kernel(const __grid_c
       scale = 0;
       for (int a = 0; a < 3; ++a) {
         const int tv = t - 2 + a;
-        if (tv < 0) continue;
-        const uint32_t hs = h_base + (uint32_t)(tv % kHSlots) * kKc * kTile + (uint32_t)g * 64u * 128u;
+        if (tv < 0 && !front) continue;
+        const uint32_t hs = (kCache ? slot_of(tv) : h_base + (uint32_t)(tv % kHSlots) * kKc * kTile) + (uint32_t)g * 64u * 128u;
         for (int kc = 0; kc < kKc; ++kc) { kstep(false, hs + (uint32_t)kc * kTile, scale); scale = 1; }
       }
       finish();
@@ -287,6 +331,24 @@ __global__ void __launch_bounds__(kThreadsTb, 1) tblock_tc_kernel(const __grid_c
             y1 = fmaf(y1, tanh_approx(y1), y1);
           }
           *reinterpret_cast<uint32_t*>(o2 + c) = pack_bf16x2(y0, y1);
+        }
+      }
+    }
+    if (kCache) {
+      // next caches: frames T-2, T-1 of [cache | chunk] (zero padding in front of the first chunk).  The LN2(h) frames are
+      // in the ring: the last E1 was followed by a group barrier, and the next write to the ring comes after another.
+      for (int j = 0; j < 2; ++j) {
+        const int tv = p.T - 2 + j;
+        for (int i = gtid; i < 64 * 16; i += 128) {
+          int row;
+          const long long off = cache_pos(i, j, row);
+          const long long pix = off - (((long long)b * 2 + j) * frame) * kC;   // (h, w, c) offset within a frame
+          uint4 hv = make_uint4(0u, 0u, 0u, 0u), nv = hv;
+          if (tv >= 0 || front) hv = *ring_unit(slot_of(tv), row, (i & 15) * 8);
+          if (tv >= 0) nv = *reinterpret_cast<const uint4*>(p.n1 + (((long long)b * p.T + tv) * frame) * kC + pix);
+          else if (front) nv = *reinterpret_cast<const uint4*>(p.cn1_in + (((long long)b * 2 + tv + 2) * frame) * kC + pix);
+          *reinterpret_cast<uint4*>(p.ch_out + off) = hv;
+          *reinterpret_cast<uint4*>(p.cn1_out + off) = nv;
         }
       }
     }
@@ -340,7 +402,7 @@ bool tblock_tc_supported(int B, int T, int H, int W, int C, bool planning) {
 cudaError_t launch_tblock_tc(const bf16* n1, const bf16* x, const bf16* w1, const float* bias1, const float* gamma2,
                              const float* beta2, const bf16* w2, const float* bias2, bf16* out, bf16* out2,
                              const float* gamma_out, const float* beta_out, bool out_silu, int B, int T, int H, int W,
-                             cudaStream_t s) {
+                             cudaStream_t s, const TbCache* cache) {
   g_tb_err.clear();
   EncodeTiledFn enc = tb_get_encode();
   if (!enc) { g_tb_err = "cuTensorMapEncodeTiled unavailable"; return cudaErrorNotSupported; }
@@ -355,6 +417,12 @@ cudaError_t launch_tblock_tc(const bf16* n1, const bf16* x, const bf16* w1, cons
   p.ln_out_silu = out_silu ? 1 : 0;
   p.g3 = gamma_out; p.b3 = beta_out;
   p.x = x; p.out = out; p.out2 = out2;
+  if (cache) {
+    if (!cache->n1_out || !cache->h_out || (!cache->n1_in != !cache->h_in)) { g_tb_err = "cache: both outputs, and both or no inputs"; return cudaErrorInvalidValue; }
+    p.n1 = n1;
+    p.cached_in = cache->n1_in ? 1 : 0;
+    p.cn1_in = cache->n1_in; p.ch_in = cache->h_in; p.cn1_out = cache->n1_out; p.ch_out = cache->h_out;
+  }
   const size_t fixed = 1024 + (size_t)kHSlots * kKc * kTile + 6 * kC * 4;
   const size_t budget = 225 * 1024;
   int stages = (int)((budget - fixed) / (2 * kTile + 16));
@@ -370,6 +438,14 @@ cudaError_t launch_tblock_tc(const bf16* n1, const bf16* x, const bf16* w1, cons
     CUresult r = enc(&maps.n1, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, const_cast<bf16*>(n1), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
                      CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) { g_tb_err = "cuTensorMapEncodeTiled(n1) failed: " + std::to_string((int)r); return cudaErrorInvalidValue; }
+    maps.cn1 = maps.n1;
+    if (p.cached_in) {
+      dims[3] = 2;
+      strides[3] = 2ull * H * W * kC * 2;
+      r = enc(&maps.cn1, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, const_cast<bf16*>(p.cn1_in), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+              CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+      if (r != CUDA_SUCCESS) { g_tb_err = "cuTensorMapEncodeTiled(n1 cache) failed: " + std::to_string((int)r); return cudaErrorInvalidValue; }
+    }
   }
   for (int i = 0; i < 2; ++i) {
     cuuint64_t dims[3] = {(cuuint64_t)(3 * kC), (cuuint64_t)kC, 1};
@@ -387,8 +463,10 @@ cudaError_t launch_tblock_tc(const bf16* n1, const bf16* x, const bf16* w1, cons
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= 64) return cudaErrorInvalidDevice;
   if (!attr[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(tblock_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
-    if (e != cudaSuccess) { g_tb_err = "cudaFuncSetAttribute(smem)"; return e; }
+    for (auto k : {tblock_tc_kernel<false>, tblock_tc_kernel<true>}) {
+      cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+      if (e != cudaSuccess) { g_tb_err = "cudaFuncSetAttribute(smem)"; return e; }
+    }
     attr[dev] = true;
     cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, dev);
     if (sms[dev] <= 0) sms[dev] = 132;
@@ -396,9 +474,11 @@ cudaError_t launch_tblock_tc(const bf16* n1, const bf16* x, const bf16* w1, cons
   const unsigned grid = (unsigned)(p.num_strips < sms[dev] ? p.num_strips : sms[dev]);
   const double M = (double)B * T * H * W;
   char det[96] = "";
-  if (prof_enabled()) snprintf(det, sizeof(det), "strip %dx%d T%d ln_out%d", p.BH, p.BW, T, p.ln_out);
+  if (prof_enabled()) snprintf(det, sizeof(det), cache ? "strip %dx%d T%d ln_out%d cache%d" : "strip %dx%d T%d ln_out%d", p.BH, p.BW, T,
+                               p.ln_out, p.cached_in);
   ProfScope _ps("tblock_tc", 2.0 * 2.0 * M * 3 * kC * kC, 2.0 * M * kC * (3.0 + (p.ln_out ? 1.0 : 0.0)), s, det);
-  tblock_tc_kernel<<<grid, kThreadsTb, smem, s>>>(maps, p);
+  if (cache) tblock_tc_kernel<true><<<grid, kThreadsTb, smem, s>>>(maps, p);
+  else tblock_tc_kernel<false><<<grid, kThreadsTb, smem, s>>>(maps, p);
   count_launch();
   return cudaGetLastError();
 }
