@@ -1,9 +1,8 @@
 // wgmma / TMA implicit-GEMM convolution for sm_90a (the tensor-core hot kernel).
 //
 // GEMM view of a causal convolution on channels-last activations [B,T,H,W,C]:
-//   M = output positions, tiled as boxes of BT x BH x BW = 128 positions per CTA tile (two 64-row wgmma tiles, one per
-//       consumer warpgroup),
-//   N = Cout tile (BN in {32, 64, 128, 256}; fp32 accumulators in registers, BN / 2 per consumer thread),
+//   M = output positions, tiled as boxes of BT x BH x BW = 128 positions per CTA tile (two 64-row wgmma tiles),
+//   N = Cout tile (BN in {32, 64, 128, 256}; fp32 accumulators in registers, BN / 2 per consumer thread and 64-row tile),
 //   K = taps x Cin, consumed in steps of 64 channels (one 128-byte swizzle row) per tap.
 // A operand, two formulations:
 //   * halo mode (stride-1 kh x kw > 1 layers): ONE 5-D TMA box per (time tap, 64-channel chunk) loads the CTA tile's input
@@ -15,10 +14,12 @@
 //   later chunks).  No im2col buffer, no padded copy.
 // B operand: TMA box {64, BN} of the pre-packed K-major bf16 weights [Cout][taps*Cin].
 // Both land in shared memory in the canonical K-major SWIZZLE_128B layout and feed wgmma.mma_async m64nBNk16.
-// Warp roles (persistent CTA, one per SM): warps 0-7 = two consumer warpgroups (wgmma on rows [64 g, 64 g + 64) of the tile,
-// then the epilogue straight from the accumulator registers: bias / residual / mix / LayerNorm / regularizer -> global
-// memory), warp 8 = TMA producer, which runs up to `stages` K steps ahead, across tile boundaries too, so that the next
-// tile's operands load while the epilogue runs.
+// Warp roles (persistent CTA, one per SM): warps 0-7 = two consumer warpgroups (wgmma, then the epilogue straight from the
+// accumulator registers: bias / residual / mix / LayerNorm / regularizer -> global memory), warp 8 = TMA producer, which
+// runs up to `stages` K steps ahead, across tile boundaries too, so that the next tile's operands load while the epilogue
+// runs.  The consumers follow one of two schedules (ping_pong()): cooperative, both warpgroups on every tile (rows
+// [64 g, 64 g + 64)), or ping-pong, each warpgroup on every second tile (all 128 rows), their main loops taking turns so
+// that one warpgroup's epilogue runs while the other one's MMAs issue.
 #include <cuda.h>
 
 #include <cstdio>
@@ -93,7 +94,8 @@ struct TcParams {
   int* reg_idx;
   double* reg_kl;
   FsqConst reg_fsq;
-  uint32_t misc_off;         // byte offset of [bias | gamma | beta] x 2 and the regularizer row buffer from the aligned base
+  uint32_t misc_off;         // byte offset of [bias | gamma | beta] x 2 (x 2 warpgroups in ping-pong) and the regularizer
+                             // row buffer from the aligned base
 };
 
 struct TcMaps {
@@ -110,6 +112,15 @@ constexpr int kProducerWarp = kConsumerWarps;
 // most of its share to the consumers (setmaxnreg)
 constexpr int kThreads = (kConsumerWarps + 4) * 32;
 constexpr int kABytes = 128 * 128;      // 128 rows x 64 bf16
+// consumer named barriers (0 is __syncthreads): 1 = bias buffer switch (cooperative), 2 = regularizer rows,
+// kBarTurn + g = warpgroup g may start its next main loop, kBarBias + g = bias buffer switch of warpgroup g (ping-pong)
+constexpr uint32_t kBarTurn = 3, kBarBias = 5;
+
+// Ping-pong consumer schedule: with short K and a heavy epilogue (bf16 N tiles of 64 and 128 channels: 18-20 K steps
+// against LayerNorm and one or two stored tiles) the cooperative schedule leaves the tensor pipe idle for the whole
+// epilogue.  BN = 256 would need 256 accumulators per thread, the split operands a second register set for the K-group
+// sum, and the BN = 32 regularizer heads gather each row across both warpgroups: those stay cooperative.
+__host__ __device__ constexpr bool ping_pong(int BN, bool split) { return !split && (BN == 64 || BN == 128); }
 
 using namespace tcx;
 
@@ -140,6 +151,16 @@ __device__ __forceinline__ bool tap_time(const TcParams& p, const TileCoord& tc,
   }
   return true;
 }
+// time taps of a tile that are loaded (not skipped as causal zero padding)
+__device__ __forceinline__ int tile_taps(const TcParams& p, const TileCoord& tc) {
+  int n = 0;
+  for (int a = 0; a < p.kt; ++a) {
+    int tv;
+    bool from_cache;
+    if (tap_time(p, tc, a, tv, from_cache)) ++n;
+  }
+  return n;
+}
 
 __device__ __forceinline__ float quad_sum(float v) {
   v += __shfl_xor_sync(0xffffffffu, v, 1);
@@ -167,19 +188,23 @@ conv_tc_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
   auto empty_bar = [&](int s) { return bar_base + 8u * (p.stages + s); };
   auto fullA_bar = [&](int s) { return bar_base + 8u * (2 * p.stages + s); };
   auto emptyA_bar = [&](int s) { return bar_base + 8u * (2 * p.stages + p.a_stages + s); };
-  float* sbias = reinterpret_cast<float*>(smem_gen + p.misc_off);   // [2][bias 256 | gamma 256 | beta 256]
-  float* rowbuf = sbias + 2 * 768;                                   // regularizer: [128 rows][33]
+  constexpr bool kPingPong = ping_pong(BN, kSplit);
+  // [2][bias 256 | gamma 256 | beta 256], ping-pong: [2 warpgroups][2][...]
+  float* sbias = reinterpret_cast<float*>(smem_gen + p.misc_off);
+  float* rowbuf = sbias + 2 * 768;                                   // regularizer (BN 32, cooperative): [128 rows][33]
 
   if (threadIdx.x == 0) {
-    // a stage / window is released by every consumer warp once its own wait has seen the MMAs that read it complete
-    // (wgmma.wait_group tracks the executing warp's share of the warpgroup's MMAs)
+    // a stage / window is released by every consumer warp that reads it (both warpgroups, or the one that owns the tile in
+    // ping-pong) once its own wait has seen the MMAs that read it complete (wgmma.wait_group tracks the executing warp's
+    // share of the warpgroup's MMAs)
+    constexpr uint32_t readers = kPingPong ? kConsumerWarps / 2 : kConsumerWarps;
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), kConsumerWarps);
+      mbar_init(empty_bar(s), readers);
     }
     for (int s = 0; s < p.a_stages; ++s) {
       mbar_init(fullA_bar(s), 1);
-      mbar_init(emptyA_bar(s), kConsumerWarps);
+      mbar_init(emptyA_bar(s), readers);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -301,17 +326,19 @@ conv_tc_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
 
   // ===================== consumers: wgmma main loop, then the epilogue from the accumulator registers =====================
   asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
-  constexpr int R = BN / 2;                  // accumulator registers per thread
+  constexpr int R = BN / 2;                  // accumulator registers per thread and 64-row half of a tile
+  constexpr int kHalves = kPingPong ? 2 : 1; // 64-row halves of a tile that one warpgroup computes
   constexpr bool kSum = kSplit && BN <= 128;  // running fp32 sum of the K groups (TcParams::kparts)
   const int g = warp >> 2, wq = warp & 3;
   const bool leader = lane == 0;
   const uint32_t hi_b = desc_hi(1024u);
   const uint32_t hi_a = halo ? desc_hi((uint32_t)p.hP * 128u) : hi_b;
-  // first A row of this warpgroup: 64 rows further into a dense tile, 8 window rows (h) further in halo mode
-  const uint32_t a_row_off = halo ? (uint32_t)(8 * g) * (uint32_t)p.hP * 128u : (uint32_t)g * 64u * 128u;
+  // A rows 64 .. 127 of a tile: 64 rows further into a dense tile, 8 window rows (h) further in halo mode
+  const uint32_t a_half = halo ? 8u * (uint32_t)p.hP * 128u : 64u * 128u;
+  const uint32_t a_row_off = kPingPong ? 0u : (uint32_t)g * a_half;   // first A row of this warpgroup
   const uint32_t a_pl = halo ? p.halo_bytes : a_bytes;        // hi plane -> lo plane (A)
   const uint32_t b_addr0 = halo ? ring_base : smem_base + kPl * a_bytes;
-  float acc[R];
+  float acc[kHalves][R];
   float sum[kSum ? R : 1];
   int stage = 0, sA = 0, sR = 0;
   uint32_t phase = 0, phA = 0;
@@ -327,9 +354,9 @@ conv_tc_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
     pend_stage = -1;
     pend_win = false;
   };
-  // one K step (64 channels): this group's 64 A rows at byte address a_addr (a window row), or of the stage's A tile when
-  // a_from_stage, against the B tile of the current stage; split: hi*hi + lo*hi (+ hi*lo unless `res`: the residual steps
-  // multiply by the identity, which has no lo plane)
+  // one K step (64 channels): this group's 64 A rows (ping-pong: both 64-row halves) at byte address a_addr (a window row),
+  // or of the stage's A tile when a_from_stage, against the B tile of the current stage; split: hi*hi + lo*hi (+ hi*lo
+  // unless `res`: the residual steps multiply by the identity, which has no lo plane)
   auto kstep = [&](bool a_from_stage, uint32_t a_addr, uint32_t scale, bool res, bool last_of_window) {
     mbar_wait(full_bar(stage), phase);
     if (a_from_stage) a_addr = smem_base + stage * stage_bytes + a_row_off;
@@ -339,10 +366,11 @@ conv_tc_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
 #pragma unroll
     for (uint32_t j = 0; j < 4u; ++j) {
       const uint64_t ah = desc(al + 2u * j, hi_a), bh = desc(bl + 2u * j, hi_b);
-      wgmma_k16<BN, kSplit>(acc, ah, bh, j == 0 ? scale : 1u);
+      wgmma_k16<BN, kSplit>(acc[0], ah, bh, j == 0 ? scale : 1u);
+      if constexpr (kPingPong) wgmma_k16<BN, kSplit>(acc[1], desc(al + (a_half >> 4) + 2u * j, hi_a), bh, j == 0 ? scale : 1u);
       if constexpr (kSplit) {
-        wgmma_k16<BN, kSplit>(acc, desc(al + (a_pl >> 4) + 2u * j, hi_a), bh, 1u);
-        if (!res) wgmma_k16<BN, kSplit>(acc, ah, desc(bl + (b_bytes >> 4) + 2u * j, hi_b), 1u);
+        wgmma_k16<BN, kSplit>(acc[0], desc(al + (a_pl >> 4) + 2u * j, hi_a), bh, 1u);
+        if (!res) wgmma_k16<BN, kSplit>(acc[0], ah, desc(bl + (b_bytes >> 4) + 2u * j, hi_b), 1u);
       }
     }
     wgmma_commit();
@@ -353,27 +381,43 @@ conv_tc_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
     if (++stage == nstages) { stage = 0; phase ^= 1u; }
   };
 
-  const int rbase = 64 * g + 16 * wq + (lane >> 2);   // this thread's rows: rbase and rbase + 8
-  const int cq = 2 * (lane & 3);                      // and columns 8j + cq, 8j + cq + 1
+  // this thread's rows: rbase and rbase + 8 (ping-pong: and rbase + 64, rbase + 72), columns 8j + cq, 8j + cq + 1
+  const int rbase = (kPingPong ? 0 : 64 * g) + 16 * wq + (lane >> 2);
+  const int cq = 2 * (lane & 3);
   const bool res_direct = (p.res_mode == 1 && !p.res_mma);
   const bool store_a = (p.ln_mode != 1);
   const float inv_n = 1.0f / (float)BN;
   int last_n0 = -1;
   uint32_t cbuf = 1;                         // bias / gamma / beta buffer in use (toggled whenever n0 changes)
 
-  for (long long tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+  // ping-pong: the CTA's tiles alternate between the warpgroups, `owner` is the one of the current tile
+  int owner = 0;
+  for (long long tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, owner ^= 1) {
     const TileCoord tc = decode_tile(p, tile);
+    if constexpr (kPingPong) {
+      if (owner != g) {
+        // the other warpgroup's tile: step the ring counters past its K steps and halo windows
+        const int taps = tile_taps(p, tc);
+        stage += taps * nsp * num_kc + res_steps;
+        if ((stage / nstages) & 1) phase ^= 1u;
+        stage %= nstages;
+        if (halo) {
+          const int nw = taps * num_kc + res_steps;
+          sA += nw;
+          if ((sA / p.a_stages) & 1) phA ^= 1u;
+          sA %= p.a_stages;
+          sR = (sR + nw) % p.a_stages;
+        }
+        continue;
+      }
+      // the tensor pipe serves one main loop at a time: start once the other warpgroup has issued its previous tile
+      if (tile != blockIdx.x) named_bar_sync(kBarTurn + g, kConsumerWarps * 32);
+    }
     // ---- main loop
     uint32_t G = 0xFFFFFFFFu;                // K steps per group (kparts)
     if constexpr (kSum) {
       if (p.kparts > 1) {
-        uint32_t nk = 0;
-        for (int a = 0; a < p.kt; ++a) {
-          int tv_;
-          bool fc_;
-          if (tap_time(p, tc, a, tv_, fc_)) nk += (uint32_t)(nsp * num_kc);
-        }
-        nk += (uint32_t)res_steps;
+        const uint32_t nk = (uint32_t)(tile_taps(p, tc) * nsp * num_kc + res_steps);
         G = (nk + (uint32_t)p.kparts - 1u) / (uint32_t)p.kparts;
       }
 #pragma unroll
@@ -384,10 +428,10 @@ conv_tc_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
       if constexpr (kSum) {
         if (ks > 0 && ks % G == 0) {
           wgmma_wait<0>();
-          acc_fence(acc);
+          acc_fence(acc[0]);
           release();
 #pragma unroll
-          for (int i = 0; i < R; ++i) sum[i] += acc[i];
+          for (int i = 0; i < R; ++i) sum[i] += acc[0][i];
           accum = 0;
         }
       }
@@ -421,261 +465,282 @@ conv_tc_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
         step(true, 0u, true, false);
       }
     }
+    // the other warpgroup's next tile (the CTA's next one) may start issuing now
+    if constexpr (kPingPong) {
+      if (tile + gridDim.x < p.num_tiles) named_bar_arrive(kBarTurn + (g ^ 1), kConsumerWarps * 32);
+    }
     wgmma_wait<0>();
-    acc_fence(acc);
+#pragma unroll
+    for (int hf = 0; hf < kHalves; ++hf) acc_fence(acc[hf]);
     release();
     if constexpr (kSum) {
 #pragma unroll
-      for (int i = 0; i < R; ++i) acc[i] += sum[i];
+      for (int i = 0; i < R; ++i) acc[0][i] += sum[i];
     }
 
     // ---- epilogue
     if (tc.n0 != last_n0) {
-      // all consumer warps walk the same tile sequence, so this branch is uniform across them; a warp can only be one
-      // barrier behind, which is why two buffers are enough
+      // all warps of the consumers of a tile (both warpgroups, or one in ping-pong) walk the same tile sequence, so this
+      // branch is uniform across them; a warp can only be one barrier behind, which is why two buffers are enough
       last_n0 = tc.n0;
       cbuf ^= 1u;
-      float* b_ = sbias + cbuf * 768;
-      for (int i = threadIdx.x; i < BN; i += kConsumerWarps * 32) {
+      constexpr int nthr = kPingPong ? 128 : kConsumerWarps * 32;
+      float* b_ = sbias + ((kPingPong ? 2 * g : 0) + cbuf) * 768;
+      for (int i = threadIdx.x % nthr; i < BN; i += nthr) {
         b_[i] = (p.bias && tc.n0 + i < p.Co_real) ? p.bias[tc.n0 + i] : 0.f;
         // with SiLU the bf16 normalisation produces y/2 directly (silu(y) = h + h*tanh(h), h = y/2)
         if (p.ln_mode) { const float sc = (p.ln_silu && !kSplit) ? 0.5f : 1.0f; b_[256 + i] = sc * p.ln_gamma[tc.n0 + i]; b_[512 + i] = sc * p.ln_beta[tc.n0 + i]; }
       }
-      asm volatile("bar.sync 1, %0;" ::"n"(kConsumerWarps * 32) : "memory");
+      named_bar_sync(kPingPong ? kBarBias + g : 1u, nthr);
     }
-    const float* bias_s = sbias + cbuf * 768;
+    const float* bias_s = sbias + ((kPingPong ? 2 * g : 0) + cbuf) * 768;
     const float* gamma_s = bias_s + 256;
     const float* beta_s = bias_s + 512;
 
-    // geometry of this thread's two rows
-    bool valid[2];
-    long long ooff[2];
-    const bf16* r0[2];
-    const bf16* r1[2];
-    const bf16* r2[2];
-    auto row_geom = [&](int row, int& t, int& h, int& w) {
-      const int dw = halo ? (row & 7) : row % p.BW;
-      const int dh = halo ? (row >> 3) : (row / p.BW) % p.BH;
-      const int dt = halo ? 0 : row / (p.BW * p.BH);
-      t = tc.t0 + dt; h = tc.h0 + dh; w = tc.w0 + dw;
-      return (t < p.To) && (h < p.Ho) && (w < p.Wo);
-    };
 #pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      int t, h, w;
-      valid[r] = row_geom(rbase + 8 * r, t, h, w);
-      ooff[r] = (long long)tc.b * p.osB + (long long)t * p.osT + (long long)h * p.osH + (long long)w * p.osW;
-      r0[r] = r1[r] = r2[r] = nullptr;
-      if (valid[r] && res_direct) {
-        r0[r] = p.res + (long long)tc.b * p.rsB + (long long)t * p.rsT + (long long)h * p.rsH + (long long)w * p.rsW + tc.n0;
-      } else if (valid[r] && p.res_mode == 3) {
-        // avg-pool of residual frames 2t-1, 2t, 2t+1 (front pad: zero / frame 0 / 1-frame cache)
-        const long long sp = (long long)tc.b * p.rsB + (long long)h * p.rsH + (long long)w * p.rsW + tc.n0;
-        const int ta = 2 * t - 1 + p.res_pool_off, tb = ta + 1, tcn = ta + 2;
-        if (ta >= 0) r0[r] = p.res + sp + (long long)ta * p.rsT;
-        else if (p.res_t_mode == 1) r0[r] = p.res + sp;
-        else if (p.res_t_mode == 2) r0[r] = p.res_cache + (((long long)tc.b * p.Ho + h) * p.Wo + w) * (long long)p.Co * (kSplit ? 2 : 1) + tc.n0;
-        if (tb < p.resT) r1[r] = p.res + sp + (long long)tb * p.rsT;
-        if (tcn < p.resT) r2[r] = p.res + sp + (long long)tcn * p.rsT;
-      }
-    }
-    // residual value of channel pair (c, c + 1) of a row: bf16 pair, or hi + lo fp16 pairs (split)
-    auto res_pair = [&](const bf16* rp, int c, float& x0, float& x1) {
-      const uint32_t hw = *reinterpret_cast<const uint32_t*>(rp + c);
-      if constexpr (kSplit) {
-        const uint32_t lw = *reinterpret_cast<const uint32_t*>(rp + p.o_lo + c);
-        x0 = f16_lo(hw) + f16_lo(lw);
-        x1 = f16_hi(hw) + f16_hi(lw);
-      } else {
-        x0 = bf16_lo(hw);
-        x1 = bf16_hi(hw);
-      }
-    };
-    // v = rb * (acc + bias) + ra * R, in place
-#pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-      const int c = 8 * j + cq;
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        float f = kSplit ? fmaf(acc[4 * j + e], p.acc_scale, bias_s[c + (e & 1)]) : acc[4 * j + e] + bias_s[c + (e & 1)];
-        if (p.rb != 1.0f) f *= p.rb;
-        acc[4 * j + e] = f;
-      }
+    for (int hf = 0; hf < kHalves; ++hf) {
+      float (&acc_h)[R] = acc[hf];
+      // first row of this half; opaque to the compiler, so that the address arithmetic of the second half is not hoisted
+      // over the first half's epilogue, where it would hold registers that the accumulators of both halves need
+      int row0 = rbase + 64 * hf;
+      asm volatile("" : "+r"(row0));
+      // geometry of this thread's two rows of this half
+      bool valid[2];
+      long long ooff[2];
+      auto row_geom = [&](int row, int& t, int& h, int& w) {
+        const int dw = halo ? (row & 7) : row % p.BW;
+        const int dh = halo ? (row >> 3) : (row / p.BW) % p.BH;
+        const int dt = halo ? 0 : row / (p.BW * p.BH);
+        t = tc.t0 + dt; h = tc.h0 + dh; w = tc.w0 + dw;
+        return (t < p.To) && (h < p.Ho) && (w < p.Wo);
+      };
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
-        if (!valid[r]) continue;
-        if (res_direct) {
-          float x0, x1;
-          res_pair(r0[r], c, x0, x1);
-          acc[4 * j + 2 * r] = fmaf(p.ra, x0, acc[4 * j + 2 * r]);
-          acc[4 * j + 2 * r + 1] = fmaf(p.ra, x1, acc[4 * j + 2 * r + 1]);
-        } else if (p.res_mode == 3) {
-          float s0 = 0.f, s1 = 0.f, x0, x1;
-          if (r0[r]) { res_pair(r0[r], c, x0, x1); s0 += x0; s1 += x1; }
-          if (r1[r]) { res_pair(r1[r], c, x0, x1); s0 += x0; s1 += x1; }
-          if (r2[r]) { res_pair(r2[r], c, x0, x1); s0 += x0; s1 += x1; }
-          const float s3 = p.ra * (1.0f / 3.0f);
-          acc[4 * j + 2 * r] = fmaf(s3, s0, acc[4 * j + 2 * r]);
-          acc[4 * j + 2 * r + 1] = fmaf(s3, s1, acc[4 * j + 2 * r + 1]);
+        int t, h, w;
+        valid[r] = row_geom(row0 + 8 * r, t, h, w);
+        ooff[r] = (long long)tc.b * p.osB + (long long)t * p.osT + (long long)h * p.osH + (long long)w * p.osW;
+      }
+      // residual value of channel pair (c, c + 1) of a row: bf16 pair, or hi + lo fp16 pairs (split)
+      auto res_pair = [&](const bf16* rp, int c, float& x0, float& x1) {
+        const uint32_t hw = *reinterpret_cast<const uint32_t*>(rp + c);
+        if constexpr (kSplit) {
+          const uint32_t lw = *reinterpret_cast<const uint32_t*>(rp + p.o_lo + c);
+          x0 = f16_lo(hw) + f16_lo(lw);
+          x1 = f16_hi(hw) + f16_hi(lw);
+        } else {
+          x0 = bf16_lo(hw);
+          x1 = bf16_hi(hw);
+        }
+      };
+      // v = rb * (acc + bias) + ra * R, in place; the residual one row at a time, so that only that row's residual
+      // pointers are live next to the accumulators
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int c = 8 * j + cq;
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          float f = kSplit ? fmaf(acc_h[4 * j + e], p.acc_scale, bias_s[c + (e & 1)]) : acc_h[4 * j + e] + bias_s[c + (e & 1)];
+          if (p.rb != 1.0f) f *= p.rb;
+          acc_h[4 * j + e] = f;
         }
       }
-    }
-
-    if (p.out_f32) {
-      // external fp32 heads / attention scores: direct stores, only the real output channels
-      if (p.out) {
+      if (res_direct || p.res_mode == 3) {
 #pragma unroll
         for (int r = 0; r < 2; ++r) {
-          if (!valid[r]) continue;
-          float* of = reinterpret_cast<float*>(p.out) + ooff[r];
-#pragma unroll
-          for (int j = 0; j < BN / 8; ++j)
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              const int n = tc.n0 + 8 * j + cq + e;
-              if (n < p.Co_real) of[(long long)n * p.osC] = acc[4 * j + 2 * r + e];
-            }
-        }
-      }
-      if (p.reg_mode) {
-        // regularizer on the complete fp32 row of a position (heads with Cout <= 32: BN == 32, n0 == 0): the rows are
-        // gathered in shared memory, thread i < 128 then owns row i with all of its channels
-        if constexpr (BN == 32) {
-#pragma unroll
-          for (int j = 0; j < 4; ++j)
-#pragma unroll
-            for (int e = 0; e < 4; ++e) rowbuf[(rbase + 8 * (e >> 1)) * 33 + 8 * j + cq + (e & 1)] = acc[4 * j + e];
-          asm volatile("bar.sync 2, %0;" ::"n"(kConsumerWarps * 32) : "memory");
-          if (threadIdx.x < 128) {
-            const int row = threadIdx.x;
-            float f[32];
-#pragma unroll
-            for (int c = 0; c < 32; ++c) f[c] = rowbuf[row * 33 + c];
-            int t, h, w;
-            const bool ok = row_geom(row, t, h, w);
-            const long long plane = p.osC;                                  // T*H*W of the [B,C,T,H,W] tensors
-            const long long pos = (long long)t * p.osT + (long long)h * p.osH + (long long)w * p.osW;
-            if (p.reg_mode == 1) {
-              float part = 0.f;
-              // z_channels is a compile-time constant inside each case: f[] stays in registers (no dynamic indexing)
-              auto kl_row = [&](auto ZC) {
-                constexpr int zc = decltype(ZC)::value;
-                const long long zb = (long long)tc.b * zc * plane + pos;
-#pragma unroll
-                for (int c = 0; c < zc; ++c) {
-                  float zv;
-                  part += kl_sample_one(f[c], f[zc + c], p.reg_sample ? p.reg_noise[zb + c * plane] : 0.f, p.reg_sample, zv);
-                  p.reg_z[zb + c * plane] = zv;
-                }
-              };
-              if (ok) {
-                if (p.reg_zc == 4) kl_row(std::integral_constant<int, 4>());
-                else if (p.reg_zc == 8) kl_row(std::integral_constant<int, 8>());
-                else kl_row(std::integral_constant<int, 16>());
-              }
-              double dsum = (double)part;
-#pragma unroll
-              for (int o = 16; o > 0; o >>= 1) dsum += __shfl_xor_sync(0xffffffffu, dsum, o);
-              if (lane == 0) atomicAdd(p.reg_kl, dsum);
-            } else if (ok) {
-              const long long zb = (long long)tc.b * p.reg_zc * plane + pos;
-              float idx = 0.f;
-#pragma unroll
-              for (int c = 0; c < VT_MAX_FSQ; ++c)
-                if (c < p.reg_zc) p.reg_z[zb + c * plane] = fsq_code(p.reg_fsq, c, f[c], idx);
-              if (p.reg_idx) p.reg_idx[(long long)tc.b * plane + pos] = (int)idx;
-            }
+          int t, h, w;
+          if (!row_geom(row0 + 8 * r, t, h, w)) continue;
+          const bf16* r0 = nullptr;
+          const bf16* r1 = nullptr;
+          const bf16* r2 = nullptr;
+          if (res_direct) {
+            r0 = p.res + (long long)tc.b * p.rsB + (long long)t * p.rsT + (long long)h * p.rsH + (long long)w * p.rsW + tc.n0;
+          } else {
+            // avg-pool of residual frames 2t-1, 2t, 2t+1 (front pad: zero / frame 0 / 1-frame cache)
+            const long long sp = (long long)tc.b * p.rsB + (long long)h * p.rsH + (long long)w * p.rsW + tc.n0;
+            const int ta = 2 * t - 1 + p.res_pool_off, tb = ta + 1, tcn = ta + 2;
+            if (ta >= 0) r0 = p.res + sp + (long long)ta * p.rsT;
+            else if (p.res_t_mode == 1) r0 = p.res + sp;
+            else if (p.res_t_mode == 2) r0 = p.res_cache + (((long long)tc.b * p.Ho + h) * p.Wo + w) * (long long)p.Co * (kSplit ? 2 : 1) + tc.n0;
+            if (tb < p.resT) r1 = p.res + sp + (long long)tb * p.rsT;
+            if (tcn < p.resT) r2 = p.res + sp + (long long)tcn * p.rsT;
           }
-          asm volatile("bar.sync 2, %0;" ::"n"(kConsumerWarps * 32) : "memory");
-        }
-      }
-      continue;
-    }
-
-    // 16-bit outputs: bf16 pairs, or hi | lo fp16 planes (split)
-    auto put = [&](void* optr, int r, int c, float y0, float y1) {
-      bf16* o = reinterpret_cast<bf16*>(optr) + ooff[r] + tc.n0 + c;
-      if constexpr (kSplit) {
-        const uint32_t hw = pack_f16x2(y0, y1);
-        *reinterpret_cast<uint32_t*>(o) = hw;
-        *reinterpret_cast<uint32_t*>(o + p.o_lo) = pack_f16x2(y0 - f16_lo(hw), y1 - f16_hi(hw));
-      } else {
-        *reinterpret_cast<uint32_t*>(o) = pack_bf16x2(y0, y1);
-      }
-    };
-    if constexpr (kSplit) {
-      // EXACT_TC: two-pass LayerNorm statistics on the fp32 values, full-precision SiLU
-      if (store_a) {
-#pragma unroll
-        for (int r = 0; r < 2; ++r)
-          if (valid[r])
-#pragma unroll
-            for (int j = 0; j < BN / 8; ++j) put(p.out, r, 8 * j + cq, acc[4 * j + 2 * r], acc[4 * j + 2 * r + 1]);
-      }
-      if (p.ln_mode) {
-        void* nout = p.ln_mode == 1 ? p.out : p.out2;
-#pragma unroll
-        for (int r = 0; r < 2; ++r) {
-          float s = 0.f;
-#pragma unroll
-          for (int j = 0; j < BN / 8; ++j) s += acc[4 * j + 2 * r] + acc[4 * j + 2 * r + 1];
-          const float mean = quad_sum(s) * inv_n;
-          float q = 0.f;
-#pragma unroll
-          for (int j = 0; j < BN / 8; ++j) {
-            const float d0 = acc[4 * j + 2 * r] - mean, d1 = acc[4 * j + 2 * r + 1] - mean;
-            q = fmaf(d0, d0, q);
-            q = fmaf(d1, d1, q);
-          }
-          const float rstd = 1.0f / sqrtf(quad_sum(q) * inv_n + 1e-6f);
-          if (!valid[r]) continue;
 #pragma unroll
           for (int j = 0; j < BN / 8; ++j) {
             const int c = 8 * j + cq;
-            float y0 = (acc[4 * j + 2 * r] - mean) * rstd * gamma_s[c] + beta_s[c];
-            float y1 = (acc[4 * j + 2 * r + 1] - mean) * rstd * gamma_s[c + 1] + beta_s[c + 1];
-            if (p.ln_silu) { y0 = silu_tc(y0); y1 = silu_tc(y1); }
-            put(nout, r, c, y0, y1);
+            if (res_direct) {
+              float x0, x1;
+              res_pair(r0, c, x0, x1);
+              acc_h[4 * j + 2 * r] = fmaf(p.ra, x0, acc_h[4 * j + 2 * r]);
+              acc_h[4 * j + 2 * r + 1] = fmaf(p.ra, x1, acc_h[4 * j + 2 * r + 1]);
+            } else {
+              float s0 = 0.f, s1 = 0.f, x0, x1;
+              if (r0) { res_pair(r0, c, x0, x1); s0 += x0; s1 += x1; }
+              if (r1) { res_pair(r1, c, x0, x1); s0 += x0; s1 += x1; }
+              if (r2) { res_pair(r2, c, x0, x1); s0 += x0; s1 += x1; }
+              const float s3 = p.ra * (1.0f / 3.0f);
+              acc_h[4 * j + 2 * r] = fmaf(s3, s0, acc_h[4 * j + 2 * r]);
+              acc_h[4 * j + 2 * r + 1] = fmaf(s3, s1, acc_h[4 * j + 2 * r + 1]);
+            }
           }
         }
       }
-    } else {
-      // BF16: statistics from the fp32 values, the normalised values from their bf16 rounding (what the unfused
-      // conv -> LayerNorm pair reads back from memory)
+
+      if (p.out_f32) {
+        // external fp32 heads / attention scores: direct stores, only the real output channels
+        if (p.out) {
 #pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        float s = 0.f, q = 0.f;
+          for (int r = 0; r < 2; ++r) {
+            if (!valid[r]) continue;
+            float* of = reinterpret_cast<float*>(p.out) + ooff[r];
 #pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-          const float f0 = acc[4 * j + 2 * r], f1 = acc[4 * j + 2 * r + 1];
-          s += f0 + f1;
-          q = fmaf(f0, f0, q);
-          q = fmaf(f1, f1, q);
-          const uint32_t kp = pack_bf16x2(f0, f1);
-          if (store_a && valid[r]) *reinterpret_cast<uint32_t*>(reinterpret_cast<bf16*>(p.out) + ooff[r] + tc.n0 + 8 * j + cq) = kp;
-          acc[4 * j + 2 * r] = bf16_lo(kp);
-          acc[4 * j + 2 * r + 1] = bf16_hi(kp);
-        }
-        if (!p.ln_mode) continue;
-        // LayerNorm over the Cout values of this row (model_3dcausal.py:62-80, eps 1e-6), optional SiLU (:26-27)
-        const float mean = quad_sum(s) * inv_n;
-        float var = fmaf(-mean, mean, quad_sum(q) * inv_n);
-        var = var < 0.f ? 0.f : var;
-        const float rstd = rsqrtf(var + 1e-6f);
-        const float nmr = -mean * rstd;
-        if (!valid[r]) continue;
-        void* nout = p.ln_mode == 1 ? p.out : p.out2;
+            for (int j = 0; j < BN / 8; ++j)
 #pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-          const int c = 8 * j + cq;
-          float y0 = fmaf(fmaf(acc[4 * j + 2 * r], rstd, nmr), gamma_s[c], beta_s[c]);
-          float y1 = fmaf(fmaf(acc[4 * j + 2 * r + 1], rstd, nmr), gamma_s[c + 1], beta_s[c + 1]);
-          if (p.ln_silu) {
-            // y holds h = LN(v)/2 (gamma, beta were halved): silu = h + h * tanh(h)
-            y0 = fmaf(y0, tanh_approx(y0), y0);
-            y1 = fmaf(y1, tanh_approx(y1), y1);
+              for (int e = 0; e < 2; ++e) {
+                const int n = tc.n0 + 8 * j + cq + e;
+                if (n < p.Co_real) of[(long long)n * p.osC] = acc_h[4 * j + 2 * r + e];
+              }
           }
-          put(nout, r, c, y0, y1);
+        }
+        if (p.reg_mode) {
+          // regularizer on the complete fp32 row of a position (heads with Cout <= 32: BN == 32, n0 == 0): the rows are
+          // gathered in shared memory, thread i < 128 then owns row i with all of its channels
+          if constexpr (BN == 32) {
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+#pragma unroll
+              for (int e = 0; e < 4; ++e) rowbuf[(rbase + 8 * (e >> 1)) * 33 + 8 * j + cq + (e & 1)] = acc_h[4 * j + e];
+            asm volatile("bar.sync 2, %0;" ::"n"(kConsumerWarps * 32) : "memory");
+            if (threadIdx.x < 128) {
+              const int row = threadIdx.x;
+              float f[32];
+#pragma unroll
+              for (int c = 0; c < 32; ++c) f[c] = rowbuf[row * 33 + c];
+              int t, h, w;
+              const bool ok = row_geom(row, t, h, w);
+              const long long plane = p.osC;                                  // T*H*W of the [B,C,T,H,W] tensors
+              const long long pos = (long long)t * p.osT + (long long)h * p.osH + (long long)w * p.osW;
+              if (p.reg_mode == 1) {
+                float part = 0.f;
+                // z_channels is a compile-time constant inside each case: f[] stays in registers (no dynamic indexing)
+                auto kl_row = [&](auto ZC) {
+                  constexpr int zc = decltype(ZC)::value;
+                  const long long zb = (long long)tc.b * zc * plane + pos;
+#pragma unroll
+                  for (int c = 0; c < zc; ++c) {
+                    float zv;
+                    part += kl_sample_one(f[c], f[zc + c], p.reg_sample ? p.reg_noise[zb + c * plane] : 0.f, p.reg_sample, zv);
+                    p.reg_z[zb + c * plane] = zv;
+                  }
+                };
+                if (ok) {
+                  if (p.reg_zc == 4) kl_row(std::integral_constant<int, 4>());
+                  else if (p.reg_zc == 8) kl_row(std::integral_constant<int, 8>());
+                  else kl_row(std::integral_constant<int, 16>());
+                }
+                double dsum = (double)part;
+#pragma unroll
+                for (int o = 16; o > 0; o >>= 1) dsum += __shfl_xor_sync(0xffffffffu, dsum, o);
+                if (lane == 0) atomicAdd(p.reg_kl, dsum);
+              } else if (ok) {
+                const long long zb = (long long)tc.b * p.reg_zc * plane + pos;
+                float idx = 0.f;
+#pragma unroll
+                for (int c = 0; c < VT_MAX_FSQ; ++c)
+                  if (c < p.reg_zc) p.reg_z[zb + c * plane] = fsq_code(p.reg_fsq, c, f[c], idx);
+                if (p.reg_idx) p.reg_idx[(long long)tc.b * plane + pos] = (int)idx;
+              }
+            }
+            asm volatile("bar.sync 2, %0;" ::"n"(kConsumerWarps * 32) : "memory");
+          }
+        }
+        continue;
+      }
+
+      // 16-bit outputs: bf16 pairs, or hi | lo fp16 planes (split)
+      auto put = [&](void* optr, int r, int c, float y0, float y1) {
+        bf16* o = reinterpret_cast<bf16*>(optr) + ooff[r] + tc.n0 + c;
+        if constexpr (kSplit) {
+          const uint32_t hw = pack_f16x2(y0, y1);
+          *reinterpret_cast<uint32_t*>(o) = hw;
+          *reinterpret_cast<uint32_t*>(o + p.o_lo) = pack_f16x2(y0 - f16_lo(hw), y1 - f16_hi(hw));
+        } else {
+          *reinterpret_cast<uint32_t*>(o) = pack_bf16x2(y0, y1);
+        }
+      };
+      if constexpr (kSplit) {
+        // EXACT_TC: two-pass LayerNorm statistics on the fp32 values, full-precision SiLU
+        if (store_a) {
+#pragma unroll
+          for (int r = 0; r < 2; ++r)
+            if (valid[r])
+#pragma unroll
+              for (int j = 0; j < BN / 8; ++j) put(p.out, r, 8 * j + cq, acc_h[4 * j + 2 * r], acc_h[4 * j + 2 * r + 1]);
+        }
+        if (p.ln_mode) {
+          void* nout = p.ln_mode == 1 ? p.out : p.out2;
+#pragma unroll
+          for (int r = 0; r < 2; ++r) {
+            float s = 0.f;
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) s += acc_h[4 * j + 2 * r] + acc_h[4 * j + 2 * r + 1];
+            const float mean = quad_sum(s) * inv_n;
+            float q = 0.f;
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+              const float d0 = acc_h[4 * j + 2 * r] - mean, d1 = acc_h[4 * j + 2 * r + 1] - mean;
+              q = fmaf(d0, d0, q);
+              q = fmaf(d1, d1, q);
+            }
+            const float rstd = 1.0f / sqrtf(quad_sum(q) * inv_n + 1e-6f);
+            if (!valid[r]) continue;
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+              const int c = 8 * j + cq;
+              float y0 = (acc_h[4 * j + 2 * r] - mean) * rstd * gamma_s[c] + beta_s[c];
+              float y1 = (acc_h[4 * j + 2 * r + 1] - mean) * rstd * gamma_s[c + 1] + beta_s[c + 1];
+              if (p.ln_silu) { y0 = silu_tc(y0); y1 = silu_tc(y1); }
+              put(nout, r, c, y0, y1);
+            }
+          }
+        }
+      } else {
+        // BF16: statistics from the fp32 values, the normalised values from their bf16 rounding (what the unfused
+        // conv -> LayerNorm pair reads back from memory)
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          float s = 0.f, q = 0.f;
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            const float f0 = acc_h[4 * j + 2 * r], f1 = acc_h[4 * j + 2 * r + 1];
+            s += f0 + f1;
+            q = fmaf(f0, f0, q);
+            q = fmaf(f1, f1, q);
+            const uint32_t kp = pack_bf16x2(f0, f1);
+            if (store_a && valid[r]) *reinterpret_cast<uint32_t*>(reinterpret_cast<bf16*>(p.out) + ooff[r] + tc.n0 + 8 * j + cq) = kp;
+            acc_h[4 * j + 2 * r] = bf16_lo(kp);
+            acc_h[4 * j + 2 * r + 1] = bf16_hi(kp);
+          }
+          if (!p.ln_mode) continue;
+          // LayerNorm over the Cout values of this row (model_3dcausal.py:62-80, eps 1e-6), optional SiLU (:26-27)
+          const float mean = quad_sum(s) * inv_n;
+          float var = fmaf(-mean, mean, quad_sum(q) * inv_n);
+          var = var < 0.f ? 0.f : var;
+          const float rstd = rsqrtf(var + 1e-6f);
+          const float nmr = -mean * rstd;
+          if (!valid[r]) continue;
+          void* nout = p.ln_mode == 1 ? p.out : p.out2;
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            const int c = 8 * j + cq;
+            float y0 = fmaf(fmaf(acc_h[4 * j + 2 * r], rstd, nmr), gamma_s[c], beta_s[c]);
+            float y1 = fmaf(fmaf(acc_h[4 * j + 2 * r + 1], rstd, nmr), gamma_s[c + 1], beta_s[c + 1]);
+            if (p.ln_silu) {
+              // y holds h = LN(v)/2 (gamma, beta were halved): silu = h + h * tanh(h)
+              y0 = fmaf(y0, tanh_approx(y0), y0);
+              y1 = fmaf(y1, tanh_approx(y1), y1);
+            }
+            put(nout, r, c, y0, y1);
+          }
         }
       }
     }
@@ -855,7 +920,8 @@ cudaError_t launch_conv_tc(const ConvP& p, const bf16* x, const bf16* w_nk, int 
     const size_t stage_bytes = (size_t)cw * ((t.halo ? 0 : (size_t)kABytes) + (size_t)t.BN * 128);
     const size_t budget = 225 * 1024;
     const size_t a_ring = (size_t)t.a_stages * t.halo_bytes * cw;
-    const size_t misc = 2 * 768 * 4 + ((reg && reg->mode) ? 128 * 33 * 4 : 0);
+    // two bias / gamma / beta buffers per consumer group (ping-pong: one group per warpgroup), regularizer rows
+    const size_t misc = (ping_pong(t.BN, split) ? 4 : 2) * 768 * 4 + ((reg && reg->mode) ? 128 * 33 * 4 : 0);
     const size_t fixed = 1024 /*align*/ + misc + 16;
     if (budget < fixed + a_ring + 2 * (stage_bytes + 16)) return 1;
     int stages = (int)((budget - fixed - a_ring) / (stage_bytes + 16));
