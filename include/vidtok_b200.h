@@ -297,10 +297,14 @@ int32_t vt_op_groupnorm(int32_t precision, const void* x, const float* gamma, co
                         int64_t frames, int64_t positions_per_frame, int32_t C, int32_t per_position,
                         int32_t apply_silu, void* workspace, int64_t workspace_bytes, void* stream);
 /* per-frame single-head attention core: q,k,v,o channels-last [frames, H, W, C] (tokens = H*W positions of a frame);
- * scale = C^-0.5.  vt_op_attention_hw runs what the model path runs for a frame of H x W: wgmma GEMMs in BF16 / EXACT_TC
- * when tokens % 64 == 0 and C % 64 == 0, fp32 FMAs otherwise.  vt_op_attention takes a token count and lays the tokens
- * out as an image 8 wide (one row if tokens % 8 != 0): the same arithmetic, not necessarily a model frame's tile plan.
- * workspace: frames*tokens*(8*tokens + 24*C) + 65536 bytes is always enough. */
+ * scale = C^-0.5.  vt_op_attention_hw runs what the model path runs for a frame of H x W, chosen from H, W and C alone:
+ *   BF16 / EXACT_TC, tokens > 1024, C % 64 == 0, C <= 512: one fused kernel (online softmax, no tokens x tokens buffer);
+ *     workspace: the output plus V^T, frames * C * (tokens + tokens rounded up to 8) * (2 bytes BF16, 4 EXACT_TC) + 2048;
+ *   BF16 / EXACT_TC, tokens <= 1024, tokens % 64 == 0 and C % 64 == 0: wgmma GEMMs through a materialised score matrix;
+ *   otherwise (and in FMA32): fp32 FMAs through a materialised score matrix.
+ * vt_op_attention takes a token count and lays the tokens out as an image 8 wide (one row if tokens % 8 != 0): the same
+ * arithmetic, not necessarily a model frame's tile plan.  workspace: frames*tokens*(8*tokens + 24*C) + 65536 bytes is
+ * always enough. */
 int32_t vt_op_attention(int32_t precision, const void* q, const void* k, const void* v, void* o, int32_t frames,
                         int32_t tokens, int32_t C, void* workspace, int64_t workspace_bytes, void* stream);
 int32_t vt_op_attention_hw(int32_t precision, const void* q, const void* k, const void* v, void* o, int32_t frames,

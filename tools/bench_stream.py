@@ -4,10 +4,11 @@ peak workspace of each configuration (vt_chunk_workspace_bytes / vt_workspace_by
   256x256 B=8 bf16    pushes of 4 frames and of 16 frames (after the 1-frame first push), and the whole clip
   720x1280 B=1 bf16   pushes of 4 frames, and the whole clip
   1080x1920 B=1 exact pushes of 4 frames only (the whole clip needs more workspace than an 80 GB card has)
+  1080x1920 B=1 bf16  pushes of 4 frames only
 
 Frames/s counts input frames of the steady pushes (the first 1-frame push is timed apart).  Prints one JSON line per
 configuration and the card, its power limit and SM clocks.
-usage: python tools/bench_stream.py [--clips 2] [--out FILE]"""
+usage: python tools/bench_stream.py [--clips 2] [--lib PATH] [--out FILE]"""
 import argparse
 import json
 import os
@@ -81,14 +82,17 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--clips", type=int, default=2)
     ap.add_argument("--out", default=None)
+    ap.add_argument("--lib", default=None, help="library to measure (default: the in-tree build)")
     args = ap.parse_args()
+    if args.lib:
+        N.LIB_PATH = os.path.abspath(args.lib)
     if not torch.cuda.is_available():
         raise SystemExit("bench_stream: no CUDA device; these numbers need an H100")
     model = kl488()
     rows = []
     with torch.no_grad():
         for (B, H, W, prec, pushes, whole) in ((8, 256, 256, "bf16", (4, 16), True), (1, 720, 1280, "bf16", (4,), True),
-                                               (1, 1080, 1920, "exact", (4,), False)):
+                                               (1, 1080, 1920, "exact", (4,), False), (1, 1080, 1920, "bf16", (4,), False)):
             model.precision = prec
             T = 17
             if whole:

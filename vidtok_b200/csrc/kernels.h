@@ -176,6 +176,15 @@ cudaError_t launch_tblock_tc(const bf16* n1, const bf16* x, const bf16* w1, cons
                              cudaStream_t s, const TbCache* cache = nullptr);
 const char* tblock_tc_last_error();
 
+// attn_tc.cu: fused per-frame attention O = softmax(Q K^T / sqrt(C)) V on wgmma with an online softmax (no tokens x tokens
+// buffer).  q, k, v, o channels-last [frames, H*W, C] in bf16 or hi|lo split rows; C % 64 == 0, C <= 512, any token count.
+// ws: attn_tc_workspace bytes (V^T, the size of v).
+bool attn_tc_supported(long long frames, long long tokens, int C, bool split, bool planning = false);
+size_t attn_tc_workspace(long long frames, long long tokens, int C, bool split);
+cudaError_t launch_attn_tc(const bf16* q, const bf16* k, const bf16* v, bf16* o, int frames, int H, int W, int C, bool split,
+                           void* ws, cudaStream_t s);
+const char* attn_tc_last_error();
+
 // conv_stem.cu (thread-built im2col A tile + wgmma for the Cin=3 stem)
 bool conv_stem_supported(const ConvP& p);
 cudaError_t launch_conv_stem(const ConvP& p, const float* x, const bf16* wpk, bf16* out, cudaStream_t s);

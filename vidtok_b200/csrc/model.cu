@@ -824,10 +824,26 @@ struct Exec {
     ar.release(S);
     return true;
   }
+  // Frames above 32 x 32 positions: the fused kernel (attn_tc.cu), online softmax, no tokens x tokens buffer; its only
+  // workspace is V^T, the size of v.  The choice depends on the frame (H, W, C) only, never on the frame count.  Frames of
+  // up to 1024 tokens keep the two-GEMM path above, whose launch plans the production-plan table pins.
+  bool attention_fused(const Act& q, const Act& k, const Act& v, Act& o) {
+    const long long frames = (long long)q.B * q.T, tokens = (long long)q.H * q.W;
+    if (!tcm || tokens <= 1024 || q.C % 64 != 0 || q.C > 512) return false;
+    if (!attn_tc_supported(frames, tokens, q.C, split, true)) return false;
+    o = new_act(q.B, q.T, q.H, q.W, q.C);
+    void* vt = alloc(attn_tc_workspace(frames, tokens, q.C, split));
+    if (ok() && !dry)
+      cuda(launch_attn_tc((const bf16*)q.p, (const bf16*)k.p, (const bf16*)v.p, (bf16*)o.p, (int)frames, q.H, q.W, q.C, split, vt, s),
+           attn_tc_last_error());
+    ar.release(vt);
+    return true;
+  }
   Act attention_core(const Act& q, const Act& k, const Act& v) {
     const int frames = q.B * q.T, tokens = q.H * q.W, C = q.C;
     {
       Act o_tc;
+      if (attention_fused(q, k, v, o_tc)) return o_tc;
       if (attention_tc(q, k, v, o_tc)) return o_tc;
     }
     Act o = new_act(q.B, q.T, q.H, q.W, C);
