@@ -13,6 +13,8 @@
 //          layout (the layout a TMA load would have produced), then fence.proxy.async: the ring is the next A operand
 //   G2(t): acc = sum_a W2[a] . H[t-2+a]            A = the shared-memory ring, B (W2 slice) by TMA
 //   E2(t): out[t] = acc + b2 + x[t]; optionally out2[t] = act(LN_next(out[t])) for the next stage
+//          x[t] comes by TMA into the ring slot of frame t-2 (free once G2(t)'s first tap is done), E2 overwrites it with
+//          out[t], and one bulk tensor store per warpgroup writes it back; out2 is stored per thread
 // Causal zero padding = skipped taps.
 //
 // Cached variant (kCache, a video streamed chunk by chunk): the taps in front of frame 0 read the previous chunk's last two
@@ -73,6 +75,7 @@ struct TbParams {
 };
 struct TbMaps {
   CUtensorMap n1, w1, w2, cn1;
+  CUtensorMap x, out;   // 64-row boxes: one consumer warpgroup's half of a strip
 };
 
 __device__ __forceinline__ float quad_sum(float v) {
@@ -82,7 +85,7 @@ __device__ __forceinline__ float quad_sum(float v) {
 }
 
 // smem layout from the 1024-aligned base:
-//   [H ring: 3 slots x kKc tiles][stage ring: stages x (A tile | B tile)][barriers][constants]
+//   [H ring: 3 slots x kKc tiles][stage ring: stages x (A tile | B tile)][barriers: full, empty, x][constants]
 template <bool kCache>
 __global__ void __launch_bounds__(kThreadsTb, 1) tblock_tc_kernel(const __grid_constant__ TbMaps maps, const TbParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -95,7 +98,8 @@ __global__ void __launch_bounds__(kThreadsTb, 1) tblock_tc_kernel(const __grid_c
   const uint32_t bar_base = ring_base + (uint32_t)p.stages * stage_bytes;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (p.stages + s); };
-  float* cst = reinterpret_cast<float*>(smem_gen + (bar_base - smem_base) + 16u * p.stages);   // bias1 | g2 | b2 | bias2 | g3 | b3
+  auto x_bar = [&](int g) { return bar_base + 16u * p.stages + 8u * g; };   // x[t] of consumer warpgroup g has landed
+  float* cst = reinterpret_cast<float*>(smem_gen + (bar_base - smem_base) + 16u * p.stages + 16u);   // bias1 | g2 | b2 | bias2 | g3 | b3
 
   for (int i = threadIdx.x; i < kC; i += kThreadsTb) {
     cst[i] = p.bias1 ? p.bias1[i] : 0.f;
@@ -110,6 +114,7 @@ __global__ void __launch_bounds__(kThreadsTb, 1) tblock_tc_kernel(const __grid_c
   if (threadIdx.x == 0) {
     // a stage is released by every consumer warp once its own wait has seen the MMAs that read it complete
     for (int s = 0; s < p.stages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), kConsumerWarps); }
+    for (int g = 0; g < 2; ++g) mbar_init(x_bar(g), 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -167,7 +172,7 @@ __global__ void __launch_bounds__(kThreadsTb, 1) tblock_tc_kernel(const __grid_c
   const uint32_t hi = desc_hi(1024u);
   float acc[kC / 2];
   int stage = 0, pend_stage = -1;
-  uint32_t phase = 0;
+  uint32_t phase = 0, xphase = 0;
   auto release = [&]() {
     if (lane == 0 && pend_stage >= 0) mbar_arrive(empty_bar(pend_stage));
     pend_stage = -1;
@@ -229,6 +234,7 @@ __global__ void __launch_bounds__(kThreadsTb, 1) tblock_tc_kernel(const __grid_c
     };
     if (front) {
       // ring slots of frames -2, -1 := the LN2(h) cache
+      if (gtid == 0) bulk_wait_read<0>();
       wg_sync();   // every warp of the group is done with the previous strip's ring
       for (int j = 0; j < 2; ++j)
         for (int i = gtid; i < 64 * 16; i += 128) {
@@ -239,6 +245,15 @@ __global__ void __launch_bounds__(kThreadsTb, 1) tblock_tc_kernel(const __grid_c
       fence_async_smem();
       wg_sync();
     }
+    // E2(t) finds x[t] (this warpgroup's 64 rows, brought by TMA) in the ring slot of frame t-2, which G2(t) no longer
+    // reads once its first tap is done, and leaves out[t] in its place for one bulk tensor store
+    const int box_w = tw * p.BW + (64 * g) % p.BW, box_h = th * p.BH + (64 * g) / p.BW;
+    auto x_load = [&](int t) {
+      if (gtid != 0) return;
+      const uint32_t dst = slot_of(t - 2) + (uint32_t)g * 64u * 128u;
+      mbar_expect_tx(x_bar(g), (uint32_t)kKc * 64u * 128u);
+      for (int kc = 0; kc < kKc; ++kc) tma_load_5d(dst + (uint32_t)kc * kTile, &maps.x, x_bar(g), kc * 64, box_w, box_h, t, b);
+    };
     for (int t = 0; t < p.T; ++t) {
       // ---- G1(t)
       uint32_t scale = 0;
@@ -248,6 +263,7 @@ __global__ void __launch_bounds__(kThreadsTb, 1) tblock_tc_kernel(const __grid_c
       }
       finish();
       // ---- E1(t): H[t mod 3] = bf16(silu(LN2(acc + b1))); statistics from fp32, normalisation of the bf16-rounded h
+      if (gtid == 0) bulk_wait_read<0>();   // the slot written here held out[t-1] for a bulk store
       wg_sync();   // every warp of the group is past G2(t-1), which read the slot written here
       const uint32_t slot = h_base + (uint32_t)(t % kHSlots) * kKc * kTile;
 #pragma unroll
@@ -286,31 +302,44 @@ __global__ void __launch_bounds__(kThreadsTb, 1) tblock_tc_kernel(const __grid_c
       fence_async_smem();
       wg_sync();
       // ---- G2(t): A = this group's rows of the H ring
+      const bool tap0 = t >= 2 || front;   // G2(t) reads the slot of frame t-2
+      if (!tap0) x_load(t);
       scale = 0;
+      int s2 = 0;
       for (int a = 0; a < 3; ++a) {
         const int tv = t - 2 + a;
         if (tv < 0 && !front) continue;
         const uint32_t hs = (kCache ? slot_of(tv) : h_base + (uint32_t)(tv % kHSlots) * kKc * kTile) + (uint32_t)g * 64u * 128u;
-        for (int kc = 0; kc < kKc; ++kc) { kstep(false, hs + (uint32_t)kc * kTile, scale); scale = 1; }
+        for (int kc = 0; kc < kKc; ++kc) {
+          kstep(false, hs + (uint32_t)kc * kTile, scale);
+          scale = 1;
+          // the wait of step kKc saw the first tap's steps complete in this warp; the group barrier, in every warp
+          if (++s2 == kKc + 1 && tap0) { wg_sync(); x_load(t); }
+        }
       }
       finish();
       // ---- E2(t): out = acc + b2 + x; out2 = act(LN_next(out)) from the bf16-rounded out
+      mbar_wait(x_bar(g), xphase);
+      xphase ^= 1u;
+      const uint32_t xslot = slot_of(t - 2);
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
         const long long off = (pos0[r] + (long long)t * frame) * kC;
-        const bf16* xr = p.x + off;
-        bf16* orow = p.out + off;
+        const int row = rbase + 8 * r;
+        uint8_t* xrow = smem_gen + (xslot - smem_base) + row * 128;
         float s = 0.f, q = 0.f;
 #pragma unroll
         for (int j = 0; j < kC / 8; ++j) {
           const int c = 8 * j + cq;
-          const uint32_t xw = *reinterpret_cast<const uint32_t*>(xr + c);
+          const int cc = c & 63, u = cc >> 3;
+          uint32_t* xo = reinterpret_cast<uint32_t*>(xrow + (c >> 6) * kTile + ((u ^ (row & 7)) << 4) + (cc & 7) * 2);
+          const uint32_t xw = *xo;
           const float f0 = acc[4 * j + 2 * r] + bias2[c] + bf16_lo(xw), f1 = acc[4 * j + 2 * r + 1] + bias2[c + 1] + bf16_hi(xw);
           s += f0 + f1;
           q = fmaf(f0, f0, q);
           q = fmaf(f1, f1, q);
           const uint32_t kp = pack_bf16x2(f0, f1);
-          *reinterpret_cast<uint32_t*>(orow + c) = kp;
+          *xo = kp;
           acc[4 * j + 2 * r] = bf16_lo(kp);
           acc[4 * j + 2 * r + 1] = bf16_hi(kp);
         }
@@ -333,6 +362,13 @@ __global__ void __launch_bounds__(kThreadsTb, 1) tblock_tc_kernel(const __grid_c
           *reinterpret_cast<uint32_t*>(o2 + c) = pack_bf16x2(y0, y1);
         }
       }
+      fence_async_smem();
+      wg_sync();
+      if (gtid == 0) {
+        for (int kc = 0; kc < kKc; ++kc)
+          tma_store_5d(&maps.out, xslot + (uint32_t)g * 64u * 128u + (uint32_t)kc * kTile, kc * 64, box_w, box_h, t, b);
+        bulk_commit();
+      }
     }
     if (kCache) {
       // next caches: frames T-2, T-1 of [cache | chunk] (zero padding in front of the first chunk).  The LN2(h) frames are
@@ -353,6 +389,7 @@ __global__ void __launch_bounds__(kThreadsTb, 1) tblock_tc_kernel(const __grid_c
       }
     }
   }
+  if (gtid == 0) bulk_wait<0>();   // the last bulk store has read shared memory before the CTA exits
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -423,7 +460,7 @@ cudaError_t launch_tblock_tc(const bf16* n1, const bf16* x, const bf16* w1, cons
     p.cached_in = cache->n1_in ? 1 : 0;
     p.cn1_in = cache->n1_in; p.ch_in = cache->h_in; p.cn1_out = cache->n1_out; p.ch_out = cache->h_out;
   }
-  const size_t fixed = 1024 + (size_t)kHSlots * kKc * kTile + 6 * kC * 4;
+  const size_t fixed = 1024 + (size_t)kHSlots * kKc * kTile + 16 + 6 * kC * 4;
   const size_t budget = 225 * 1024;
   int stages = (int)((budget - fixed) / (2 * kTile + 16));
   if (stages > 4) stages = 4;
@@ -439,6 +476,14 @@ cudaError_t launch_tblock_tc(const bf16* n1, const bf16* x, const bf16* w1, cons
                      CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) { g_tb_err = "cuTensorMapEncodeTiled(n1) failed: " + std::to_string((int)r); return cudaErrorInvalidValue; }
     maps.cn1 = maps.n1;
+    // x and out: one consumer warpgroup's 64 rows of a strip, the rows (h, w) in strip order
+    const int bw = p.BW < 64 ? p.BW : 64;
+    cuuint32_t box64[5] = {64, (cuuint32_t)bw, (cuuint32_t)(64 / bw), 1, 1};
+    for (int i = 0; i < 2; ++i) {
+      r = enc(i ? &maps.out : &maps.x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, i ? (void*)out : const_cast<bf16*>(x), dims, strides, box64, es,
+              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+      if (r != CUDA_SUCCESS) { g_tb_err = "cuTensorMapEncodeTiled(x / out) failed: " + std::to_string((int)r); return cudaErrorInvalidValue; }
+    }
     if (p.cached_in) {
       dims[3] = 2;
       strides[3] = 2ull * H * W * kC * 2;
