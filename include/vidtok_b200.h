@@ -103,9 +103,6 @@ void vt_profile_start(void);
 void vt_profile_start_detailed(void); /* keys additionally carry the layer geometry */
 int32_t vt_profile_stop(char* json, int32_t cap);
 
-/* diagnostics: co-resident 2-CTA clusters of the conv kernel for a given dynamic shared-memory size */
-int32_t vt_debug_cluster_query(int32_t smem_bytes, char* msg, int32_t cap);
-
 /* ---- model lifetime (replaces AutoencodingEngine.__init__, autoencoder.py:103-144) ---- */
 int32_t vt_model_create(const vt_model_desc* desc, int32_t device, vt_model** out);
 void vt_model_destroy(vt_model* m);

@@ -43,7 +43,6 @@ _SIGS = {
     "vt_last_error": (C.c_char_p, []),
     "vt_abi_version": (_I32, []),
     "vt_launch_count": (_I64, [_I32]),
-    "vt_debug_cluster_query": (_I32, [_I32, C.c_char_p, _I32]),
     "vt_profile_start": (None, []),
     "vt_profile_start_detailed": (None, []),
     "vt_profile_stop": (_I32, [C.c_char_p, _I32]),

@@ -32,6 +32,7 @@
 
 #include "common.cuh"
 #include "kernels.h"
+#include "tc_host.h"
 #include "tc_ptx.cuh"
 
 namespace vt {
@@ -369,22 +370,6 @@ __global__ void __launch_bounds__(kThreadsAt, 1) attn_tc_kernel(const __grid_con
     }
   }
 
-  typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-  EncodeTiledFn at_get_encode() {
-    static EncodeTiledFn fn = nullptr;
-    static bool tried = false;
-    if (!tried) {
-      tried = true;
-      void* f = nullptr;
-      cudaDriverEntryPointQueryResult q;
-      if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-        fn = (EncodeTiledFn)f;
-    }
-    return fn;
-  }
-
   constexpr size_t kSmemBudget = 227 * 1024;
   size_t at_fixed_smem(int nc, bool split) {
     const int cw = split ? 2 : 1;
@@ -415,7 +400,7 @@ __global__ void __launch_bounds__(kThreadsAt, 1) attn_tc_kernel(const __grid_con
     if (tokens > (1LL << 30)) { g_at_err = "too many tokens per frame"; return false; }
     if (frames * ((tokens + kBM - 1) / kBM) >= (1LL << 31)) { g_at_err = "grid too large"; return false; }
     if (at_stages(C / 64, split) < 2) { g_at_err = "shared memory"; return false; }
-    if (!planning && !at_get_encode()) { g_at_err = "cuTensorMapEncodeTiled unavailable"; return false; }
+    if (!planning && !tmap_encoder()) { g_at_err = "cuTensorMapEncodeTiled unavailable"; return false; }
     return true;
   }
 
@@ -429,7 +414,6 @@ __global__ void __launch_bounds__(kThreadsAt, 1) attn_tc_kernel(const __grid_con
     g_at_err.clear();
     const long long tokens = (long long)H * W;
     if (!attn_tc_supported(frames, tokens, C, split, false)) return cudaErrorInvalidValue;
-    EncodeTiledFn enc = at_get_encode();
     const int cw = split ? 2 : 1;
     const long long tpad = (tokens + 7) / 8 * 8;
     const int cols = cw * C;
@@ -445,25 +429,19 @@ __global__ void __launch_bounds__(kThreadsAt, 1) attn_tc_kernel(const __grid_con
       if (e != cudaSuccess) { g_at_err = "V transpose launch"; return e; }
     }
     AtMaps maps;
-    cuuint32_t es[3] = {1, 1, 1};
     for (int i = 0; i < 2; ++i) {
       // q / k: [frames][tokens][cw * C], boxes of 64 channels x 64 (q) / 128 (k) tokens
       cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)tokens, (cuuint64_t)frames};
       cuuint64_t strides[2] = {(cuuint64_t)cols * 2, (cuuint64_t)tokens * cols * 2};
       cuuint32_t box[3] = {64, (cuuint32_t)(i ? kBN : kBM), 1};
-      CUresult r = enc(i ? &maps.k : &maps.q, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<bf16*>(i ? k : q), dims, strides, box, es,
-                       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      if (r != CUDA_SUCCESS) { g_at_err = "cuTensorMapEncodeTiled(q/k) failed: " + std::to_string((int)r); return cudaErrorInvalidValue; }
+      if (!encode_tmap_16b(i ? &maps.k : &maps.q, 3, i ? k : q, dims, strides, box, "q/k", g_at_err)) return cudaErrorInvalidValue;
     }
     {
       // V^T: [frames][cw * C][tpad], boxes of 64 tokens x 64 channels
       cuuint64_t dims[3] = {(cuuint64_t)tokens, (cuuint64_t)cols, (cuuint64_t)frames};
       cuuint64_t strides[2] = {(cuuint64_t)tpad * 2, (cuuint64_t)tpad * cols * 2};
       cuuint32_t box[3] = {64, 64, 1};
-      CUresult r = enc(&maps.vt, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, vt, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                       CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      if (r != CUDA_SUCCESS) { g_at_err = "cuTensorMapEncodeTiled(v^T) failed: " + std::to_string((int)r); return cudaErrorInvalidValue; }
+      if (!encode_tmap_16b(&maps.vt, 3, vt, dims, strides, box, "v^T", g_at_err)) return cudaErrorInvalidValue;
     }
     AtParams p;
     memset(&p, 0, sizeof(p));
@@ -476,17 +454,15 @@ __global__ void __launch_bounds__(kThreadsAt, 1) attn_tc_kernel(const __grid_con
     p.sl2 = 1.4426950408889634f / sqrtf((float)C);
     p.o = o;
     const size_t smem = at_fixed_smem(p.nc, split) + (size_t)p.stages * ((size_t)cw * kUnit + 16);
-    static bool attr[64] = {false};
     int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev < 0 || dev >= 64) return cudaErrorInvalidDevice;
-    if (!attr[dev]) {
-      for (auto kf : {attn_tc_kernel<false, 1>, attn_tc_kernel<false, 2>, attn_tc_kernel<true, 1>, attn_tc_kernel<true, 2>}) {
-        cudaError_t e = cudaFuncSetAttribute(kf, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget);
-        if (e != cudaSuccess) { g_at_err = "cudaFuncSetAttribute(smem)"; return e; }
-      }
-      attr[dev] = true;
-  }
+    const cudaError_t dev_err = current_device(dev);
+    if (dev_err != cudaSuccess) { g_at_err = "no current device, or its index is out of range"; return dev_err; }
+    {
+      static SmemLimitOnce smem_limit;
+      const cudaError_t e = smem_limit.ensure(dev, (int)kSmemBudget, attn_tc_kernel<false, 1>, attn_tc_kernel<false, 2>,
+                                              attn_tc_kernel<true, 1>, attn_tc_kernel<true, 2>);
+      if (e != cudaSuccess) { g_at_err = "cudaFuncSetAttribute(smem)"; return e; }
+    }
   const unsigned grid = (unsigned)((long long)frames * p.q_tiles);
   const double tk = (double)tokens;
   char det[96] = "";

@@ -11,6 +11,7 @@
 
 #include "common.cuh"
 #include "kernels.h"
+#include "tc_host.h"
 #include "tc_ptx.cuh"
 
 namespace vt {
@@ -299,10 +300,9 @@ cudaError_t launch_conv_stem(const ConvP& p, const float* x, const bf16* wpk, bf
   const size_t pl = p.split ? 2 : 1;
   const size_t smem = 1024 + pl * kATile + pl * (size_t)p.Co * 256 + (((size_t)p.Ci * 3 * PH * PW * 4 + 15) & ~(size_t)15) + 256 * 4 + 128 * 4;
   int dev = 0;
-  cudaGetDevice(&dev);
-  int num_sms = 0;
-  cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
-  if (num_sms <= 0) num_sms = 132;
+  const cudaError_t dev_err = current_device(dev);
+  if (dev_err != cudaSuccess) return dev_err;
+  const int num_sms = device_sms(dev);
   const double M = (double)t.num_tiles * 128;
   char det[96] = "";
   if (prof_enabled()) snprintf(det, sizeof(det), "k333 %d->%d @%dx%dx%d", p.Ci, p.Co, p.To, p.Hi, p.Wi);

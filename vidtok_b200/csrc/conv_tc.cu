@@ -30,6 +30,7 @@
 
 #include "common.cuh"
 #include "kernels.h"
+#include "tc_host.h"
 #include "tc_ptx.cuh"
 
 namespace vt {
@@ -757,39 +758,6 @@ __global__ void fill_identity_kernel(bf16* e, int f16, float value) {
 // ---------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn get_encode() {
-  static EncodeTiledFn fn = nullptr;
-  static bool tried = false;
-  if (!tried) {
-    tried = true;
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-        q == cudaDriverEntryPointSuccess)
-      fn = (EncodeTiledFn)p;
-  }
-  return fn;
-}
-
-// Per-device state (ADVICE r1): cudaFuncSetAttribute applies to the current device only, and the SM count may differ.
-constexpr int kMaxDev = 64;
-int device_num_sms() {
-  static int sms[kMaxDev] = {0};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev < 0 || dev >= kMaxDev) return 132;
-  if (sms[dev] == 0) {
-    int n = 0;
-    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    sms[dev] = n > 0 ? n : 132;
-  }
-  return sms[dev];
-}
-cudaError_t ensure_func_attrs();
-
 bool choose_tile(const ConvP& p, int rows, int& BW, int& BH, int& BT, long long* padded_out = nullptr) {
   const bool allow_bt = (p.st == 1) && (p.t_mode == 0);
   long long best = -1;
@@ -817,38 +785,7 @@ int choose_bn(int Co) {
 
 }  // namespace
 
-namespace {
-template <int BN, bool kSplit>
-cudaError_t set_smem_attr() {
-  return cudaFuncSetAttribute(conv_tc_kernel<BN, kSplit>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-}
-cudaError_t ensure_func_attrs() {
-  static bool done[kMaxDev] = {false};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev < 0 || dev >= kMaxDev) return cudaErrorInvalidDevice;
-  if (done[dev]) return cudaSuccess;
-  cudaError_t e = cudaSuccess;
-  for (cudaError_t x : {set_smem_attr<32, false>(), set_smem_attr<64, false>(), set_smem_attr<128, false>(), set_smem_attr<256, false>(),
-                        set_smem_attr<32, true>(), set_smem_attr<64, true>(), set_smem_attr<128, true>(), set_smem_attr<256, true>()})
-    if (x != cudaSuccess) e = x;
-  if (e == cudaSuccess) done[dev] = true;
-  return e;
-}
-}  // namespace
-
 const char* conv_tc_last_error() { return g_tc_err.c_str(); }
-
-int conv_tc_cluster_query(int smem, char* msg, int cap) {
-  cudaError_t e = set_smem_attr<128, false>();
-  int n = -1;
-  cudaError_t e2 = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, conv_tc_kernel<128, false>, kThreads, smem);
-  cudaFuncAttributes fa;
-  cudaFuncGetAttributes(&fa, conv_tc_kernel<128, false>);
-  snprintf(msg, cap, "setattr=%s occ=%s ctas_per_sm=%d regs=%d static_smem=%zu maxdyn=%d", cudaGetErrorString(e), cudaGetErrorString(e2), n,
-           fa.numRegs, fa.sharedSizeBytes, fa.maxDynamicSharedSizeBytes);
-  return n;
-}
 
 bool conv_tc_can_fuse_ln(const ConvP& p) {
   return p.Co <= 256 && choose_bn(p.Co) == p.Co && (!p.split || split_ln_fusion_keeps_kparts(p.Co, p.kt * p.kh * p.kw * (p.Ci / 64)));
@@ -877,15 +814,14 @@ bool conv_tc_supported(const ConvP& p, DType tout, bool planning) {
   if (p.t_mode == 2 && p.sh != 1) return no("cache mode with spatial stride");
   if (!planning && p.t_mode == 2 && (!p.cache || p.cacheT <= 0)) return no("cache mode without cache");
   if (p.Wi > 65535 || p.Hi > 65535) return no("extent");
-  if (!planning && !get_encode()) return no("cuTensorMapEncodeTiled unavailable");
+  if (!planning && !tmap_encoder()) return no("cuTensorMapEncodeTiled unavailable");
   return true;
 }
 
 // w_nk: [Co_pad][Kpad] bf16 with Co_pad = roundup(Co, 32) (rows >= Co are zero).
 cudaError_t launch_conv_tc(const ConvP& p, const bf16* x, const bf16* w_nk, int Kpad, void* out, DType tout, cudaStream_t s,
                            int w_batches, long long w_batch_stride, const TcLnFusion* ln, const TcRegFusion* reg) {
-  EncodeTiledFn enc = get_encode();
-  if (!enc) { g_tc_err = "cuTensorMapEncodeTiled unavailable"; return cudaErrorNotSupported; }
+  if (!tmap_encoder()) { g_tc_err = "cuTensorMapEncodeTiled unavailable"; return cudaErrorNotSupported; }
   const bool split = p.split != 0;
   const int cw = split ? 2 : 1;              // bf16 elements per logical channel (hi | lo planes)
   const bool out_bf16 = tout != DT_F32;      // DT_BF16, or DT_SPLIT (two 16-bit planes)
@@ -893,9 +829,9 @@ cudaError_t launch_conv_tc(const ConvP& p, const bf16* x, const bf16* w_nk, int 
   TcParams t;
   memset(&t, 0, sizeof(t));
   const int Co_pad = (p.Co + 31) / 32 * 32;
-  const int num_sms = device_num_sms();
-  static int halo_env = -1;   // VT_TC_HALO=0 switches the halo windows off (experiment knob)
-  if (halo_env < 0) { const char* e = getenv("VT_TC_HALO"); halo_env = e ? atoi(e) : 1; }
+  int dev = 0;
+  const cudaError_t dev_err = current_device(dev);
+  if (dev_err != cudaSuccess) { g_tc_err = "no current device, or its index is out of range"; return dev_err; }
   size_t smem = 0;
   // Tile geometry + shared-memory plan.  Split operands double every operand tile: when the halo windows leave fewer
   // than 2 pipeline stages, fall back to one A box per tap.
@@ -907,7 +843,7 @@ cudaError_t launch_conv_tc(const ConvP& p, const bf16* x, const bf16* w_nk, int 
     // halo mode: spatial taps reuse one shared-memory window (see TcParams::halo)
     const bool geom = p.sh == 1 && p.sw == 1 && p.kh * p.kw > 1 && p.kh <= 3 && p.kw <= 3 && p.Ho == p.Hi && p.Wo == p.Wi &&
                       w_batches <= 1 && p.Wo % 8 == 0 && p.Ho % 16 == 0;
-    if (allow_halo && halo_env && geom) {
+    if (allow_halo && geom) {
       t.halo = 1;
       t.BW = 8; t.BH = 16; t.BT = 1;
       t.hP = 16;
@@ -927,7 +863,7 @@ cudaError_t launch_conv_tc(const ConvP& p, const bf16* x, const bf16* w_nk, int 
     int stages = (int)((budget - fixed - a_ring) / (stage_bytes + 16));
     if (stages > 8) stages = 8;
     {
-      static int cap = -1;   // VT_TC_STAGES: experiment knob (pipeline-depth sensitivity)
+      static int cap = -1;   // VT_TC_STAGES caps the pipeline depth: lets the tests run the shortest (2-stage) ring
       if (cap < 0) { const char* e = getenv("VT_TC_STAGES"); cap = e ? atoi(e) : 0; }
       if (cap >= 2 && stages > cap) stages = cap;
     }
@@ -1004,12 +940,7 @@ cudaError_t launch_conv_tc(const ConvP& p, const bf16* x, const bf16* w_nk, int 
     cuuint64_t strides[4] = {(cuuint64_t)sw_ * 2, (cuuint64_t)sh_ * 2, (cuuint64_t)st_ * 2, (cuuint64_t)bs * 2};
     cuuint32_t box[5] = {64, (cuuint32_t)t.BW, (cuuint32_t)t.BH, (cuuint32_t)t.BT, 1};
     if (t.halo) { box[1] = (cuuint32_t)t.hP; box[2] = (cuuint32_t)(16 + p.kh - 1); }
-    cuuint32_t es[5] = {1, 1, 1, 1, 1};
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, const_cast<bf16*>(base), dims, strides, box, es,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { g_tc_err = "cuTensorMapEncodeTiled(activation) failed: " + std::to_string((int)r); return false; }
-    return true;
+    return encode_tmap_16b(m, 5, base, dims, strides, box, "activation", g_tc_err);
   };
   if (p.sh == 1) {
     if (!encode_act(&maps.a[0], x, p.Wi, p.Hi, p.isW, p.isH, p.Ti, p.isT, p.isB)) return cudaErrorInvalidValue;
@@ -1034,52 +965,41 @@ cudaError_t launch_conv_tc(const ConvP& p, const bf16* x, const bf16* w_nk, int 
     cuuint64_t dims[3] = {(cuuint64_t)(cw * Kpad), (cuuint64_t)Co_pad, (cuuint64_t)nb};
     cuuint64_t strides[2] = {(cuuint64_t)(cw * Kpad) * 2, (cuuint64_t)(nb > 1 ? w_batch_stride : (long long)cw * Kpad * Co_pad) * 2};
     cuuint32_t box[3] = {64, (cuuint32_t)t.BN, 1};
-    cuuint32_t es[3] = {1, 1, 1};
-    CUresult r = enc(&maps.b, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<bf16*>(w_nk), dims, strides, box, es,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { g_tc_err = "cuTensorMapEncodeTiled(weights) failed: " + std::to_string((int)r); return cudaErrorInvalidValue; }
+    if (!encode_tmap_16b(&maps.b, 3, w_nk, dims, strides, box, "weights", g_tc_err)) return cudaErrorInvalidValue;
   }
   // output / residual maps (output geometry) and the identity used by the residual-through-MMA K steps
   auto encode_out = [&](CUtensorMap* m, const void* base, int Tn, long long sW, long long sH, long long sT, long long sB, int bw, int bh, int bt) -> bool {
     cuuint64_t dims[5] = {(cuuint64_t)(cw * p.Co), (cuuint64_t)p.Wo, (cuuint64_t)p.Ho, (cuuint64_t)Tn, (cuuint64_t)p.B};
     cuuint64_t strides[4] = {(cuuint64_t)sW * 2, (cuuint64_t)sH * 2, (cuuint64_t)sT * 2, (cuuint64_t)sB * 2};
     cuuint32_t box[5] = {64, (cuuint32_t)bw, (cuuint32_t)bh, (cuuint32_t)bt, 1};
-    cuuint32_t es[5] = {1, 1, 1, 1, 1};
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, const_cast<void*>(base), dims, strides, box, es,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { g_tc_err = "cuTensorMapEncodeTiled(output/residual) failed: " + std::to_string((int)r); return false; }
-    return true;
+    return encode_tmap_16b(m, 5, base, dims, strides, box, "output/residual", g_tc_err);
   };
   maps.r = maps.a[0]; maps.e = maps.b;
   if (t.res_mma) {
     // 256 x 256 identity: bf16 I, or the 16 fp16 matrices 2^s * I of the split mode; built once per device on the launching stream
-    static bf16* ident_dev[2][64] = {{nullptr}};
-    int devid = 0;
-    cudaGetDevice(&devid);
-    if (devid < 0 || devid >= 64) { g_tc_err = "device index out of range"; return cudaErrorInvalidValue; }
+    static bf16* ident_dev[2][kMaxDevices] = {{nullptr}};
     const int ik = split ? 1 : 0;
-    if (!ident_dev[ik][devid]) {
+    if (!ident_dev[ik][dev]) {
       const int nmat = split ? 16 : 1;
-      cudaError_t e = cudaMalloc(&ident_dev[ik][devid], (size_t)nmat * 256 * 256 * sizeof(bf16));
+      cudaError_t e = cudaMalloc(&ident_dev[ik][dev], (size_t)nmat * 256 * 256 * sizeof(bf16));
       if (e != cudaSuccess) { g_tc_err = "cudaMalloc(identity)"; return e; }
-      for (int i = 0; i < nmat; ++i) fill_identity_kernel<<<256, 256, 0, s>>>(ident_dev[ik][devid] + (size_t)i * 256 * 256, ik, ldexpf(1.0f, i));
+      for (int i = 0; i < nmat; ++i) fill_identity_kernel<<<256, 256, 0, s>>>(ident_dev[ik][dev] + (size_t)i * 256 * 256, ik, ldexpf(1.0f, i));
     }
-    bf16* ident = ident_dev[ik][devid] + (size_t)(split ? ident_s : 0) * 256 * 256;
+    bf16* ident = ident_dev[ik][dev] + (size_t)(split ? ident_s : 0) * 256 * 256;
     if (!encode_out(&maps.r, p.res, p.resT, p.rsW, p.rsH, p.rsT, p.rsB, t.halo ? t.hP : t.BW, t.halo ? 16 + p.kh - 1 : t.BH, t.BT)) return cudaErrorInvalidValue;
     cuuint64_t dims[3] = {256, 256, 1};
     cuuint64_t strides[2] = {512, 256 * 512};
     cuuint32_t box[3] = {64, (cuuint32_t)t.BN, 1};
-    cuuint32_t es[3] = {1, 1, 1};
-    CUresult r = enc(&maps.e, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, ident, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { g_tc_err = "cuTensorMapEncodeTiled(identity) failed: " + std::to_string((int)r); return cudaErrorInvalidValue; }
+    if (!encode_tmap_16b(&maps.e, 3, ident, dims, strides, box, "identity", g_tc_err)) return cudaErrorInvalidValue;
   }
   {
-    cudaError_t e = ensure_func_attrs();
+    static SmemLimitOnce smem_limit;
+    cudaError_t e = smem_limit.ensure(dev, 227 * 1024, conv_tc_kernel<32, false>, conv_tc_kernel<64, false>, conv_tc_kernel<128, false>,
+                                      conv_tc_kernel<256, false>, conv_tc_kernel<32, true>, conv_tc_kernel<64, true>,
+                                      conv_tc_kernel<128, true>, conv_tc_kernel<256, true>);
     if (e != cudaSuccess) { g_tc_err = "cudaFuncSetAttribute(smem)"; return e; }
   }
+  const int num_sms = device_sms(dev);
   const unsigned grid = (unsigned)(t.num_tiles < num_sms ? t.num_tiles : num_sms);
   const double Mrows = (double)p.B * p.To * p.Ho * p.Wo;
   // plan key of the launch (profiler detail): geometry, tile, N tile, halo windows, fused LayerNorm, residual mode (m: through

@@ -156,8 +156,6 @@ cudaError_t launch_pack_w_tap_planes(const float* w, bf16* out, int Co, int Ci, 
 // x [batch][rows][cols] -> y [batch][cols][rows] (bf16), rows and cols multiples of 32
 cudaError_t launch_transpose_bf16(const bf16* x, bf16* y, int batch, int rows, int cols, cudaStream_t s, bool split = false);
 const char* conv_tc_last_error();
-// diagnostics: resident CTAs of the conv kernel per SM with `smem` dynamic bytes, plus its register / smem attributes
-int conv_tc_cluster_query(int smem, char* msg, int cap);
 
 // tblock_tc.cu: ResnetCausalBlock1D (k311 conv -> LayerNorm -> SiLU -> k311 conv + residual) for C = 128, v1.0 padding
 bool tblock_tc_supported(int B, int T, int H, int W, int C, bool planning = false);

@@ -1368,7 +1368,6 @@ int64_t vt_launch_count(int32_t reset) {
   return v;
 }
 
-int32_t vt_debug_cluster_query(int32_t smem, char* msg, int32_t cap) { return conv_tc_cluster_query(smem, msg, cap); }
 void vt_profile_start(void) { prof_set_detail(false); prof_start(); }
 void vt_profile_start_detailed(void) { prof_set_detail(true); prof_start(); }
 int32_t vt_profile_stop(char* json, int32_t cap) { return prof_stop(json, cap); }

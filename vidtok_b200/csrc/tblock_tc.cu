@@ -27,12 +27,12 @@
 #include <cuda.h>
 
 #include <cstdio>
-#include <cstdlib>
 #include <cstring>
 #include <string>
 
 #include "common.cuh"
 #include "kernels.h"
+#include "tc_host.h"
 #include "tc_ptx.cuh"
 
 namespace vt {
@@ -392,22 +392,6 @@ __global__ void __launch_bounds__(kThreadsTb, 1) tblock_tc_kernel(const __grid_c
   if (gtid == 0) bulk_wait<0>();   // the last bulk store has read shared memory before the CTA exits
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn tb_get_encode() {
-  static EncodeTiledFn fn = nullptr;
-  static bool tried = false;
-  if (!tried) {
-    tried = true;
-    void* f = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-      fn = (EncodeTiledFn)f;
-  }
-  return fn;
-}
-
 // strip box of 128 positions that tiles H x W exactly: the widest power-of-two BW <= 128 dividing W, BH = 128 / BW
 bool strip_box(int H, int W, int& BW, int& BH) {
   for (int bw = 128; bw >= 1; bw >>= 1) {
@@ -423,14 +407,11 @@ const char* tblock_tc_last_error() { return g_tb_err.c_str(); }
 
 bool tblock_tc_supported(int B, int T, int H, int W, int C, bool planning) {
   g_tb_err.clear();
-  static int env = -1;   // VT_TBLOCK=0: the model runs the block as two conv_tc launches instead (measurement knob)
-  if (env < 0) { const char* e = getenv("VT_TBLOCK"); env = e ? atoi(e) : 1; }
-  if (!env) { g_tb_err = "disabled (VT_TBLOCK=0)"; return false; }
   if (C != kC) { g_tb_err = "C != 128"; return false; }
   if (B <= 0 || T <= 0) { g_tb_err = "empty"; return false; }
   int BW, BH;
   if (!strip_box(H, W, BW, BH)) { g_tb_err = "H x W not tileable by a 128-position box"; return false; }
-  if (!planning && !tb_get_encode()) { g_tb_err = "cuTensorMapEncodeTiled unavailable"; return false; }
+  if (!planning && !tmap_encoder()) { g_tb_err = "cuTensorMapEncodeTiled unavailable"; return false; }
   return true;
 }
 
@@ -441,8 +422,7 @@ cudaError_t launch_tblock_tc(const bf16* n1, const bf16* x, const bf16* w1, cons
                              const float* gamma_out, const float* beta_out, bool out_silu, int B, int T, int H, int W,
                              cudaStream_t s, const TbCache* cache) {
   g_tb_err.clear();
-  EncodeTiledFn enc = tb_get_encode();
-  if (!enc) { g_tb_err = "cuTensorMapEncodeTiled unavailable"; return cudaErrorNotSupported; }
+  if (!tmap_encoder()) { g_tb_err = "cuTensorMapEncodeTiled unavailable"; return cudaErrorNotSupported; }
   TbParams p;
   memset(&p, 0, sizeof(p));
   if (!strip_box(H, W, p.BW, p.BH)) { g_tb_err = "H x W not tileable"; return cudaErrorInvalidValue; }
@@ -471,52 +451,36 @@ cudaError_t launch_tblock_tc(const bf16* n1, const bf16* x, const bf16* w1, cons
     cuuint64_t dims[5] = {(cuuint64_t)kC, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)T, (cuuint64_t)B};
     cuuint64_t strides[4] = {(cuuint64_t)kC * 2, (cuuint64_t)W * kC * 2, (cuuint64_t)H * W * kC * 2, (cuuint64_t)T * H * W * kC * 2};
     cuuint32_t box[5] = {64, (cuuint32_t)p.BW, (cuuint32_t)p.BH, 1, 1};
-    cuuint32_t es[5] = {1, 1, 1, 1, 1};
-    CUresult r = enc(&maps.n1, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, const_cast<bf16*>(n1), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { g_tb_err = "cuTensorMapEncodeTiled(n1) failed: " + std::to_string((int)r); return cudaErrorInvalidValue; }
+    if (!encode_tmap_16b(&maps.n1, 5, n1, dims, strides, box, "n1", g_tb_err)) return cudaErrorInvalidValue;
     maps.cn1 = maps.n1;
     // x and out: one consumer warpgroup's 64 rows of a strip, the rows (h, w) in strip order
     const int bw = p.BW < 64 ? p.BW : 64;
     cuuint32_t box64[5] = {64, (cuuint32_t)bw, (cuuint32_t)(64 / bw), 1, 1};
-    for (int i = 0; i < 2; ++i) {
-      r = enc(i ? &maps.out : &maps.x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, i ? (void*)out : const_cast<bf16*>(x), dims, strides, box64, es,
-              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      if (r != CUDA_SUCCESS) { g_tb_err = "cuTensorMapEncodeTiled(x / out) failed: " + std::to_string((int)r); return cudaErrorInvalidValue; }
-    }
+    for (int i = 0; i < 2; ++i)
+      if (!encode_tmap_16b(i ? &maps.out : &maps.x, 5, i ? (const void*)out : x, dims, strides, box64, "x / out", g_tb_err))
+        return cudaErrorInvalidValue;
     if (p.cached_in) {
       dims[3] = 2;
       strides[3] = 2ull * H * W * kC * 2;
-      r = enc(&maps.cn1, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, const_cast<bf16*>(p.cn1_in), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-              CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      if (r != CUDA_SUCCESS) { g_tb_err = "cuTensorMapEncodeTiled(n1 cache) failed: " + std::to_string((int)r); return cudaErrorInvalidValue; }
+      if (!encode_tmap_16b(&maps.cn1, 5, p.cn1_in, dims, strides, box, "n1 cache", g_tb_err)) return cudaErrorInvalidValue;
     }
   }
   for (int i = 0; i < 2; ++i) {
     cuuint64_t dims[3] = {(cuuint64_t)(3 * kC), (cuuint64_t)kC, 1};
     cuuint64_t strides[2] = {(cuuint64_t)(3 * kC) * 2, (cuuint64_t)(3 * kC) * kC * 2};
     cuuint32_t box[3] = {64, (cuuint32_t)kC, 1};
-    cuuint32_t es[3] = {1, 1, 1};
-    CUresult r = enc(i ? &maps.w2 : &maps.w1, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<bf16*>(i ? w2 : w1), dims, strides, box, es,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { g_tb_err = "cuTensorMapEncodeTiled(weights) failed: " + std::to_string((int)r); return cudaErrorInvalidValue; }
+    if (!encode_tmap_16b(i ? &maps.w2 : &maps.w1, 3, i ? w2 : w1, dims, strides, box, "weights", g_tb_err)) return cudaErrorInvalidValue;
   }
-  static bool attr[64] = {false};
-  static int sms[64] = {0};
   int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev < 0 || dev >= 64) return cudaErrorInvalidDevice;
-  if (!attr[dev]) {
-    for (auto k : {tblock_tc_kernel<false>, tblock_tc_kernel<true>}) {
-      cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
-      if (e != cudaSuccess) { g_tb_err = "cudaFuncSetAttribute(smem)"; return e; }
-    }
-    attr[dev] = true;
-    cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, dev);
-    if (sms[dev] <= 0) sms[dev] = 132;
+  const cudaError_t dev_err = current_device(dev);
+  if (dev_err != cudaSuccess) { g_tb_err = "no current device, or its index is out of range"; return dev_err; }
+  {
+    static SmemLimitOnce smem_limit;
+    const cudaError_t e = smem_limit.ensure(dev, 227 * 1024, tblock_tc_kernel<false>, tblock_tc_kernel<true>);
+    if (e != cudaSuccess) { g_tb_err = "cudaFuncSetAttribute(smem)"; return e; }
   }
-  const unsigned grid = (unsigned)(p.num_strips < sms[dev] ? p.num_strips : sms[dev]);
+  const int num_sms = device_sms(dev);
+  const unsigned grid = (unsigned)(p.num_strips < num_sms ? p.num_strips : num_sms);
   const double M = (double)B * T * H * W;
   char det[96] = "";
   if (prof_enabled()) snprintf(det, sizeof(det), cache ? "strip %dx%d T%d ln_out%d cache%d" : "strip %dx%d T%d ln_out%d", p.BH, p.BW, T,
