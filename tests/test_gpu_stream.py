@@ -228,6 +228,54 @@ def test_v11_stream_equals_tile_encode_without_overlap(case):
         assert torch.equal(x_s, x_t)
 
 
+@pytest.mark.parametrize("case", ["tiny_kl_v10", "tiny_fsq_v11_tiled"])
+def test_fresh_chunk_state_refuses_a_later_chunk(case):
+    """A chunk state that has not run a first chunk holds no cached frames: a later chunk is refused with VT_ERR_NOT_READY
+    (-3), naming the cache, before anything reads it; the same state then takes a first chunk as a fresh stream does."""
+    from vidtok_b200.engine import _ptr, _stream_ptr
+    from vidtok_b200.streaming import DecodeStream, EncodeStream
+    from vidtok_b200.synth import synth_clip
+    d, meta = load_golden(case)
+    model = _model(resolved_model_cfg(meta), synth_weights(meta, d))
+    model.precision = "bf16"
+    s = model.spec
+    tdf = int(s.time_downsample_factor)
+    B, _, _, H, W = meta["input"]
+    x = synth_clip(B, 1 + tdf, H, W, seed=meta["input_seed"]).cuda()
+    dev = x.device
+    with torch.no_grad():
+        enc = EncodeStream(model, B, H, W)
+        lib = enc.native.lib
+        Hz, Wz = enc.Hz, enc.Wz
+        noise = torch.randn((B, s.z_channels, 2, Hz, Wz))   # 1 + tdf frames: two latent frames
+        xc = x[:, :, 1:].contiguous()                        # tdf frames: a later chunk
+        nc = noise[:, :, 1:].contiguous().to(dev)
+        z = torch.empty((B, s.z_channels, 1, Hz, Wz), device=dev)
+        idx = torch.empty((B, 1, Hz, Wz), dtype=torch.int32, device=dev)
+        kl = torch.zeros((1,), device=dev)
+        ws = enc.state.workspace(tdf)
+        rc = lib.vt_encode_chunk(enc.state.handle, 0, _ptr(xc), s.in_channels, tdf, _ptr(nc), _ptr(z), _ptr(idx), _ptr(kl),
+                                 _ptr(ws), ws.numel(), _stream_ptr(dev))
+        msg = lib.vt_last_error().decode()
+        assert rc == -3 and msg.startswith("cache encoder.") and "empty" in msg, (rc, msg)
+        z_s, _ = enc.push(x, noise=noise)
+        enc.close()
+        z_f, _ = _stream_encode(model, x, [1 + tdf], noise)
+        assert torch.equal(z_s, z_f)
+
+        dec = DecodeStream(model, B, Hz, Wz)
+        zc = z_f[:, :, 1:].float().contiguous()
+        To = dec.native.decoded_frames(1) if s.version == 1 else tdf
+        out = torch.empty((B, s.out_ch, To, H, W), device=dev)
+        ws = dec.state.workspace(1)
+        rc = lib.vt_decode_chunk(dec.state.handle, 0, _ptr(zc), s.z_channels, 1, _ptr(out), _ptr(ws), ws.numel(), _stream_ptr(dev))
+        msg = lib.vt_last_error().decode()
+        assert rc == -3 and msg.startswith("cache decoder.") and "empty" in msg, (rc, msg)
+        x_s = dec.push(z_f)
+        dec.close()
+        assert torch.equal(x_s, _stream_decode(model, z_f, [z_f.shape[2]]))
+
+
 # ---------------------------------------------------------------------------------------------------------------
 # op level: the cached fused temporal block
 # ---------------------------------------------------------------------------------------------------------------

@@ -188,9 +188,4 @@ struct ConvP {
   int fsq_levels[VT_MAX_FSQ];
 };
 
-struct ConvLaunch {  // host-side convenience
-  long long M;       // B*To*Ho*Wo
-  int K;             // kt*kh*kw*Ci
-};
-
 }  // namespace vt

@@ -255,12 +255,15 @@ struct Act {
   long long frame() const { return (long long)H * W * C; }
 };
 
+// A per-layer chunk cache, double-buffered: a chunk reads what the previous chunk left and writes its own tail for the next.
 struct CacheBuf {
   void* buf[2] = {nullptr, nullptr};
   int cur = 0;
-  int T = 0;
   size_t bytes = 0;
   bool valid = false;
+  void* in() const { return buf[cur]; }         // the previous chunk's tail, read by this chunk
+  void* out() const { return buf[cur ^ 1]; }    // this chunk's tail, read by the next chunk
+  void commit() { cur ^= 1; valid = true; }
 };
 
 }  // namespace vt
@@ -348,6 +351,53 @@ struct ConvOpt {
   mutable bool fused_reg = false;
 };
 
+// ---- ConvP layout: every descriptor the executor and the operator entry points launch is built from these ------------
+// zeroed but for the input extent, unit strides and unit upsampling
+static ConvP conv_p(int B, int Ti, int Hi, int Wi, int Ci) {
+  ConvP p;
+  memset(&p, 0, sizeof(p));
+  p.B = B; p.Ti = Ti; p.Hi = Hi; p.Wi = Wi; p.Ci = Ci;
+  p.st = p.sh = p.sw = 1; p.ut = p.uh = p.uw = 1;
+  return p;
+}
+// element strides of one operand
+struct Strides { long long B, T, H, W, C; };
+// channels-last [B][T][H][W][C] with cw storage elements per channel (2 for split rows); bs >= 0 overrides the batch stride
+// (views into a larger tensor)
+static Strides cl_strides(int T, int H, int W, int C, long long cw, long long bs = -1) {
+  const long long sW = cw * C, sH = W * sW, sT = H * sH;
+  return {bs >= 0 ? bs : T * sT, sT, sH, sW, 1};
+}
+// the caller's fp32 [B][C][T][H][W] tensors
+static Strides ncdhw_strides(int C, int T, int H, int W) {
+  const long long sT = (long long)H * W, sC = T * sT;
+  return {C * sC, sT, W, 1, sC};
+}
+static void set_in(ConvP& p, const Strides& s) { p.isB = s.B; p.isT = s.T; p.isH = s.H; p.isW = s.W; p.isC = s.C; }
+static void set_out(ConvP& p, const Strides& s) { p.osB = s.B; p.osT = s.T; p.osH = s.H; p.osW = s.W; p.osC = s.C; }
+static void set_res(ConvP& p, const Strides& s) { p.rsB = s.B; p.rsT = s.T; p.rsH = s.H; p.rsW = s.W; }   // channel stride 1
+// To / Ho / Wo from the input extent, taps, strides, upsampling and front padding already in p; pt_back, ph1, pw1: the
+// padding behind the end of each axis.  False when the output is empty.
+static bool conv_out_size(ConvP& p, int pt_back, int ph1, int pw1) {
+  p.To = (p.t_rep + p.ut * p.Ti + p.pt + pt_back - p.kt) / p.st + 1 - p.to_off;
+  p.Ho = (p.uh * p.Hi + p.ph + ph1 - p.kh) / p.sh + 1;
+  p.Wo = (p.uw * p.Wi + p.pw + pw1 - p.kw) / p.sw + 1;
+  return p.To > 0 && p.Ho > 0 && p.Wo > 0;
+}
+// The encoder stem on conv_stem: 3x3x3 conv_in from the caller's fp32 [B,Ci,T,H,W] tensor after t_rep copies of frame 0,
+// channels-last output.  Time padding mode, cache and acc_scale are the caller's.
+static ConvP stem_p(int B, int Ci, int T, int H, int W, int Co, int t_rep, bool split, const float* bias) {
+  ConvP p = conv_p(B, T, H, W, Ci);
+  p.split = split ? 1 : 0;
+  set_in(p, ncdhw_strides(Ci, T, H, W));
+  p.To = T + t_rep; p.Ho = H; p.Wo = W; p.Co = Co;
+  set_out(p, cl_strides(p.To, H, W, Co, split ? 2 : 1));
+  p.kt = p.kh = p.kw = 3;
+  p.pt = 2; p.ph = 1; p.pw = 1; p.t_rep = t_rep;
+  p.bias = bias;
+  return p;
+}
+
 // effective precision of one stack: MIXED = encoder EXACT_TC, decoder BF16
 static inline int stack_prec(int precision, bool decoder) {
   if (precision == VT_PREC_MIXED) return decoder ? VT_PREC_BF16 : VT_PREC_EXACT_TC;
@@ -433,19 +483,24 @@ struct Exec {
     }
     return val;
   }
-  CacheBuf* get_cache(const std::string& key, int T, size_t bytes) {
+  // The chunk cache under `key`, (re)allocated or taken from the pool when its size changes.  A later chunk of a real run reads
+  // what the previous chunk committed: an empty cache there is VT_ERR_NOT_READY.  Null on error.
+  CacheBuf* cache(const std::string& key, size_t bytes) {
     CacheBuf& c = ck->caches[key];
     if (c.bytes != bytes) {
-      if (dry) { c.bytes = bytes; c.T = T; return &c; }
+      if (dry) { c.bytes = bytes; return &c; }
       for (int i = 0; i < 2; ++i) {
         if (c.buf[i]) pool_put(m, c.bytes, c.buf[i]);
         c.buf[i] = pool_take(m, bytes);
         if (!c.buf[i] && !cuda(cudaMalloc(&c.buf[i], bytes), "cudaMalloc(causal cache)")) return nullptr;
       }
-      c.bytes = bytes; c.T = T; c.valid = false; c.cur = 0;
+      c.bytes = bytes; c.valid = false; c.cur = 0;
     }
+    if (!dry && !ck->first && !c.valid) { rc = fail(VT_ERR_NOT_READY, "cache %s empty on a non-first chunk", key.c_str()); return nullptr; }
     return &c;
   }
+  // this chunk's tail becomes the next chunk's input (a dry run leaves the caches as they are)
+  void commit(CacheBuf* c) { if (c && !dry) c->commit(); }
   // streaming: caches live across chunks (v1.1 tiling, v1.0 streams)
   bool streaming() const { return ck && ck->persist; }
   // dst [rows][2][fe] := the last two frames of [front (2 frames) | x (T frames)], rows of x T * fe apart; null front: zero
@@ -471,8 +526,8 @@ struct Exec {
   Act conv_ext_stream(const ConvW& w, const float* x, int B, int C, int T, int H, int W, int t_rep, const std::string& key, ConvOpt o) {
     Act out;
     const long long rows = (long long)B * C, fe = (long long)H * W;
-    CacheBuf* cb = get_cache(key, 2, (size_t)rows * 2 * fe * sizeof(float));
-    if (!ok()) return out;
+    CacheBuf* cb = cache(key, (size_t)rows * 2 * fe * sizeof(float));
+    if (!cb) return out;
     Act in;
     in.B = B; in.C = C; in.H = H; in.W = W;
     if (ck->first) {
@@ -482,25 +537,24 @@ struct Exec {
       if (ok() && !dry) {
         if (t_rep > 0 && T == 1) {   // padded input [x0 ... x0]
           for (int j = 0; j < 2; ++j)
-            cuda(launch_copy_frames(DT_F32, x, (float*)cb->buf[cb->cur ^ 1] + j * fe, (int)rows, fe, 2 * fe, fe, s), "cache tail");
+            cuda(launch_copy_frames(DT_F32, x, (float*)cb->out() + j * fe, (int)rows, fe, 2 * fe, fe, s), "cache tail");
         } else {
-          tail2(DT_F32, x, nullptr, cb->buf[cb->cur ^ 1], rows, T, fe);
+          tail2(DT_F32, x, nullptr, cb->out(), rows, T, fe);
         }
       }
     } else {
       float* xc = (float*)alloc((size_t)rows * (2 + T) * fe * sizeof(float));
       if (!ok()) return out;
       if (!dry) {
-        if (!cb->valid) { rc = fail(VT_ERR_NOT_READY, "cache %s empty on a non-first chunk", key.c_str()); return out; }
-        cat2(DT_F32, cb->buf[cb->cur], x, xc, rows, T, fe);
-        tail2(DT_F32, x, cb->buf[cb->cur], cb->buf[cb->cur ^ 1], rows, T, fe);
+        cat2(DT_F32, cb->in(), x, xc, rows, T, fe);
+        tail2(DT_F32, x, cb->in(), cb->out(), rows, T, fe);
       }
       in.p = xc; in.T = 2 + T;
       o.ext_in = xc; o.to_off = 2;
       out = conv(w, in, o);
       ar.release(xc);
     }
-    if (!dry) { cb->cur ^= 1; cb->valid = true; }
+    commit(cb);
     return out;
   }
 
@@ -509,19 +563,19 @@ struct Exec {
     Act out;
     if (!ok()) return out;
     const bool v11 = m->desc.version == 1;
-    ConvP p;
-    memset(&p, 0, sizeof(p));
-    p.B = in.B; p.Ti = in.T; p.Hi = in.H; p.Wi = in.W; p.Ci = in.C;
+    ConvP p = conv_p(in.B, in.T, in.H, in.W, in.C);
     if (in.C != w.Ci) { rc = fail(VT_ERR_INVALID, "conv: Cin mismatch %d vs %d", in.C, w.Ci); return out; }
     if (o.ext_in && o.ext_in_indices) {
-      p.isC = 0; p.isT = (long long)in.H * in.W; p.isB = p.isT * in.T; p.isH = in.W; p.isW = 1;
+      Strides is = ncdhw_strides(1, in.T, in.H, in.W);   // the int32 token tensor [B,T,H,W]: no channel axis
+      is.C = 0;
+      set_in(p, is);
       p.fsq_d = m->desc.fsq_num_levels;
       for (int i = 0; i < VT_MAX_FSQ && i < p.fsq_d; ++i) p.fsq_levels[i] = m->desc.fsq_levels[i];
     } else if (o.ext_in) {
-      p.isC = (long long)in.T * in.H * in.W; p.isB = p.isC * in.C; p.isT = (long long)in.H * in.W; p.isH = in.W; p.isW = 1;
+      set_in(p, ncdhw_strides(in.C, in.T, in.H, in.W));
     } else {
       // (stride overrides in ConvOpt count storage elements: bf16 values for split rows)
-      p.isC = 1; p.isW = (long long)cw * in.C; p.isH = (long long)in.W * p.isW; p.isT = p.isH * in.H; p.isB = o.in_bs >= 0 ? o.in_bs : p.isT * in.T;
+      set_in(p, cl_strides(in.T, in.H, in.W, in.C, cw, o.in_bs));
     }
     p.split = split ? 1 : 0;
     p.acc_scale = split ? 1.0f / w.wscale3 : 1.0f;
@@ -541,23 +595,19 @@ struct Exec {
     const int ph0 = o.ph0 >= 0 ? o.ph0 : hp / 2, ph1 = o.ph1 >= 0 ? o.ph1 : hp - hp / 2;
     const int pw0 = o.pw0 >= 0 ? o.pw0 : wp / 2, pw1 = o.pw1 >= 0 ? o.pw1 : wp - wp / 2;
     p.ph = ph0; p.pw = pw0;
-    const int Tv = o.t_rep + o.ut * in.T;
-    p.To = (Tv + p.pt + ptb - w.kt) / o.st + 1 - o.to_off;
-    p.Ho = (o.uh * in.H + ph0 + ph1 - w.kh) / o.sh + 1;
-    p.Wo = (o.uw * in.W + pw0 + pw1 - w.kw) / o.sw + 1;
     p.Co = w.Co;
-    if (p.To <= 0 || p.Ho <= 0 || p.Wo <= 0) { rc = fail(VT_ERR_INVALID, "conv: empty output"); return out; }
+    if (!conv_out_size(p, ptb, ph1, pw1)) { rc = fail(VT_ERR_INVALID, "conv: empty output"); return out; }
     out.B = in.B; out.T = p.To; out.H = p.Ho; out.W = p.Wo; out.C = w.Co;
     if (o.ext_out) {
       out.p = o.ext_out;
-      p.osC = (long long)p.To * p.Ho * p.Wo; p.osB = p.osC * p.Co; p.osT = (long long)p.Ho * p.Wo; p.osH = p.Wo; p.osW = 1;
+      set_out(p, ncdhw_strides(p.Co, p.To, p.Ho, p.Wo));
     } else if (o.out_view) {
       out.p = o.out_view;
-      p.osC = 1; p.osW = o.ov_sW; p.osH = o.ov_sH; p.osT = o.ov_sT; p.osB = o.ov_sB;
+      set_out(p, Strides{o.ov_sB, o.ov_sT, o.ov_sH, o.ov_sW, 1});
     } else {
       out.p = alloc((size_t)out.elems() * dtype_size(ta));
       out.owned = true;
-      p.osC = 1; p.osW = (long long)cw * p.Co; p.osH = (long long)p.Wo * p.osW; p.osT = p.osH * p.Ho; p.osB = p.osT * p.To;
+      set_out(p, cl_strides(p.To, p.Ho, p.Wo, p.Co, cw));
     }
     if (!ok()) return out;
     // time padding mode
@@ -565,26 +615,24 @@ struct Exec {
     CacheBuf* cb = nullptr;
     int cache_off = 0;
     if (v11 && w.kt > 1) p.t_mode = 1;
-    if (w.kt > 1 && (v11 || streaming())) {
-      if (ck && o.cache_key && ck->persist) {
-        cache_off = cache_offset_for(o.cache_key);
-        cb = get_cache(o.cache_key, p.pt, (size_t)in.B * p.pt * in.frame() * dtype_size(o.ext_in ? DT_F32 : ta));
-        if (!ok()) return out;
-        if (!ck->first) {
-          if (!dry && !cb->valid) { rc = fail(VT_ERR_NOT_READY, "causal cache %s empty on a non-first chunk", o.cache_key); return out; }
-          p.t_mode = 2;
-          p.cache = cb->buf[cb->cur];
-          p.cacheT = p.pt;   // (folded 2x time upsampling: frames of the upsampled axis)
-        }
+    if (w.kt > 1 && streaming() && o.cache_key) {
+      cache_off = cache_offset_for(o.cache_key);
+      cb = cache(o.cache_key, (size_t)in.B * p.pt * in.frame() * dtype_size(o.ext_in ? DT_F32 : ta));
+      if (!cb) return out;
+      if (!ck->first) {
+        p.t_mode = 2;
+        p.cache = cb->in();
+        p.cacheT = p.pt;   // (folded 2x time upsampling: frames of the upsampled axis)
       }
     }
     p.bias = w.bias;
     p.res_mode = o.res_mode;
     p.ra = o.ra; p.rb = o.rb;
+    CacheBuf* pc = nullptr;   // avg-pool branch of res_mode 3
     if (o.res_mode) {
       const Act& r = *o.res;
       p.res = r.p;
-      p.rsW = (long long)cw * r.C; p.rsH = (long long)r.W * p.rsW; p.rsT = p.rsH * r.H; p.rsB = o.res_bs >= 0 ? o.res_bs : p.rsT * r.T;
+      set_res(p, cl_strides(r.T, r.H, r.W, r.C, cw, o.res_bs));
       p.resT = r.T;
       if (r.C != w.Co) { rc = fail(VT_ERR_INVALID, "conv: residual channel mismatch"); return out; }
       if (o.res_mode == 3) {
@@ -592,10 +640,9 @@ struct Exec {
         p.res_pool_off = o.res_pool_off;
         if (v11) p.res_t_mode = 1;   // replicate (model_3dcausal_v1_1.py:293-294)
         if (streaming() && o.cache_key) {
-          const std::string pk = std::string(o.cache_key) + "#pool";
-          CacheBuf* pc = get_cache(pk, 1, (size_t)r.B * r.frame() * dtype_size(ta));
-          if (!ok()) return out;
-          if (!ck->first) { p.res_t_mode = 2; p.res_cache = pc->buf[pc->cur]; }
+          pc = cache(std::string(o.cache_key) + "#pool", (size_t)r.B * r.frame() * dtype_size(ta));
+          if (!pc) return out;
+          if (!ck->first) { p.res_t_mode = 2; p.res_cache = pc->in(); }
         }
       }
     }
@@ -642,33 +689,28 @@ struct Exec {
       }
       // cache := tail of the padded input (after the conv consumed the old cache)
       if (cb) {
-        const int nxt = cb->cur ^ 1;
         if (o.ut == 2) {
           // v1.0 folded 2x time upsampling: the last two upsampled frames are the last input frame twice
           const char* last = (const char*)in.p + (size_t)(in.T - 1) * in.frame() * dtype_size(tin);
           for (int j = 0; j < 2 && ok(); ++j)
-            cuda(launch_copy_frames(tin, last, (char*)cb->buf[nxt] + (size_t)j * in.frame() * dtype_size(tin), in.B, (long long)in.T * in.frame(),
+            cuda(launch_copy_frames(tin, last, (char*)cb->out() + (size_t)j * in.frame() * dtype_size(tin), in.B, (long long)in.T * in.frame(),
                                     2 * in.frame(), in.frame(), s), "cache_update");
           if (!ok()) return out;
         } else {
           // v1.0: zero frames in front of the first chunk (v1.1 replicates frame 0)
           const bool zero_front = !v11 && ck->first;
-          if (zero_front && !cuda(cudaMemsetAsync(cb->buf[cb->cur], 0, cb->bytes, s), "cache_update")) return out;
-          if (!cuda(launch_cache_update(tin, o.ext_in ? (const void*)o.ext_in : in.p, cb->buf[cb->cur], cb->buf[nxt], in.B, in.T,
+          if (zero_front && !cuda(cudaMemsetAsync(cb->in(), 0, cb->bytes, s), "cache_update")) return out;
+          if (!cuda(launch_cache_update(tin, o.ext_in ? (const void*)o.ext_in : in.p, cb->in(), cb->out(), in.B, in.T,
                                         p.pt, cache_off, ck->first && !zero_front, in.frame(), o.ext_in ? p.isB : p.isB / cw, s), "cache_update")) return out;
         }
-        cb->cur = nxt;
-        cb->valid = true;
+        commit(cb);
       }
-      if (o.res_mode == 3 && streaming() && o.cache_key) {
+      if (pc) {
         // avg-pool branch cache = last frame of the padded input (model_3dcausal_v1_1.py:298)
-        CacheBuf& pc = ck->caches[std::string(o.cache_key) + "#pool"];
         const Act& r = *o.res;
-        const int nxt = pc.cur ^ 1;
-        if (!cuda(launch_copy_frames(ta, (const char*)r.p + (size_t)(r.T - 1) * r.frame() * dtype_size(ta), pc.buf[nxt], r.B,
+        if (!cuda(launch_copy_frames(ta, (const char*)r.p + (size_t)(r.T - 1) * r.frame() * dtype_size(ta), pc->out(), r.B,
                                      (long long)r.T * r.frame(), r.frame(), r.frame(), s), "pool cache")) return out;
-        pc.cur = nxt;
-        pc.valid = true;
+        commit(pc);
       }
     }
     return out;
@@ -735,14 +777,11 @@ struct Exec {
     TbCache tc;
     if (streaming()) {
       const size_t cbytes = (size_t)st.x.B * 2 * st.x.frame() * sizeof(bf16);
-      cc[0] = get_cache(r.key + ".conv1", 2, cbytes);
-      if (ok()) cc[1] = get_cache(r.key + ".conv2", 2, cbytes);
-      if (!ok()) return true;
-      if (!ck->first) {
-        if (!dry && (!cc[0]->valid || !cc[1]->valid)) { rc = fail(VT_ERR_NOT_READY, "causal cache %s empty on a non-first chunk", r.key.c_str()); return true; }
-        tc.n1_in = (const bf16*)cc[0]->buf[cc[0]->cur]; tc.h_in = (const bf16*)cc[1]->buf[cc[1]->cur];
-      }
-      tc.n1_out = (bf16*)cc[0]->buf[cc[0]->cur ^ 1]; tc.h_out = (bf16*)cc[1]->buf[cc[1]->cur ^ 1];
+      cc[0] = cache(r.key + ".conv1", cbytes);
+      if (cc[0]) cc[1] = cache(r.key + ".conv2", cbytes);
+      if (!cc[1]) return true;
+      if (!ck->first) { tc.n1_in = (const bf16*)cc[0]->in(); tc.h_in = (const bf16*)cc[1]->in(); }
+      tc.n1_out = (bf16*)cc[0]->out(); tc.h_out = (bf16*)cc[1]->out();
     }
     Act n1 = take_norm(st, r.n1, true, true);
     Act out = new_act(st.x.B, st.x.T, st.x.H, st.x.W, 128);
@@ -752,8 +791,8 @@ struct Exec {
       cuda(launch_tblock_tc((const bf16*)n1.p, (const bf16*)st.x.p, r.c1.w_nk, r.c1.bias, r.n2.gamma, r.n2.beta, r.c2.w_nk, r.c2.bias,
                             (bf16*)out.p, next ? (bf16*)out2.p : nullptr, next ? next->gamma : nullptr, next ? next->beta : nullptr,
                             next_silu, st.x.B, st.x.T, st.x.H, st.x.W, s, cc[0] ? &tc : nullptr), tblock_tc_last_error());
-      for (CacheBuf* c : cc)
-        if (c) { c->cur ^= 1; c->valid = true; }
+      commit(cc[0]);
+      commit(cc[1]);
     }
     free_act(n1);
     if (st.n.p) free_act(st.n);
@@ -794,18 +833,16 @@ struct Exec {
   bool attention_tc(const Act& q, const Act& k, const Act& v, Act& o) {
     const int frames = q.B * q.T, tokens = q.H * q.W, C = q.C;
     if (!tcm || tokens % 64 != 0 || C % 64 != 0 || tokens % 32 != 0) return false;
-    ConvP ps;
-    memset(&ps, 0, sizeof(ps));
-    ps.B = frames; ps.Ti = 1; ps.Hi = q.H; ps.Wi = q.W; ps.Ci = C;
+    ConvP ps = conv_p(frames, 1, q.H, q.W, C);
     ps.split = split ? 1 : 0;
-    ps.isC = 1; ps.isW = (long long)cw * C; ps.isH = (long long)q.W * ps.isW; ps.isT = ps.isH * q.H; ps.isB = ps.isT;
+    set_in(ps, cl_strides(1, q.H, q.W, C, cw));
     ps.To = 1; ps.Ho = q.H; ps.Wo = q.W; ps.Co = tokens;
-    ps.osC = 1; ps.osW = tokens; ps.osH = (long long)q.W * tokens; ps.osT = ps.osH * q.H; ps.osB = ps.osT;
-    ps.kt = ps.kh = ps.kw = 1; ps.st = ps.sh = ps.sw = 1; ps.ut = ps.uh = ps.uw = 1;
+    set_out(ps, cl_strides(1, q.H, q.W, tokens, 1));   // fp32 scores
+    ps.kt = ps.kh = ps.kw = 1;
     ps.ra = 0.f; ps.rb = 1.0f / sqrtf((float)C);
     ConvP pv = ps;
-    pv.Ci = tokens; pv.isW = (long long)cw * tokens; pv.isH = (long long)q.W * pv.isW; pv.isT = pv.isH * q.H; pv.isB = pv.isT;
-    pv.Co = C; pv.osW = (long long)cw * C; pv.osH = (long long)q.W * pv.osW; pv.osT = pv.osH * q.H; pv.osB = pv.osT;
+    pv.Ci = tokens; set_in(pv, cl_strides(1, q.H, q.W, tokens, cw));
+    pv.Co = C; set_out(pv, cl_strides(1, q.H, q.W, C, cw));
     pv.rb = 1.0f;
     if (!dry && (!conv_tc_supported(ps, DT_F32) || !conv_tc_supported(pv, ta))) return false;
     o = new_act(q.B, q.T, q.H, q.W, C);
@@ -1029,8 +1066,8 @@ struct Exec {
     const bool first = !ck || ck->first;
     CacheBuf* cb = nullptr;
     if (persist) {
-      cb = get_cache(lv.tkey + "#up", n, (size_t)x.B * n * fe * es);
-      if (!ok()) { free_act(x); return; }
+      cb = cache(lv.tkey + "#up", (size_t)x.B * n * fe * es);
+      if (!cb) { free_act(x); return; }
     }
     Act xu;
     Act view;
@@ -1050,10 +1087,9 @@ struct Exec {
           if (nb > 0) cuda(launch_time_interp2x(ta, xb + (size_t)na * fe * es, yb + (size_t)2 * na * fe * es, 1, nb, (long long)x.H * x.W, x.C, s), "time_interp2x");
         }
         if (cb) {  // cache = x[:, -n:]
-          const int nxt = cb->cur ^ 1;
           if (x.T < n) { rc = fail(VT_ERR_INVALID, "time_up: first chunk shorter than num_temp_upsample"); }
-          else cuda(launch_copy_frames(ta, (const char*)x.p + (size_t)(x.T - n) * fe * es, cb->buf[nxt], x.B, (long long)x.T * fe, (long long)n * fe, (long long)n * fe, s), "up cache");
-          cb->cur = nxt; cb->valid = true;
+          else cuda(launch_copy_frames(ta, (const char*)x.p + (size_t)(x.T - n) * fe * es, cb->out(), x.B, (long long)x.T * fe, (long long)n * fe, (long long)n * fe, s), "up cache");
+          commit(cb);
         }
       }
       view = xu;
@@ -1062,15 +1098,11 @@ struct Exec {
       Act xc = new_act(x.B, n + x.T, x.H, x.W, x.C);
       big = new_act(x.B, 2 * (n + x.T), x.H, x.W, x.C);
       if (ok() && !dry) {
-        if (!cb->valid) rc = fail(VT_ERR_NOT_READY, "time_up cache empty on a non-first chunk");
-        if (ok()) {
-          cuda(launch_copy_frames(ta, cb->buf[cb->cur], xc.p, x.B, (long long)n * fe, (long long)(n + x.T) * fe, (long long)n * fe, s), "up cat a");
-          cuda(launch_copy_frames(ta, x.p, (char*)xc.p + (size_t)n * fe * es, x.B, (long long)x.T * fe, (long long)(n + x.T) * fe, (long long)x.T * fe, s), "up cat b");
-          const int nxt = cb->cur ^ 1;
-          cuda(launch_copy_frames(ta, (const char*)xc.p + (size_t)(x.T - n) * fe * es, cb->buf[nxt], x.B, (long long)(n + x.T) * fe, (long long)n * fe, (long long)n * fe, s), "up cache");
-          cb->cur = nxt;
-          cuda(launch_time_interp2x(ta, xc.p, big.p, x.B, n + x.T, (long long)x.H * x.W, x.C, s), "time_interp2x");
-        }
+        cuda(launch_copy_frames(ta, cb->in(), xc.p, x.B, (long long)n * fe, (long long)(n + x.T) * fe, (long long)n * fe, s), "up cat a");
+        cuda(launch_copy_frames(ta, x.p, (char*)xc.p + (size_t)n * fe * es, x.B, (long long)x.T * fe, (long long)(n + x.T) * fe, (long long)x.T * fe, s), "up cat b");
+        cuda(launch_copy_frames(ta, (const char*)xc.p + (size_t)(x.T - n) * fe * es, cb->out(), x.B, (long long)(n + x.T) * fe, (long long)n * fe, (long long)n * fe, s), "up cache");
+        commit(cb);
+        cuda(launch_time_interp2x(ta, xc.p, big.p, x.B, n + x.T, (long long)x.H * x.W, x.C, s), "time_interp2x");
       }
       free_act(xc);
       view = big;
@@ -1144,29 +1176,18 @@ static void run_encoder(Exec& ex, const float* x_ext, int B, int T, int H, int W
   if (ex.streaming() && ex.tcm && stem_w && T + t_rep >= 2 && e.conv_in.Ci * 27 <= 128) {
     // chunked v1.1 / streamed v1.0 on the stem kernel: the causal cache (last two padded input frames,
     // model_3dcausal_v1_1.py:230-233) is kept in the caller's layout (fp32 [B,C,2,H,W]) and read by the kernel's patch loader
-    CacheBuf* cb = ex.get_cache("encoder.conv_in#stem", 2, (size_t)B * d.in_channels * 2 * H * W * sizeof(float));
+    CacheBuf* cb = ex.cache("encoder.conv_in#stem", (size_t)B * d.in_channels * 2 * H * W * sizeof(float));
+    if (!cb) return;
     st.x = ex.new_act(B, T + t_rep, H, W, e.conv_in.Co);
     if (ex.ok() && !ex.dry) {
-      if (!ex.ck->first && !cb->valid) { ex.rc = fail(VT_ERR_NOT_READY, "stem cache empty on a non-first chunk"); return; }
-      ConvP p;
-      memset(&p, 0, sizeof(p));
-      p.B = B; p.Ti = T; p.Hi = H; p.Wi = W; p.Ci = d.in_channels;
-      p.isW = 1; p.isH = W; p.isT = (long long)H * W; p.isC = p.isT * T; p.isB = p.isC * p.Ci;
-      p.To = T + t_rep; p.Ho = H; p.Wo = W; p.Co = e.conv_in.Co;
-      p.split = ex.split ? 1 : 0;
+      ConvP p = stem_p(B, d.in_channels, T, H, W, e.conv_in.Co, t_rep, ex.split, e.conv_in.bias);
       p.acc_scale = ex.split ? 1.0f / e.conv_in.wscale3 : 1.0f;
-      p.osC = 1; p.osW = (long long)p.Co * ex.cw; p.osH = (long long)W * p.osW; p.osT = p.osH * H; p.osB = p.osT * p.To;
-      p.kt = p.kh = p.kw = 3; p.st = p.sh = p.sw = 1; p.ut = p.uh = p.uw = 1;
-      p.pt = 2; p.ph = 1; p.pw = 1; p.t_rep = t_rep;
       p.t_mode = ex.ck->first ? (d.version == 1 ? 1 : 0) : 2;   // first chunk: replicate (v1.1) / zero (v1.0) padding
-      p.cache = cb->buf[cb->cur]; p.cacheT = 2;
-      p.bias = e.conv_in.bias;
+      p.cache = cb->in(); p.cacheT = 2;
       if (!conv_stem_supported(p)) { ex.rc = fail(VT_ERR_INVALID, "stem kernel rejected the chunk geometry"); return; }
       ex.cuda(launch_conv_stem(p, x_ext, stem_w, (bf16*)st.x.p, ex.s), "conv_stem");
-      const int nxt = cb->cur ^ 1;
-      ex.cuda(launch_stem_cache_update(x_ext, (float*)cb->buf[nxt], B, d.in_channels, T, t_rep, H, W, ex.s), "stem cache");
-      cb->cur = nxt;
-      cb->valid = true;
+      ex.cuda(launch_stem_cache_update(x_ext, (float*)cb->out(), B, d.in_channels, T, t_rep, H, W, ex.s), "stem cache");
+      ex.commit(cb);
     }
   } else if (d.version == 1 && ex.ck && ex.ck->persist) {
     // chunked v1.1: the causal cache of conv_in holds *padded input* frames; materialise the replicate-padded chunk
@@ -1255,25 +1276,24 @@ static void run_decoder(Exec& ex, const float* z_ext, int B, int Tz, int Hz, int
     if (ex.ok() && ex.streaming()) {
       // streamed v1.0: the cache holds the planes of the last two input frames; later chunks gather over [cache | planes]
       const long long fe = (long long)P.H * P.W * 128;
-      CacheBuf* cb = ex.get_cache("decoder.conv_out#planes", 2, (size_t)P.B * 2 * fe * sizeof(bf16));
-      if (!ex.ok()) return;
+      CacheBuf* cb = ex.cache("decoder.conv_out#planes", (size_t)P.B * 2 * fe * sizeof(bf16));
+      if (!cb) return;
       if (ex.ck->first) {
         if (!ex.dry) {
           ex.cuda(launch_tap_planes_gather((const bf16*)P.p, g.conv_out.bias, x_out, P.B, P.T, P.H, P.W, 128, g.conv_out.Co,
                                            d.time_downsample_factor - 1, ex.s), "tap_planes_gather");
-          ex.tail2(DT_BF16, P.p, nullptr, cb->buf[cb->cur ^ 1], P.B, P.T, fe);
+          ex.tail2(DT_BF16, P.p, nullptr, cb->out(), P.B, P.T, fe);
         }
       } else {
         bf16* Pc = (bf16*)ex.alloc((size_t)P.B * (2 + P.T) * fe * sizeof(bf16));
         if (ex.ok() && !ex.dry) {
-          if (!cb->valid) { ex.rc = fail(VT_ERR_NOT_READY, "decoder head cache empty on a non-first chunk"); return; }
-          ex.cat2(DT_BF16, cb->buf[cb->cur], P.p, Pc, P.B, P.T, fe);
-          ex.tail2(DT_BF16, P.p, cb->buf[cb->cur], cb->buf[cb->cur ^ 1], P.B, P.T, fe);
+          ex.cat2(DT_BF16, cb->in(), P.p, Pc, P.B, P.T, fe);
+          ex.tail2(DT_BF16, P.p, cb->in(), cb->out(), P.B, P.T, fe);
           ex.cuda(launch_tap_planes_gather(Pc, g.conv_out.bias, x_out, P.B, 2 + P.T, P.H, P.W, 128, g.conv_out.Co, 2, ex.s), "tap_planes_gather");
         }
         ex.ar.release(Pc);
       }
-      if (!ex.dry) { cb->cur ^= 1; cb->valid = true; }
+      ex.commit(cb);
     } else if (ex.ok() && !ex.dry) {
       ex.cuda(launch_tap_planes_gather((const bf16*)P.p, g.conv_out.bias, x_out, P.B, P.T, P.H, P.W, 128, g.conv_out.Co,
                                        d.noncausal ? 0 : d.time_downsample_factor - 1, ex.s, d.noncausal ? 1 : 2), "tap_planes_gather");
@@ -1604,19 +1624,28 @@ int32_t vt_decoded_frames(const vt_model* m, int32_t Tz) {
   return t;
 }
 
-static int check_hw(const vt_model* m, int H, int W) {
-  int f = 1;
-  for (int l = 0; l < m->desc.num_levels; ++l)
-    if (contains(m->spatial_ds, l)) f *= 2;
-  if (H % f != 0 || W % f != 0) return fail(VT_ERR_INVALID, "H and W must be multiples of %d", f);
-  return VT_OK;
-}
-
 static int spatial_factor(const vt_model* m) {
   int f = 1;
   for (int l = 0; l < m->desc.num_levels; ++l)
     if (contains(m->spatial_ds, l)) f *= 2;
   return f;
+}
+static int check_hw(const vt_model* m, int H, int W) {
+  const int f = spatial_factor(m);
+  if (H % f != 0 || W % f != 0) return fail(VT_ERR_INVALID, "H and W must be multiples of %d", f);
+  return VT_OK;
+}
+// what every encode entry point checks of its model and input
+static int check_encode_input(const vt_model* m, int C) {
+  if (!m->finalized) return fail(VT_ERR_NOT_READY, "vt_model_finalize has not been called");
+  if (C != m->desc.in_channels) return fail(VT_ERR_INVALID, "input has %d channels, the model expects in_channels = %d", C, m->desc.in_channels);
+  return VT_OK;
+}
+// ... and every decode entry point (token indices have no channel axis)
+static int check_decode_input(const vt_model* m, int Cz, bool from_indices = false) {
+  if (!m->finalized) return fail(VT_ERR_NOT_READY, "vt_model_finalize has not been called");
+  if (!from_indices && Cz != m->desc.z_channels) return fail(VT_ERR_INVALID, "latent has %d channels, the model expects z_channels = %d", Cz, m->desc.z_channels);
+  return VT_OK;
 }
 // v1.0 streams: the whole clip's time padding is replicated tdf-1 frames, then stride-2 resampling, so the first chunk
 // must have 1 (mod tdf) frames and later chunks whole groups of tdf frames
@@ -1665,42 +1694,48 @@ int64_t vt_workspace_bytes(const vt_model* m, int32_t precision, int32_t B, int3
   return (int64_t)(peak + 4096);
 }
 
-int32_t vt_encode(vt_model* m, int32_t precision, const float* x, int32_t B, int32_t C, int32_t T, int32_t H, int32_t W,
-                  const float* noise, float* z, int32_t* indices, float* kl_loss, float* h_pre, void* workspace,
-                  int64_t workspace_bytes, void* stream) {
-  if (!m || !x || !z) return fail(VT_ERR_INVALID, "null argument");
-  if (!m->finalized) return fail(VT_ERR_NOT_READY, "vt_model_finalize has not been called");
-  if (C != m->desc.in_channels) return fail(VT_ERR_INVALID, "input has %d channels, the model expects in_channels = %d", C, m->desc.in_channels);
-  if (B <= 0 || T <= 0) return fail(VT_ERR_INVALID, "bad shape");
-  int rc = check_precision(precision);
-  if (rc) return rc;
-  rc = check_hw(m, H, W);
-  if (rc) return rc;
-  VT_CUDA(cudaSetDevice(m->device));
-  cudaStream_t s = (cudaStream_t)stream;
+// The body of vt_encode and of each chunk: the encoder, then the regularizer (fused into conv_out's epilogue when that runs on
+// the wgmma path).  ex is set up with its stream, workspace and chunk context; h_pre (optional) receives the encoder output
+// before the regularizer, fp32 [B,Cz,Tz,Hz,Wz].
+static int encode(Exec& ex, const float* x, int B, int T, int H, int W, const float* noise, float* z, int32_t* indices,
+                  float* kl_loss, float* h_pre) {
+  vt_model* m = ex.m;
   int Tz, Hz, Wz;
   latent_shape(m, T, H, W, &Tz, &Hz, &Wz);
-  Exec ex(m, stack_prec(precision, false), s, workspace, (size_t)workspace_bytes, false);
-  vt_chunk_state one; one.m = m; one.persist = false; one.first = true;
-  if (m->desc.version == 1) ex.ck = &one;
-  const size_t hb = (size_t)B * (m->desc.double_z ? 2 : 1) * m->desc.z_channels * Tz * Hz * Wz * sizeof(float);
-  float* hp = h_pre ? h_pre : (float*)ex.alloc(hb);
+  float* hp = h_pre ? h_pre : (float*)ex.alloc((size_t)B * (m->desc.double_z ? 2 : 1) * m->desc.z_channels * Tz * Hz * Wz * sizeof(float));
   if (!ex.ok()) return ex.rc;
   TcRegFusion rf;
-  rc = make_reg_fusion(m, noise, z, indices, s, &rf);
+  int rc = make_reg_fusion(m, noise, z, indices, ex.s, &rf);
   if (rc) return rc;
   bool reg_done = false;
   run_encoder(ex, x, B, T, H, W, hp, &rf, h_pre != nullptr, &reg_done);
   if (!ex.ok()) return ex.rc;
-  if (reg_done) return finish_reg_fusion(m, B, kl_loss, s);
-  return regularize(m, hp, noise, B, Tz, Hz, Wz, z, indices, kl_loss, s);
+  if (reg_done) return finish_reg_fusion(m, B, kl_loss, ex.s);
+  return regularize(m, hp, noise, B, Tz, Hz, Wz, z, indices, kl_loss, ex.s);
+}
+
+int32_t vt_encode(vt_model* m, int32_t precision, const float* x, int32_t B, int32_t C, int32_t T, int32_t H, int32_t W,
+                  const float* noise, float* z, int32_t* indices, float* kl_loss, float* h_pre, void* workspace,
+                  int64_t workspace_bytes, void* stream) {
+  if (!m || !x || !z) return fail(VT_ERR_INVALID, "null argument");
+  int rc = check_encode_input(m, C);
+  if (rc) return rc;
+  if (B <= 0 || T <= 0) return fail(VT_ERR_INVALID, "bad shape");
+  rc = check_precision(precision);
+  if (rc) return rc;
+  rc = check_hw(m, H, W);
+  if (rc) return rc;
+  VT_CUDA(cudaSetDevice(m->device));
+  Exec ex(m, stack_prec(precision, false), (cudaStream_t)stream, workspace, (size_t)workspace_bytes, false);
+  vt_chunk_state one; one.m = m; one.persist = false; one.first = true;
+  if (m->desc.version == 1) ex.ck = &one;
+  return encode(ex, x, B, T, H, W, noise, z, indices, kl_loss, h_pre);
 }
 
 int32_t vt_decode(vt_model* m, int32_t precision, const void* z, int32_t from_indices, int32_t B, int32_t Cz, int32_t Tz,
                   int32_t Hz, int32_t Wz, float* x_out, void* workspace, int64_t workspace_bytes, void* stream) {
   if (!m || !z || !x_out) return fail(VT_ERR_INVALID, "null argument");
-  if (!m->finalized) return fail(VT_ERR_NOT_READY, "vt_model_finalize has not been called");
-  if (!from_indices && Cz != m->desc.z_channels) return fail(VT_ERR_INVALID, "latent has %d channels, the model expects z_channels = %d", Cz, m->desc.z_channels);
+  if (int rc = check_decode_input(m, Cz, from_indices != 0)) return rc;
   if (B <= 0 || Tz <= 0 || Hz <= 0 || Wz <= 0) return fail(VT_ERR_INVALID, "bad shape");
   if (check_precision(precision)) return VT_ERR_INVALID;
   VT_CUDA(cudaSetDevice(m->device));
@@ -1775,28 +1810,16 @@ static int encode_chunk(vt_chunk_state* cs, int32_t is_first, const float* x_chu
   if (!cs || !x_chunk || !z) return fail(VT_ERR_INVALID, "null argument");
   if (cs->is_decoder) return fail(VT_ERR_INVALID, "decoder state passed to vt_encode_chunk");
   vt_model* m = cs->m;
-  if (C != m->desc.in_channels) return fail(VT_ERR_INVALID, "input has %d channels, the model expects in_channels = %d", C, m->desc.in_channels);
-  if (!m->finalized) return fail(VT_ERR_NOT_READY, "vt_model_finalize has not been called");
-  VT_CUDA(cudaSetDevice(m->device));
-  cudaStream_t s = (cudaStream_t)stream;
-  if (Tc <= 0) return fail(VT_ERR_INVALID, "bad shape");
-  int rc0 = check_stream_chunk(m, is_first != 0, Tc);
-  if (rc0) return rc0;
-  cs->first = is_first != 0;
-  int Tz, Hz, Wz;
-  latent_shape(m, Tc, cs->H, cs->W, &Tz, &Hz, &Wz);
-  Exec ex(m, stack_prec(cs->prec, false), s, workspace, (size_t)workspace_bytes, false);
-  ex.ck = cs;
-  float* hp = h_out ? h_out : (float*)ex.alloc((size_t)cs->B * (m->desc.double_z ? 2 : 1) * m->desc.z_channels * Tz * Hz * Wz * sizeof(float));
-  if (!ex.ok()) return ex.rc;
-  TcRegFusion rf;
-  int rc = make_reg_fusion(m, noise, z, indices, s, &rf);
+  int rc = check_encode_input(m, C);
   if (rc) return rc;
-  bool reg_done = false;
-  run_encoder(ex, x_chunk, cs->B, Tc, cs->H, cs->W, hp, &rf, h_out != nullptr, &reg_done);
-  if (!ex.ok()) return ex.rc;
-  if (reg_done) return finish_reg_fusion(m, cs->B, kl_loss, s);
-  return regularize(m, hp, noise, cs->B, Tz, Hz, Wz, z, indices, kl_loss, s);
+  VT_CUDA(cudaSetDevice(m->device));
+  if (Tc <= 0) return fail(VT_ERR_INVALID, "bad shape");
+  rc = check_stream_chunk(m, is_first != 0, Tc);
+  if (rc) return rc;
+  cs->first = is_first != 0;
+  Exec ex(m, stack_prec(cs->prec, false), (cudaStream_t)stream, workspace, (size_t)workspace_bytes, false);
+  ex.ck = cs;
+  return encode(ex, x_chunk, cs->B, Tc, cs->H, cs->W, noise, z, indices, kl_loss, h_out);
 }
 int32_t vt_encode_chunk(vt_chunk_state* cs, int32_t is_first, const float* x_chunk, int32_t C, int32_t Tc, const float* noise,
                         float* z, int32_t* indices, float* kl_loss, void* workspace, int64_t workspace_bytes,
@@ -1809,8 +1832,7 @@ int32_t vt_decode_chunk(vt_chunk_state* cs, int32_t is_first, const float* z_chu
   if (!cs || !z_chunk || !x_out) return fail(VT_ERR_INVALID, "null argument");
   if (!cs->is_decoder) return fail(VT_ERR_INVALID, "encoder state passed to vt_decode_chunk");
   vt_model* m = cs->m;
-  if (Cz != m->desc.z_channels) return fail(VT_ERR_INVALID, "latent has %d channels, the model expects z_channels = %d", Cz, m->desc.z_channels);
-  if (!m->finalized) return fail(VT_ERR_NOT_READY, "vt_model_finalize has not been called");
+  if (int rc = check_decode_input(m, Cz)) return rc;
   if (Tzc <= 0) return fail(VT_ERR_INVALID, "bad shape");
   VT_CUDA(cudaSetDevice(m->device));
   cs->first = is_first != 0;
@@ -1949,10 +1971,10 @@ static int encode_video(vt_model* m, int32_t precision, const float* x, int32_t 
                         float* kl_loss, const VideoAux* aux, void* workspace, int64_t workspace_bytes, void* stream) {
   if (!m || !x || !z || !workspace) return fail(VT_ERR_INVALID, "null argument");
   if (m->desc.version != 1) return fail(VT_ERR_INVALID, "temporal tiling exists only in the v1.1 model family");
-  if (!m->finalized) return fail(VT_ERR_NOT_READY, "vt_model_finalize has not been called");
-  if (C != m->desc.in_channels) return fail(VT_ERR_INVALID, "input has %d channels, the model expects in_channels = %d", C, m->desc.in_channels);
+  int rc = check_encode_input(m, C);
+  if (rc) return rc;
   if (B <= 0 || T <= 0 || t_chunk_enc <= 0) return fail(VT_ERR_INVALID, "bad shape");
-  int rc = check_precision(precision);
+  rc = check_precision(precision);
   if (rc) return rc;
   rc = check_hw(m, H, W);
   if (rc) return rc;
@@ -2087,10 +2109,10 @@ int32_t vt_decode_video(vt_model* m, int32_t precision, const float* z, int32_t 
                         int64_t workspace_bytes, void* stream) {
   if (!m || !z || !x_out || !workspace) return fail(VT_ERR_INVALID, "null argument");
   if (m->desc.version != 1) return fail(VT_ERR_INVALID, "temporal tiling exists only in the v1.1 model family");
-  if (!m->finalized) return fail(VT_ERR_NOT_READY, "vt_model_finalize has not been called");
-  if (Cz != m->desc.z_channels) return fail(VT_ERR_INVALID, "latent has %d channels, the model expects z_channels = %d", Cz, m->desc.z_channels);
+  int rc = check_decode_input(m, Cz);
+  if (rc) return rc;
   if (B <= 0 || Tz <= 0 || t_chunk_dec <= 0) return fail(VT_ERR_INVALID, "bad shape");
-  int rc = check_precision(precision);
+  rc = check_precision(precision);
   if (rc) return rc;
   const vt_model_desc& d = m->desc;
   const int tdf = d.time_downsample_factor;
@@ -2173,26 +2195,18 @@ static int op_conv_impl(int precision, int force_simt, const vt_conv_desc* d, co
     return fail(VT_ERR_INVALID, "operator precision must be FMA32, BF16 or EXACT_TC");
   const DType ta = act_type(precision);
   const long long cw = ta == DT_SPLIT ? 2 : 1;
-  ConvP p;
-  memset(&p, 0, sizeof(p));
+  ConvP p = conv_p(d->B, d->Ti, d->Hi, d->Wi, d->Ci);
   p.split = ta == DT_SPLIT ? 1 : 0;
-  p.B = d->B; p.Ti = d->Ti; p.Hi = d->Hi; p.Wi = d->Wi; p.Ci = d->Ci;
-  p.isC = 1; p.isW = cw * d->Ci; p.isH = (long long)d->Wi * p.isW; p.isT = p.isH * d->Hi; p.isB = p.isT * d->Ti;
+  set_in(p, cl_strides(d->Ti, d->Hi, d->Wi, d->Ci, cw));
   p.kt = d->kt; p.kh = d->kh; p.kw = d->kw; p.st = d->st; p.sh = d->sh; p.sw = d->sw;
   p.ut = d->ut; p.uh = d->uh; p.uw = d->uw;
   p.pt = d->pt; p.ph = d->ph0; p.pw = d->pw0;
   p.to_off = e ? e->to_off : 0;
-  p.To = (d->ut * d->Ti + d->pt - d->kt) / d->st + 1 - p.to_off;
-  p.Ho = (d->uh * d->Hi + d->ph0 + d->ph1 - d->kh) / d->sh + 1;
-  p.Wo = (d->uw * d->Wi + d->pw0 + d->pw1 - d->kw) / d->sw + 1;
   p.Co = d->Co;
-  if (p.To <= 0 || p.Ho <= 0 || p.Wo <= 0) return fail(VT_ERR_INVALID, "conv: empty output");
+  if (!conv_out_size(p, 0, d->ph1, d->pw1)) return fail(VT_ERR_INVALID, "conv: empty output");
   const bool out_f32 = e && e->out_f32_ncdhw;
-  if (out_f32) {   // external fp32 [B,Co,To,Ho,Wo] (the heads)
-    p.osC = (long long)p.To * p.Ho * p.Wo; p.osB = p.osC * p.Co; p.osT = (long long)p.Ho * p.Wo; p.osH = p.Wo; p.osW = 1;
-  } else {
-    p.osC = 1; p.osW = cw * p.Co; p.osH = (long long)p.Wo * p.osW; p.osT = p.osH * p.Ho; p.osB = p.osT * p.To;
-  }
+  // out_f32: external fp32 [B,Co,To,Ho,Wo] (the heads)
+  set_out(p, out_f32 ? ncdhw_strides(p.Co, p.To, p.Ho, p.Wo) : cl_strides(p.To, p.Ho, p.Wo, p.Co, cw));
   if (e && e->t_mode) {
     if (e->t_mode == 2 && (!cache || e->cacheT <= 0)) return fail(VT_ERR_INVALID, "t_mode 2 needs a cache of cacheT frames");
     p.t_mode = e->t_mode; p.cache = cache; p.cacheT = e->cacheT;
@@ -2203,11 +2217,13 @@ static int op_conv_impl(int precision, int force_simt, const vt_conv_desc* d, co
   if (d->res_mode && !res) return fail(VT_ERR_INVALID, "residual mode without residual tensor");
   if (d->res_mode == 1 || d->res_mode == 2) {
     const int rT = d->res_mode == 2 ? (p.To + 1) / 2 : p.To;
-    p.rsW = cw * p.Co; p.rsH = (long long)p.Wo * p.rsW; p.rsT = p.rsH * p.Ho; p.rsB = p.rsT * rT; p.resT = rT;
+    set_res(p, cl_strides(rT, p.Ho, p.Wo, p.Co, cw));
+    p.resT = rT;
     const bool mix = d->res_mode == 2 || (e && e->res_mix);
     p.ra = mix ? d->alpha : 1.f; p.rb = mix ? 1.f - d->alpha : 1.f;
   } else if (d->res_mode == 3) {
-    p.rsW = cw * p.Co; p.rsH = (long long)p.Wo * p.rsW; p.rsT = p.rsH * p.Ho; p.rsB = p.rsT * d->Ti; p.resT = d->Ti;
+    set_res(p, cl_strides(d->Ti, p.Ho, p.Wo, p.Co, cw));
+    p.resT = d->Ti;
     p.ra = d->alpha; p.rb = 1.f - d->alpha;
     if (e) { p.res_t_mode = e->res_t_mode; p.res_cache = e->res_t_mode == 2 ? cache : nullptr; }
   } else {
@@ -2320,16 +2336,7 @@ int32_t vt_op_conv_stem(int32_t precision, const float* x, const float* w, const
   if (precision != VT_PREC_BF16 && precision != VT_PREC_EXACT_TC) return fail(VT_ERR_INVALID, "the stem kernel is a wgmma kernel (BF16 / EXACT_TC)");
   cudaStream_t s = (cudaStream_t)stream;
   const bool split = precision == VT_PREC_EXACT_TC;
-  ConvP p;
-  memset(&p, 0, sizeof(p));
-  p.split = split ? 1 : 0;
-  p.B = B; p.Ti = T; p.Hi = H; p.Wi = W; p.Ci = Ci;
-  p.isW = 1; p.isH = W; p.isT = (long long)H * W; p.isC = p.isT * T; p.isB = p.isC * Ci;
-  p.To = T + t_rep; p.Ho = H; p.Wo = W; p.Co = Co;
-  p.osC = 1; p.osW = (long long)Co * (split ? 2 : 1); p.osH = (long long)W * p.osW; p.osT = p.osH * H; p.osB = p.osT * p.To;
-  p.kt = p.kh = p.kw = 3; p.st = p.sh = p.sw = 1; p.ut = p.uh = p.uw = 1;
-  p.pt = 2; p.ph = 1; p.pw = 1; p.t_rep = t_rep;
-  p.bias = bias;
+  ConvP p = stem_p(B, Ci, T, H, W, Co, t_rep, split, bias);
   if (!conv_stem_supported(p)) return fail(VT_ERR_INVALID, "stem kernel does not take this geometry");
   bf16* wpk = nullptr;
   float wsc = 0.f;
@@ -2358,13 +2365,11 @@ int32_t vt_op_head_planes(const void* x, const float* w, const float* bias, floa
   VT_CUDA(cudaMalloc(&wp, (size_t)128 * Ci * sizeof(bf16)));
   VT_CUDA(cudaMalloc(&P, (size_t)B * T * H * W * 128 * sizeof(bf16)));
   VT_CUDA(launch_pack_w_tap_planes(w, wp, Co, Ci, 128, s));
-  ConvP p;
-  memset(&p, 0, sizeof(p));
-  p.B = B; p.Ti = T; p.Hi = H; p.Wi = W; p.Ci = Ci;
-  p.isC = 1; p.isW = Ci; p.isH = (long long)W * Ci; p.isT = p.isH * H; p.isB = p.isT * T;
+  ConvP p = conv_p(B, T, H, W, Ci);
+  set_in(p, cl_strides(T, H, W, Ci, 1));
   p.To = T; p.Ho = H; p.Wo = W; p.Co = 128;
-  p.osC = 1; p.osW = 128; p.osH = (long long)W * 128; p.osT = p.osH * H; p.osB = p.osT * T;
-  p.kt = p.kh = p.kw = 1; p.st = p.sh = p.sw = 1; p.ut = p.uh = p.uw = 1;
+  set_out(p, cl_strides(T, H, W, 128, 1));
+  p.kt = p.kh = p.kw = 1;
   p.ra = 0.f; p.rb = 1.f;
   cudaError_t er = cudaSuccess;
   if (!conv_tc_supported(p, DT_BF16)) er = cudaErrorInvalidValue;
