@@ -52,7 +52,7 @@ def test_non_causal_models_are_rejected():
 
 
 def test_streamed_1080p_exact_workspace_is_bounded():
-    """kl488 at 1080x1920 in exact: the whole 17-frame clip needs ~106 GB of workspace (more than an 80 GB card); a stream of
+    """kl488 at 1080x1920 in exact: the whole 17-frame clip needs ~133 GB of workspace (more than an 80 GB card); a stream of
     4-frame chunks needs a fixed amount, whatever the video's length."""
     from vidtok_b200 import _native as N
     from vidtok_b200.engine import ChunkState

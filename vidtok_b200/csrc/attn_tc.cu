@@ -393,14 +393,13 @@ __global__ void __launch_bounds__(kThreadsAt, 1) attn_tc_kernel(const __grid_con
 
   const char* attn_tc_last_error() { return g_at_err.c_str(); }
 
-  bool attn_tc_supported(long long frames, long long tokens, int C, bool split, bool planning) {
+  bool attn_tc_supported(long long frames, long long tokens, int C, bool split) {
     g_at_err.clear();
     if (frames <= 0 || tokens <= 0) { g_at_err = "empty"; return false; }
     if (C <= 0 || C % 64 != 0 || C > 512) { g_at_err = "C must be a multiple of 64, at most 512"; return false; }
     if (tokens > (1LL << 30)) { g_at_err = "too many tokens per frame"; return false; }
     if (frames * ((tokens + kBM - 1) / kBM) >= (1LL << 31)) { g_at_err = "grid too large"; return false; }
     if (at_stages(C / 64, split) < 2) { g_at_err = "shared memory"; return false; }
-    if (!planning && !tmap_encoder()) { g_at_err = "cuTensorMapEncodeTiled unavailable"; return false; }
     return true;
   }
 
@@ -411,9 +410,9 @@ __global__ void __launch_bounds__(kThreadsAt, 1) attn_tc_kernel(const __grid_con
 
   cudaError_t launch_attn_tc(const bf16* q, const bf16* k, const bf16* v, bf16* o, int frames, int H, int W, int C, bool split,
                              void* ws, cudaStream_t s) {
-    g_at_err.clear();
+    if (!tmap_encoder()) { g_at_err = "cuTensorMapEncodeTiled unavailable"; return cudaErrorNotSupported; }
     const long long tokens = (long long)H * W;
-    if (!attn_tc_supported(frames, tokens, C, split, false)) return cudaErrorInvalidValue;
+    if (!attn_tc_supported(frames, tokens, C, split)) return cudaErrorInvalidValue;
     const int cw = split ? 2 : 1;
     const long long tpad = (tokens + 7) / 8 * 8;
     const int cols = cw * C;

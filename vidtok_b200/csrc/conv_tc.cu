@@ -25,6 +25,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <mutex>
 #include <string>
 #include <type_traits>
 
@@ -758,7 +759,7 @@ __global__ void fill_identity_kernel(bf16* e, int f16, float value) {
 // ---------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------
-bool choose_tile(const ConvP& p, int rows, int& BW, int& BH, int& BT, long long* padded_out = nullptr) {
+bool choose_tile(const ConvP& p, int rows, int& BW, int& BH, int& BT) {
   const bool allow_bt = (p.st == 1) && (p.t_mode == 0);
   long long best = -1;
   auto ceil_to = [](int v, int b) { return (long long)((v + b - 1) / b) * b; };
@@ -771,7 +772,7 @@ bool choose_tile(const ConvP& p, int rows, int& BW, int& BH, int& BT, long long*
       const long long padded = ceil_to(p.Wo, bw) * ceil_to(p.Ho, bh) * ceil_to(p.To, bt);
       // prefer less padding; then square-ish spatial tiles (halo reuse in L2); then BT == 1
       const long long cost = padded * 1024 + (long long)(bw > 16 ? bw - 16 : 16 - bw) * 4 + (bt - 1);
-      if (best < 0 || cost < best) { best = cost; BW = bw; BH = bh; BT = bt; if (padded_out) *padded_out = padded; }
+      if (best < 0 || cost < best) { best = cost; BW = bw; BH = bh; BT = bt; }
     }
   }
   return best >= 0;
@@ -787,18 +788,15 @@ int choose_bn(int Co) {
 
 const char* conv_tc_last_error() { return g_tc_err.c_str(); }
 
-bool conv_tc_can_fuse_ln(const ConvP& p) {
-  return p.Co <= 256 && choose_bn(p.Co) == p.Co && (!p.split || split_ln_fusion_keeps_kparts(p.Co, p.kt * p.kh * p.kw * (p.Ci / 64)));
-}
-
-bool conv_tc_supported(const ConvP& p, DType tout, bool planning) {
+bool conv_tc_plan(const ConvP& p, DType tout, const TcLnFusion* ln, const TcRegFusion* reg, int w_batches, TcPlan* out) {
   g_tc_err.clear();
   auto no = [&](const char* why) { g_tc_err = why; return false; };
   if (p.Ci % 64 != 0) return no("Cin % 64 != 0");
   const int Co_pad = (p.Co + 31) / 32 * 32;
   if (choose_bn(Co_pad) == 0) return no("Cout has no valid N tile");
-  const long long cw = p.split ? 2 : 1;
-  if (p.split ? (tout == DT_BF16) : (tout == DT_SPLIT)) return no("activation layout of input and output differ");
+  const bool split = p.split != 0;
+  const long long cw = split ? 2 : 1;   // bf16 elements per logical channel (hi | lo planes)
+  if (split ? (tout == DT_BF16) : (tout == DT_SPLIT)) return no("activation layout of input and output differ");
   if (p.isC != 1 || p.isW != cw * p.Ci || p.isH != (long long)p.Wi * cw * p.Ci || p.isT != (long long)p.Hi * p.Wi * cw * p.Ci) return no("input is not dense channels-last");
   if (p.isB % 8 != 0) return no("batch stride not 16-byte aligned");
   if (tout != DT_F32) {
@@ -812,27 +810,26 @@ bool conv_tc_supported(const ConvP& p, DType tout, bool planning) {
   if (p.res_mode != 0 && p.res_mode != 1 && p.res_mode != 3) return no("residual mode");
   if (p.res_mode != 0 && tout == DT_F32) return no("residual with fp32 output");
   if (p.t_mode == 2 && p.sh != 1) return no("cache mode with spatial stride");
-  if (!planning && p.t_mode == 2 && (!p.cache || p.cacheT <= 0)) return no("cache mode without cache");
   if (p.Wi > 65535 || p.Hi > 65535) return no("extent");
-  if (!planning && !tmap_encoder()) return no("cuTensorMapEncodeTiled unavailable");
-  return true;
-}
-
-// w_nk: [Co_pad][Kpad] bf16 with Co_pad = roundup(Co, 32) (rows >= Co are zero).
-cudaError_t launch_conv_tc(const ConvP& p, const bf16* x, const bf16* w_nk, int Kpad, void* out, DType tout, cudaStream_t s,
-                           int w_batches, long long w_batch_stride, const TcLnFusion* ln, const TcRegFusion* reg) {
-  if (!tmap_encoder()) { g_tc_err = "cuTensorMapEncodeTiled unavailable"; return cudaErrorNotSupported; }
-  const bool split = p.split != 0;
-  const int cw = split ? 2 : 1;              // bf16 elements per logical channel (hi | lo planes)
-  const bool out_bf16 = tout != DT_F32;      // DT_BF16, or DT_SPLIT (two 16-bit planes)
-  if (split != (tout == DT_SPLIT) && tout != DT_F32) { g_tc_err = "split activations need a split (or fp32) output"; return cudaErrorInvalidValue; }
-  TcParams t;
-  memset(&t, 0, sizeof(t));
-  const int Co_pad = (p.Co + 31) / 32 * 32;
-  int dev = 0;
-  const cudaError_t dev_err = current_device(dev);
-  if (dev_err != cudaSuccess) { g_tc_err = "no current device, or its index is out of range"; return dev_err; }
-  size_t smem = 0;
+  if (w_batches > 1 && w_batches != p.B) return no("batched weights need one weight matrix per batch element");
+  TcPlan t = TcPlan();
+  t.p = p; t.tout = tout; t.w_batches = w_batches;
+  const int nk = p.kt * p.kh * p.kw * (p.Ci / 64);   // K steps
+  // A fused LayerNorm needs one N tile over Cout.  Split mode: N tiles wider than 128 have no registers left for the running
+  // sum of the kparts groups, and from 16 K steps on, where the plan sums in kparts, the tensor core's chained fp32
+  // accumulation alone would exceed fp32-class error (measured 1.2-1.4x the 4e-5 (1 + |ref|) bound at 72-108 K steps, 256
+  // channels), so such a LayerNorm runs as its own kernel after a kparts convolution.
+  if (ln && ln->mode) {
+    if (tout != DT_F32 && p.Co <= 256 && choose_bn(p.Co) == p.Co && (!split || p.Co <= 128 || nk < 16)) t.ln = *ln;
+    else g_tc_err = "fused LayerNorm needs one N tile covering Cout, a 16-bit output and (split) Cout <= 128 or < 16 K steps";
+  }
+  // the regularizer epilogue: the thread that owns a position holds all of its channels (Co_pad == 32: one 32-wide N tile)
+  if (reg && reg->mode) {
+    const int need = reg->mode == 1 ? 2 * reg->zc : reg->zc;
+    const bool zc_ok = reg->mode == 1 ? (reg->zc == 4 || reg->zc == 8 || reg->zc == 16) : reg->zc <= VT_MAX_FSQ;
+    if (tout == DT_F32 && Co_pad == 32 && need <= p.Co && zc_ok && p.osW == 1) t.reg = *reg;
+    else g_tc_err = "regularizer epilogue needs an fp32 [B,C,T,H,W] head with Cout <= 32 holding all latent channels";
+  }
   // Tile geometry + shared-memory plan.  Split operands double every operand tile: when the halo windows leave fewer
   // than 2 pipeline stages, fall back to one A box per tap.
   auto plan = [&](bool allow_halo, int bn_cap) -> int {
@@ -850,45 +847,70 @@ cudaError_t launch_conv_tc(const ConvP& p, const bf16* x, const bf16* w_nk, int 
       t.halo_bytes = (uint32_t)((16 + p.kh - 1) * t.hP * 128);
       t.a_stages = 2;
     }
-    t.tilesW = (p.Wo + t.BW - 1) / t.BW; t.tilesH = (p.Ho + t.BH - 1) / t.BH; t.tilesT = (p.To + t.BT - 1) / t.BT;
-    t.num_n_tiles = Co_pad / t.BN;
-    t.num_tiles = (long long)p.B * t.tilesT * t.tilesH * t.tilesW * t.num_n_tiles;
     const size_t stage_bytes = (size_t)cw * ((t.halo ? 0 : (size_t)kABytes) + (size_t)t.BN * 128);
     const size_t budget = 225 * 1024;
     const size_t a_ring = (size_t)t.a_stages * t.halo_bytes * cw;
     // two bias / gamma / beta buffers per consumer group (ping-pong: one group per warpgroup), regularizer rows
-    const size_t misc = (ping_pong(t.BN, split) ? 4 : 2) * 768 * 4 + ((reg && reg->mode) ? 128 * 33 * 4 : 0);
+    const size_t misc = (ping_pong(t.BN, split) ? 4 : 2) * 768 * 4 + (t.reg.mode ? 128 * 33 * 4 : 0);
     const size_t fixed = 1024 /*align*/ + misc + 16;
     if (budget < fixed + a_ring + 2 * (stage_bytes + 16)) return 1;
     int stages = (int)((budget - fixed - a_ring) / (stage_bytes + 16));
     if (stages > 8) stages = 8;
-    {
-      static int cap = -1;   // VT_TC_STAGES caps the pipeline depth: lets the tests run the shortest (2-stage) ring
-      if (cap < 0) { const char* e = getenv("VT_TC_STAGES"); cap = e ? atoi(e) : 0; }
-      if (cap >= 2 && stages > cap) stages = cap;
-    }
+    // VT_TC_STAGES caps the pipeline depth: lets the tests run the shortest (2-stage) ring
+    static const int cap = [] { const char* e = getenv("VT_TC_STAGES"); return e ? atoi(e) : 0; }();
+    if (cap >= 2 && stages > cap) stages = cap;
     t.stages = stages;
     // smem layout from the 1024-aligned base: [halo windows] [stages x (A | B)] [barriers] [bias/gamma/beta | regularizer rows]
     const size_t bars = 8 * (2 * (size_t)stages + 2 * (size_t)t.a_stages);
     t.misc_off = (uint32_t)((a_ring + stages * stage_bytes + bars + 15) & ~(size_t)15);
-    smem = 1024 + t.misc_off + misc;
+    t.smem = 1024 + t.misc_off + misc;
     // split + long K: the K steps of a tile are summed in groups (TcParams::kparts; needs BN <= 128)
-    t.kparts = 1;
-    const int nk_ = p.kt * p.kh * p.kw * (p.Ci / 64);
-    if (split && t.BN <= 128 && nk_ >= 16) t.kparts = nk_ >= 64 ? 8 : 4;
+    t.kparts = (split && t.BN <= 128 && nk >= 16) ? (nk >= 64 ? 8 : 4) : 1;
     return 0;
   };
-  {
-    // split + long K without a fused LayerNorm: narrow N tiles leave registers for the running sum (TcParams::kparts)
-    const bool need_row = ln && ln->mode;
-    const int nk = p.kt * p.kh * p.kw * (p.Ci / 64);
-    const int bn_pref = (split && !need_row && w_batches <= 1) ? (nk >= 128 ? 64 : (nk >= 16 ? 128 : 0)) : 0;
-    int rc = plan(true, bn_pref);
-    if (rc == 1) rc = plan(false, bn_pref);
-    if (rc == 1 && !need_row) rc = plan(false, 128);
-    if (rc == 1) g_tc_err = "not enough shared memory for 2 stages";
-    if (rc != 0) return cudaErrorInvalidValue;
+  // split + long K without a fused LayerNorm: narrow N tiles leave registers for the running sum (TcParams::kparts)
+  const bool need_row = t.ln.mode != 0;
+  const int bn_pref = (split && !need_row && w_batches <= 1) ? (nk >= 128 ? 64 : (nk >= 16 ? 128 : 0)) : 0;
+  int rc = plan(true, bn_pref);
+  if (rc == 1) rc = plan(false, bn_pref);
+  if (rc == 1 && !need_row) rc = plan(false, 128);
+  if (rc == 1) return no("not enough shared memory for 2 stages");
+  if (rc != 0) return false;
+  // (split mode: the weights carry a power-of-two scale 2^s that the epilogue removes from the whole accumulator, so the
+  // residual is multiplied by 2^s * I -- exact in fp16 for s <= 15; larger scales fall back to the epilogue add)
+  bool ident_ok = true;
+  if (split) {
+    const float ws = p.acc_scale != 0.f ? 1.0f / p.acc_scale : 1.0f;
+    t.ident_s = ilogbf(ws);
+    ident_ok = t.ident_s >= 0 && t.ident_s <= 15 && ldexpf(1.0f, t.ident_s) == ws;
   }
+  t.res_mma = (ident_ok && p.res_mode == 1 && p.ra == 1.0f && p.rb == 1.0f && t.BN % 64 == 0 && p.Co % 64 == 0 && p.rsW % 8 == 0 &&
+               p.rsH % 8 == 0 && p.rsT % 8 == 0 && p.rsB % 8 == 0 && (((uintptr_t)p.res) & 15) == 0) ? 1 : 0;
+  *out = t;
+  return true;
+}
+
+// (Co_pad = roundup(Co, 32): weight rows >= Co are zero)
+cudaError_t launch_conv_tc(const TcPlan& pl, const bf16* x, const bf16* w_nk, void* out, cudaStream_t s, long long w_batch_stride) {
+  if (!tmap_encoder()) { g_tc_err = "cuTensorMapEncodeTiled unavailable"; return cudaErrorNotSupported; }
+  const ConvP& p = pl.p;
+  const TcRegFusion& reg = pl.reg;
+  const bool split = p.split != 0;
+  const int cw = split ? 2 : 1;
+  if (reg.mode ? (!reg.z || (reg.mode == 1 && (!reg.kl_acc || (reg.sample && !reg.noise)))) : !out) { g_tc_err = "null output"; return cudaErrorInvalidValue; }
+  if (p.t_mode == 2 && (!p.cache || p.cacheT <= 0)) { g_tc_err = "cache mode without cache"; return cudaErrorInvalidValue; }
+  int dev = 0;
+  const cudaError_t dev_err = current_device(dev);
+  if (dev_err != cudaSuccess) { g_tc_err = "no current device, or its index is out of range"; return dev_err; }
+  const int Co_pad = (p.Co + 31) / 32 * 32, Kpad = p.kt * p.kh * p.kw * p.Ci;
+  TcParams t;
+  memset(&t, 0, sizeof(t));
+  t.BW = pl.BW; t.BH = pl.BH; t.BT = pl.BT; t.BN = pl.BN;
+  t.halo = pl.halo; t.hP = pl.hP; t.a_stages = pl.a_stages; t.halo_bytes = pl.halo_bytes;
+  t.stages = pl.stages; t.misc_off = pl.misc_off; t.kparts = pl.kparts; t.res_mma = pl.res_mma;
+  t.tilesW = (p.Wo + t.BW - 1) / t.BW; t.tilesH = (p.Ho + t.BH - 1) / t.BH; t.tilesT = (p.To + t.BT - 1) / t.BT;
+  t.num_n_tiles = Co_pad / t.BN;
+  t.num_tiles = (long long)p.B * t.tilesT * t.tilesH * t.tilesW * t.num_n_tiles;
   t.split = split ? 1 : 0; t.a_lo = p.Ci; t.b_lo = Kpad; t.o_lo = p.Co;
   t.acc_scale = (split && p.acc_scale != 0.f) ? p.acc_scale : 1.0f;
   t.B = p.B; t.To = p.To; t.Ho = p.Ho; t.Wo = p.Wo; t.Co = p.Co; t.Ti = p.Ti;
@@ -899,39 +921,15 @@ cudaError_t launch_conv_tc(const ConvP& p, const bf16* x, const bf16* w_nk, int 
   t.rsB = p.rsB; t.rsT = p.rsT; t.rsH = p.rsH; t.rsW = p.rsW; t.resT = p.resT; t.res_t_mode = p.res_t_mode; t.res_pool_off = p.res_pool_off;
   t.res_cache = (const bf16*)p.res_cache; t.ra = p.ra; t.rb = p.rb;
   t.out = out; t.osB = p.osB; t.osT = p.osT; t.osH = p.osH; t.osW = p.osW; t.osC = p.osC;
-  t.out_f32 = (tout == DT_F32) ? 1 : 0;
+  t.out_f32 = (pl.tout == DT_F32) ? 1 : 0;
   t.Co_real = p.Co;
-  if (ln && ln->mode) {
-    if (t.BN != p.Co || !out_bf16) { g_tc_err = "fused LayerNorm needs one N tile covering Cout and bf16 output"; return cudaErrorInvalidValue; }
-    t.ln_mode = ln->mode; t.ln_silu = ln->silu ? 1 : 0; t.ln_gamma = ln->gamma; t.ln_beta = ln->beta; t.out2 = ln->out2;
+  t.ln_mode = pl.ln.mode; t.ln_silu = pl.ln.silu ? 1 : 0; t.ln_gamma = pl.ln.gamma; t.ln_beta = pl.ln.beta; t.out2 = pl.ln.out2;
+  if (reg.mode) {
+    t.reg_mode = reg.mode; t.reg_zc = reg.zc; t.reg_sample = reg.sample; t.reg_noise = reg.noise; t.reg_z = reg.z;
+    t.reg_idx = reg.indices; t.reg_kl = reg.kl_acc;
+    if (reg.mode == 2) t.reg_fsq = make_fsq_const(reg.zc, reg.fsq_levels);
   }
-  if (reg && reg->mode) {
-    const int need = reg->mode == 1 ? 2 * reg->zc : reg->zc;
-    if (tout != DT_F32 || Co_pad != 32 || t.BN != 32 || need > p.Co || (reg->mode == 1 ? (reg->zc != 4 && reg->zc != 8 && reg->zc != 16) : reg->zc > VT_MAX_FSQ) || !reg->z ||
-        (reg->mode == 1 && (!reg->kl_acc || (reg->sample && !reg->noise))) || p.osW != 1) {
-      g_tc_err = "regularizer epilogue needs an fp32 [B,C,T,H,W] head with Cout <= 32 holding all latent channels";
-      return cudaErrorInvalidValue;
-    }
-    t.reg_mode = reg->mode; t.reg_zc = reg->zc; t.reg_sample = reg->sample; t.reg_noise = reg->noise; t.reg_z = reg->z;
-    t.reg_idx = reg->indices; t.reg_kl = reg->kl_acc;
-    if (reg->mode == 2) t.reg_fsq = make_fsq_const(reg->zc, reg->fsq_levels);
-  } else if (!out) {
-    g_tc_err = "null output";
-    return cudaErrorInvalidValue;
-  }
-  t.w_batched = w_batches > 1 ? 1 : 0;
-  if (t.w_batched && w_batches != p.B) { g_tc_err = "batched weights need one weight matrix per batch element"; return cudaErrorInvalidValue; }
-  // (split mode: the weights carry a power-of-two scale 2^s that the epilogue removes from the whole accumulator, so the
-  // residual is multiplied by 2^s * I -- exact in fp16 for s <= 15; larger scales fall back to the epilogue add)
-  int ident_s = 0;
-  bool ident_ok = true;
-  if (split) {
-    const float ws = 1.0f / t.acc_scale;
-    ident_s = ilogbf(ws);
-    ident_ok = ident_s >= 0 && ident_s <= 15 && ldexpf(1.0f, ident_s) == ws;
-  }
-  t.res_mma = (ident_ok && p.res_mode == 1 && p.ra == 1.0f && p.rb == 1.0f && t.BN % 64 == 0 && p.Co % 64 == 0 && p.rsW % 8 == 0 && p.rsH % 8 == 0 &&
-               p.rsT % 8 == 0 && p.rsB % 8 == 0 && (((uintptr_t)p.res) & 15) == 0) ? 1 : 0;
+  t.w_batched = pl.w_batches > 1 ? 1 : 0;
 
   TcMaps maps;
   // activation view: element (c, w, h, t, b) at base + c + w*sw_ + h*sh_ + t*isT + b*bs  (elements)
@@ -954,13 +952,12 @@ cudaError_t launch_conv_tc(const ConvP& p, const bf16* x, const bf16* w_nk, int 
           return cudaErrorInvalidValue;
   }
   if (p.t_mode == 2) {
-    if (p.sh != 1) { g_tc_err = "cache mode with spatial stride"; return cudaErrorInvalidValue; }
     if (!encode_act(&maps.c, (const bf16*)p.cache, p.Wi, p.Hi, p.isW, p.isH, p.cacheT, p.isT, (long long)p.cacheT * p.Hi * p.Wi * p.Ci * cw)) return cudaErrorInvalidValue;
   } else {
     maps.c = maps.a[0];
   }
   {
-    const int nb = w_batches > 1 ? w_batches : 1;
+    const int nb = pl.w_batches > 1 ? pl.w_batches : 1;
     // split weights: [Co_pad][hi(Kpad) | lo(Kpad)]
     cuuint64_t dims[3] = {(cuuint64_t)(cw * Kpad), (cuuint64_t)Co_pad, (cuuint64_t)nb};
     cuuint64_t strides[2] = {(cuuint64_t)(cw * Kpad) * 2, (cuuint64_t)(nb > 1 ? w_batch_stride : (long long)cw * Kpad * Co_pad) * 2};
@@ -976,16 +973,24 @@ cudaError_t launch_conv_tc(const ConvP& p, const bf16* x, const bf16* w_nk, int 
   };
   maps.r = maps.a[0]; maps.e = maps.b;
   if (t.res_mma) {
-    // 256 x 256 identity: bf16 I, or the 16 fp16 matrices 2^s * I of the split mode; built once per device on the launching stream
+    // 256 x 256 identity: bf16 I, or the 16 fp16 matrices 2^s * I of the split mode; built once per device, and filled
+    // before any launch can read it
     static bf16* ident_dev[2][kMaxDevices] = {{nullptr}};
+    static std::mutex ident_mu;
     const int ik = split ? 1 : 0;
-    if (!ident_dev[ik][dev]) {
-      const int nmat = split ? 16 : 1;
-      cudaError_t e = cudaMalloc(&ident_dev[ik][dev], (size_t)nmat * 256 * 256 * sizeof(bf16));
-      if (e != cudaSuccess) { g_tc_err = "cudaMalloc(identity)"; return e; }
-      for (int i = 0; i < nmat; ++i) fill_identity_kernel<<<256, 256, 0, s>>>(ident_dev[ik][dev] + (size_t)i * 256 * 256, ik, ldexpf(1.0f, i));
+    {
+      std::lock_guard<std::mutex> lock(ident_mu);
+      if (!ident_dev[ik][dev]) {
+        const int nmat = split ? 16 : 1;
+        bf16* e = nullptr;
+        cudaError_t err = cudaMalloc(&e, (size_t)nmat * 256 * 256 * sizeof(bf16));
+        if (err != cudaSuccess) { g_tc_err = "cudaMalloc(identity)"; return err; }
+        for (int i = 0; i < nmat; ++i) fill_identity_kernel<<<256, 256, 0, s>>>(e + (size_t)i * 256 * 256, ik, ldexpf(1.0f, i));
+        if ((err = cudaStreamSynchronize(s)) != cudaSuccess) { cudaFree(e); g_tc_err = "identity fill"; return err; }
+        ident_dev[ik][dev] = e;
+      }
     }
-    bf16* ident = ident_dev[ik][dev] + (size_t)(split ? ident_s : 0) * 256 * 256;
+    const bf16* ident = ident_dev[ik][dev] + (size_t)pl.ident_s * 256 * 256;
     if (!encode_out(&maps.r, p.res, p.resT, p.rsW, p.rsH, p.rsT, p.rsB, t.halo ? t.hP : t.BW, t.halo ? 16 + p.kh - 1 : t.BH, t.BT)) return cudaErrorInvalidValue;
     cuuint64_t dims[3] = {256, 256, 1};
     cuuint64_t strides[2] = {512, 256 * 512};
@@ -1007,8 +1012,8 @@ cudaError_t launch_conv_tc(const ConvP& p, const bf16* x, const bf16* w_nk, int 
   char det[160] = "";
   if (prof_enabled()) snprintf(det, sizeof(det), "k%d%d%d s%d%d %d->%d @%dx%dx%d tile%dx%dx%d bn%d%s ln%d r%d%s p%d t%d st%d", p.kt, p.kh, p.kw, p.st, p.sh, p.Ci, p.Co, p.To, p.Ho, p.Wo, t.BT, t.BH, t.BW, t.BN, t.halo ? " halo" : "", t.ln_mode, p.res_mode, t.res_mma ? "m" : "", split ? t.kparts : 1, p.t_mode, t.stages);
   ProfScope _ps(split ? "conv_tc3" : "conv_tc", 2.0 * Mrows * p.kt * p.kh * p.kw * p.Ci * p.Co,
-                2.0 * cw * ((double)p.B * p.Ti * p.Hi * p.Wi * p.Ci) + Mrows * p.Co * (tout == DT_F32 ? 4.0 : 2.0 * cw), s, det);
-  auto launch = [&](auto kern) { kern<<<grid, kThreads, smem, s>>>(maps, t); };
+                2.0 * cw * ((double)p.B * p.Ti * p.Hi * p.Wi * p.Ci) + Mrows * p.Co * (pl.tout == DT_F32 ? 4.0 : 2.0 * cw), s, det);
+  auto launch = [&](auto kern) { kern<<<grid, kThreads, pl.smem, s>>>(maps, t); };
   switch (t.BN * 2 + (split ? 1 : 0)) {
     case 64: launch(conv_tc_kernel<32, false>); break;
     case 65: launch(conv_tc_kernel<32, true>); break;

@@ -135,18 +135,23 @@ struct TcRegFusion {
   double* kl_acc = nullptr;      // KL: sum over all elements of mean^2 + var - 1 - logvar (cleared by the caller)
   int fsq_levels[VT_MAX_FSQ] = {0};
 };
-bool conv_tc_can_fuse_ln(const ConvP& p);
-// Split mode: a fused LayerNorm needs one N tile over Cout, and N tiles wider than 128 have no registers left for the
-// running sum of the kparts groups.  From 16 K steps on, where the plan sums in kparts, the tensor core's chained fp32
-// accumulation alone would exceed fp32-class error (measured 1.2-1.4x the 4e-5 (1 + |ref|) bound at 72-108 K steps,
-// 256 channels), so such a LayerNorm runs as its own kernel after a kparts convolution.
-inline bool split_ln_fusion_keeps_kparts(int Co, int k_steps) { return Co <= 128 || k_steps < 16; }
-// planning = true: geometry-only answer (workspace dry runs: no device pointers, possibly no driver)
-bool conv_tc_supported(const ConvP& p, DType tout, bool planning = false);
-// out may be null when a regularizer epilogue consumes the result (reg != nullptr)
-cudaError_t launch_conv_tc(const ConvP& p, const bf16* x, const bf16* w_nk, int Kpad, void* out, DType tout, cudaStream_t s,
-                           int w_batches = 1, long long w_batch_stride = 0, const TcLnFusion* ln = nullptr,
-                           const TcRegFusion* reg = nullptr);
+// One conv_tc launch as conv_tc_plan decides it (the tile fields are those of conv_tc.cu's TcParams)
+struct TcPlan {
+  ConvP p;
+  DType tout;
+  int w_batches, BN, BW, BH, BT, halo, hP, a_stages, stages, kparts, res_mma, ident_s;
+  uint32_t halo_bytes, misc_off;
+  size_t smem;
+  TcLnFusion ln;                 // the requested epilogues that are taken (mode 0 otherwise)
+  TcRegFusion reg;
+};
+// The wgmma plan of p with output type tout from geometry alone: no driver or runtime call, so a workspace dry run plans
+// what the launch runs.  ln / reg request fused epilogues; one that does not fit is left out (mode 0) with the reason in
+// conv_tc_last_error().  False, with the reason there, when conv_tc cannot run p.
+bool conv_tc_plan(const ConvP& p, DType tout, const TcLnFusion* ln, const TcRegFusion* reg, int w_batches, TcPlan* out);
+// w_nk: [Co_pad][K = taps * Cin] bf16 weights, w_batch_stride apart when batched; out may be null when a regularizer
+// epilogue consumes the result.  A driver without cuTensorMapEncodeTiled is a launch error.
+cudaError_t launch_conv_tc(const TcPlan& pl, const bf16* x, const bf16* w_nk, void* out, cudaStream_t s, long long w_batch_stride = 0);
 cudaError_t launch_kl_clear(double* scratch, cudaStream_t s);
 cudaError_t launch_kl_finish(const double* scratch, int B, float* kl_loss, cudaStream_t s);
 // decoder head through per-tap partial outputs (see elementwise.cu)
@@ -158,7 +163,7 @@ cudaError_t launch_transpose_bf16(const bf16* x, bf16* y, int batch, int rows, i
 const char* conv_tc_last_error();
 
 // tblock_tc.cu: ResnetCausalBlock1D (k311 conv -> LayerNorm -> SiLU -> k311 conv + residual) for C = 128, v1.0 padding
-bool tblock_tc_supported(int B, int T, int H, int W, int C, bool planning = false);
+bool tblock_tc_supported(int B, int T, int H, int W, int C);
 // Causal caches of a streamed video, bf16 [B,2,H,W,128] each: n1 = the block's input frames t-2, t-1, h = its LN2(h) frames
 // (conv2's input).  *_in null: the first chunk (zero padding in front); *_out receive the chunk's last two frames and must
 // not alias the inputs.
@@ -177,7 +182,7 @@ const char* tblock_tc_last_error();
 // attn_tc.cu: fused per-frame attention O = softmax(Q K^T / sqrt(C)) V on wgmma with an online softmax (no tokens x tokens
 // buffer).  q, k, v, o channels-last [frames, H*W, C] in bf16 or hi|lo split rows; C % 64 == 0, C <= 512, any token count.
 // ws: attn_tc_workspace bytes (V^T, the size of v).
-bool attn_tc_supported(long long frames, long long tokens, int C, bool split, bool planning = false);
+bool attn_tc_supported(long long frames, long long tokens, int C, bool split);
 size_t attn_tc_workspace(long long frames, long long tokens, int C, bool split);
 cudaError_t launch_attn_tc(const bf16* q, const bf16* k, const bf16* v, bf16* o, int frames, int H, int W, int C, bool split,
                            void* ws, cudaStream_t s);

@@ -161,6 +161,36 @@ static void add_attn(vt_model* m, AttnW& a, const std::string& key, int C) {
 }
 static bool contains(const std::vector<int>& v, int x) { return std::find(v.begin(), v.end(), x) != v.end(); }
 
+// The kt x kh x kw phase conv of "nearest 2x upsample, then c" (one per output parity class)
+static void phase_conv(ConvW& ph, const ConvW& c, int kt, int kh, int kw) {
+  ph.Co = c.Co; ph.Ci = c.Ci; ph.kt = kt; ph.kh = kh; ph.kw = kw; ph.Co_pad = c.Co; ph.Kpad = kt * kh * kw * c.Ci;
+}
+// Everything the launch plans depend on is fixed with the model's geometry, so that a workspace dry run plans the same
+// kernels before and after vt_model_finalize: the wgmma weight rows, the phase-collapsed upsampling convs (decoder
+// Upsample / v1.0 TimeUpsampleResCausal2x), the stem kernel and the decoder head's tap planes.
+static void plan_geometry(vt_model* m) {
+  for (ConvW* c : m->convs) {
+    c->Co_pad = (c->Co + 31) / 32 * 32;
+    c->Kpad = c->Ci % 64 == 0 ? c->taps() * c->Ci : 0;
+  }
+  for (auto& lv : m->dec.levels) {
+    lv.has_up_phase = lv.has_resample && lv.resample.Ci % 64 == 0 && lv.resample.Co % 32 == 0;
+    lv.has_tup_phase = lv.has_tres && m->desc.version == 0 && lv.tconv.Ci % 64 == 0 && lv.tconv.Co % 32 == 0;
+    if (lv.has_up_phase)
+      for (ConvW& ph : lv.up_ph) phase_conv(ph, lv.resample, 1, 2, 2);
+    if (lv.has_tup_phase)
+      for (ConvW& ph : lv.tup_ph) phase_conv(ph, lv.tconv, 2, 3, 3);
+  }
+  ConvW& c = m->enc.conv_in;
+  c.stem = c.Ci * 27 <= 128 && c.Co % 64 == 0 && c.Co <= 256 && c.kt == 3 && c.kh == 3 && c.kw == 3;
+  // decoder head as tap planes (v1.0 only: zero causal padding, no chunk caches): a 1x1x1 conv Cin -> 128
+  const ConvW& h = m->dec.conv_out;
+  if (m->desc.version == 0 && h.kt == 3 && h.kh == 3 && h.kw == 3 && h.Co <= 4 && h.Ci % 64 == 0) {
+    ConvW& hp = m->head_planes;
+    hp.Co = 128; hp.Ci = h.Ci; hp.Co_pad = 128; hp.Kpad = h.Ci;
+  }
+}
+
 static void build_manifest(vt_model* m) {
   const vt_model_desc& d = m->desc;
   const int L = d.num_levels;
@@ -242,6 +272,7 @@ static void build_manifest(vt_model* m) {
   }
   add_norm(m, g.norm_out, "decoder.norm_out", block_in);
   add_conv3d(m, g.conv_out, "decoder.conv_out", d.out_ch, block_in, 3);
+  plan_geometry(m);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -559,12 +590,11 @@ struct Exec {
   }
 
   // ---- convolution ----------------------------------------------------------------------------
-  Act conv(const ConvW& w, const Act& in, const ConvOpt& o) {
-    Act out;
-    if (!ok()) return out;
+  // The descriptor conv(w, in, o) launches, but for the chunk-cache pointers: extents, strides, padding, time mode, residual.
+  bool conv_desc(const ConvW& w, const Act& in, const ConvOpt& o, ConvP& p) {
     const bool v11 = m->desc.version == 1;
-    ConvP p = conv_p(in.B, in.T, in.H, in.W, in.C);
-    if (in.C != w.Ci) { rc = fail(VT_ERR_INVALID, "conv: Cin mismatch %d vs %d", in.C, w.Ci); return out; }
+    p = conv_p(in.B, in.T, in.H, in.W, in.C);
+    if (in.C != w.Ci) { rc = fail(VT_ERR_INVALID, "conv: Cin mismatch %d vs %d", in.C, w.Ci); return false; }
     if (o.ext_in && o.ext_in_indices) {
       Strides is = ncdhw_strides(1, in.T, in.H, in.W);   // the int32 token tensor [B,T,H,W]: no channel axis
       is.C = 0;
@@ -596,89 +626,88 @@ struct Exec {
     const int pw0 = o.pw0 >= 0 ? o.pw0 : wp / 2, pw1 = o.pw1 >= 0 ? o.pw1 : wp - wp / 2;
     p.ph = ph0; p.pw = pw0;
     p.Co = w.Co;
-    if (!conv_out_size(p, ptb, ph1, pw1)) { rc = fail(VT_ERR_INVALID, "conv: empty output"); return out; }
-    out.B = in.B; out.T = p.To; out.H = p.Ho; out.W = p.Wo; out.C = w.Co;
-    if (o.ext_out) {
-      out.p = o.ext_out;
-      set_out(p, ncdhw_strides(p.Co, p.To, p.Ho, p.Wo));
-    } else if (o.out_view) {
-      out.p = o.out_view;
-      set_out(p, Strides{o.ov_sB, o.ov_sT, o.ov_sH, o.ov_sW, 1});
-    } else {
-      out.p = alloc((size_t)out.elems() * dtype_size(ta));
-      out.owned = true;
-      set_out(p, cl_strides(p.To, p.Ho, p.Wo, p.Co, cw));
+    if (!conv_out_size(p, ptb, ph1, pw1)) { rc = fail(VT_ERR_INVALID, "conv: empty output"); return false; }
+    if (o.ext_out) set_out(p, ncdhw_strides(p.Co, p.To, p.Ho, p.Wo));
+    else if (o.out_view) set_out(p, Strides{o.ov_sB, o.ov_sT, o.ov_sH, o.ov_sW, 1});
+    else set_out(p, cl_strides(p.To, p.Ho, p.Wo, p.Co, cw));
+    // time padding mode: zeros, replicate (v1.1), or the chunk cache on a later chunk of a stream
+    const bool cached = streaming() && o.cache_key && !ck->first;
+    if (v11 && w.kt > 1) p.t_mode = 1;
+    if (w.kt > 1 && cached) { p.t_mode = 2; p.cacheT = p.pt; }   // (folded 2x time upsampling: frames of the upsampled axis)
+    p.bias = w.bias;
+    p.res_mode = o.res_mode;
+    p.ra = o.ra; p.rb = o.rb;
+    if (o.res_mode) {
+      const Act& r = *o.res;
+      if (r.C != w.Co) { rc = fail(VT_ERR_INVALID, "conv: residual channel mismatch"); return false; }
+      p.res = r.p;
+      set_res(p, cl_strides(r.T, r.H, r.W, r.C, cw, o.res_bs));
+      p.resT = r.T;
+      if (o.res_mode == 3) {
+        p.res_pool_off = o.res_pool_off;
+        p.res_t_mode = cached ? 2 : (v11 ? 1 : 0);   // v1.1: replicate (model_3dcausal_v1_1.py:293-294)
+      }
     }
+    return true;
+  }
+  // The wgmma plan of conv(w, in, o) for its descriptor p, with the epilogues o requests; false: the conv does not run on conv_tc.
+  bool tc_plan(const ConvW& w, const ConvP& p, const ConvOpt& o, TcPlan* pl) const {
+    if (!tcm || o.force_simt || o.ext_in || !w.Kpad) return false;
+    TcLnFusion lf;
+    const NormW* ln = o.ln1 ? o.ln1 : o.ln2;
+    if (ln && m->desc.norm_type == VT_NORM_LAYERNORM) {
+      lf.mode = o.ln1 ? 1 : 2; lf.silu = o.ln1 ? o.ln1_silu : o.ln2_silu; lf.gamma = ln->gamma; lf.beta = ln->beta; lf.out2 = o.ln2_view;
+    }
+    return conv_tc_plan(p, o.ext_out ? DT_F32 : ta, &lf, o.reg, 1, pl);
+  }
+  // whether conv(w, in, o) would fuse LayerNorm ln (the next stage's norm) into its epilogue
+  bool fuses_ln(const ConvW& w, const Act& in, ConvOpt o, const NormW* ln, bool silu) {
+    o.ln2 = ln; o.ln2_silu = silu;
+    ConvP p;
+    TcPlan pl;
+    return ln && conv_desc(w, in, o, p) && tc_plan(w, p, o, &pl) && pl.ln.mode != 0;
+  }
+  Act conv(const ConvW& w, const Act& in, const ConvOpt& o) {
+    Act out;
+    ConvP p;
+    if (!ok() || !conv_desc(w, in, o, p)) return out;
+    out.B = in.B; out.T = p.To; out.H = p.Ho; out.W = p.Wo; out.C = w.Co;
+    out.p = o.ext_out ? (void*)o.ext_out : o.out_view;
+    if (!out.p) { out.p = alloc((size_t)out.elems() * dtype_size(ta)); out.owned = true; }
     if (!ok()) return out;
-    // time padding mode
-    p.t_mode = 0;
     CacheBuf* cb = nullptr;
     int cache_off = 0;
-    if (v11 && w.kt > 1) p.t_mode = 1;
     if (w.kt > 1 && streaming() && o.cache_key) {
       cache_off = cache_offset_for(o.cache_key);
       cb = cache(o.cache_key, (size_t)in.B * p.pt * in.frame() * dtype_size(o.ext_in ? DT_F32 : ta));
       if (!cb) return out;
-      if (!ck->first) {
-        p.t_mode = 2;
-        p.cache = cb->in();
-        p.cacheT = p.pt;   // (folded 2x time upsampling: frames of the upsampled axis)
-      }
+      if (p.t_mode == 2) p.cache = cb->in();
     }
-    p.bias = w.bias;
-    p.res_mode = o.res_mode;
-    p.ra = o.ra; p.rb = o.rb;
     CacheBuf* pc = nullptr;   // avg-pool branch of res_mode 3
-    if (o.res_mode) {
+    if (o.res_mode == 3 && streaming() && o.cache_key) {
       const Act& r = *o.res;
-      p.res = r.p;
-      set_res(p, cl_strides(r.T, r.H, r.W, r.C, cw, o.res_bs));
-      p.resT = r.T;
-      if (r.C != w.Co) { rc = fail(VT_ERR_INVALID, "conv: residual channel mismatch"); return out; }
-      if (o.res_mode == 3) {
-        p.res_t_mode = 0;
-        p.res_pool_off = o.res_pool_off;
-        if (v11) p.res_t_mode = 1;   // replicate (model_3dcausal_v1_1.py:293-294)
-        if (streaming() && o.cache_key) {
-          pc = cache(std::string(o.cache_key) + "#pool", (size_t)r.B * r.frame() * dtype_size(ta));
-          if (!pc) return out;
-          if (!ck->first) { p.res_t_mode = 2; p.res_cache = pc->in(); }
-        }
-      }
+      pc = cache(std::string(o.cache_key) + "#pool", (size_t)r.B * r.frame() * dtype_size(ta));
+      if (!pc) return out;
+      if (p.res_t_mode == 2) p.res_cache = pc->in();
     }
     const DType tin = o.ext_in ? DT_F32 : ta;
     const DType tout = o.ext_out ? DT_F32 : ta;
-    const bf16* wtc = split ? w.w_nk3 : w.w_nk;
-    const bool tc = tcm && !o.force_simt && !o.ext_in && w.Kpad > 0 && conv_tc_supported(p, tout, dry);
-    // LayerNorm fusion into the epilogue: the planning (dry) pass and the real pass must take the same decision
-    TcLnFusion lf;
-    if (tc && tout != DT_F32 && m->desc.norm_type == VT_NORM_LAYERNORM && conv_tc_can_fuse_ln(p)) {
-      if (o.ln1) {
-        lf.mode = 1; lf.silu = o.ln1_silu; lf.gamma = o.ln1->gamma; lf.beta = o.ln1->beta;
-        o.fused1 = true;
-      } else if (o.ln2) {
-        lf.mode = 2; lf.silu = o.ln2_silu; lf.gamma = o.ln2->gamma; lf.beta = o.ln2->beta;
-        if (o.out_view) {
-          lf.out2 = o.ln2_view;
-        } else {
-          o.ln2_act = new_act(out.B, out.T, out.H, out.W, out.C);
-          lf.out2 = o.ln2_act.p;
-        }
-        o.fused2 = true;
-        if (!ok()) return out;
-      }
+    TcPlan pl;
+    const bool tc = tc_plan(w, p, o, &pl);
+    o.fused1 = tc && pl.ln.mode == 1;
+    o.fused2 = tc && pl.ln.mode == 2;
+    o.fused_reg = tc && pl.reg.mode != 0;
+    if (o.fused2 && !o.out_view) {
+      o.ln2_act = new_act(out.B, out.T, out.H, out.W, out.C);
+      pl.ln.out2 = o.ln2_act.p;
+      if (!ok()) return out;
     }
-    // regularizer epilogue: same decision in the planning pass and the real pass (geometry only)
-    const bool reg_fuse = tc && o.reg && o.reg->mode && tout == DT_F32 && w.Co_pad == 32 &&
-                          (o.reg->mode == 1 ? (o.reg->zc == 4 || o.reg->zc == 8 || o.reg->zc == 16) : o.reg->zc <= VT_MAX_FSQ);
-    o.fused_reg = reg_fuse;
     if (!dry) {
       const bf16* wst = split ? w.w_stem3 : w.w_stem;
-      const bool stem = tcm && !o.force_simt && o.ext_in && !o.ext_in_indices && !o.ext_out && !o.out_view && wst && conv_stem_supported(p);
+      const bool stem = tcm && !o.force_simt && o.ext_in && !o.ext_in_indices && !o.ext_out && !o.out_view && w.stem && conv_stem_supported(p);
       if (tc) {
-        void* optr = (reg_fuse && o.reg_only) ? nullptr : out.p;
-        if (!cuda(launch_conv_tc(p, (const bf16*)in.p, wtc, w.Kpad, optr, tout, s, 1, 0, lf.mode ? &lf : nullptr, reg_fuse ? o.reg : nullptr),
-                  conv_tc_last_error())) return out;
+        void* optr = (o.fused_reg && o.reg_only) ? nullptr : out.p;
+        if (!cuda(launch_conv_tc(pl, (const bf16*)in.p, split ? w.w_nk3 : w.w_nk, optr, s), conv_tc_last_error())) return out;
       } else if (stem) {
         if (!cuda(launch_conv_stem(p, o.ext_in, wst, (bf16*)out.p, s), "conv_stem")) return out;
       } else if (!w.w_kn) {
@@ -698,7 +727,7 @@ struct Exec {
           if (!ok()) return out;
         } else {
           // v1.0: zero frames in front of the first chunk (v1.1 replicates frame 0)
-          const bool zero_front = !v11 && ck->first;
+          const bool zero_front = m->desc.version == 0 && ck->first;
           if (zero_front && !cuda(cudaMemsetAsync(cb->in(), 0, cb->bytes, s), "cache_update")) return out;
           if (!cuda(launch_cache_update(tin, o.ext_in ? (const void*)o.ext_in : in.p, cb->in(), cb->out(), in.B, in.T,
                                         p.pt, cache_off, ck->first && !zero_front, in.frame(), o.ext_in ? p.isB : p.isB / cw, s), "cache_update")) return out;
@@ -770,8 +799,8 @@ struct Exec {
   // ResnetCausalBlock1D as ONE launch (tblock_tc.cu): BF16 mode, v1.0 zero padding, LayerNorm, 128 channels
   bool resblock1d_fused(const ResBlockW& r, Stream& st, const NormW* next, bool next_silu) {
     if (prec != VT_PREC_BF16 || m->desc.version != 0 || m->desc.noncausal || m->desc.norm_type != VT_NORM_LAYERNORM) return false;
-    if (r.c1.Ci != 128 || r.c1.Co != 128 || r.c2.Co != 128 || !r.c1.w_nk || !r.c2.w_nk || r.c1.kt != 3 || r.c1.kh != 1) return false;
-    if (!tblock_tc_supported(st.x.B, st.x.T, st.x.H, st.x.W, st.x.C, dry)) return false;
+    if (r.c1.Ci != 128 || r.c1.Co != 128 || r.c2.Co != 128 || r.c1.kt != 3 || r.c1.kh != 1) return false;
+    if (!tblock_tc_supported(st.x.B, st.x.T, st.x.H, st.x.W, st.x.C)) return false;
     // streaming: the conv1 / conv2 caches of the two-launch path (n1 and LN2(h) frames t-2, t-1), read and written in-kernel
     CacheBuf* cc[2] = {nullptr, nullptr};
     TbCache tc;
@@ -844,17 +873,18 @@ struct Exec {
     pv.Ci = tokens; set_in(pv, cl_strides(1, q.H, q.W, tokens, cw));
     pv.Co = C; set_out(pv, cl_strides(1, q.H, q.W, C, cw));
     pv.rb = 1.0f;
-    if (!dry && (!conv_tc_supported(ps, DT_F32) || !conv_tc_supported(pv, ta))) return false;
+    TcPlan pls, plv;
+    if (!conv_tc_plan(ps, DT_F32, nullptr, nullptr, frames, &pls) || !conv_tc_plan(pv, ta, nullptr, nullptr, frames, &plv)) return false;
     o = new_act(q.B, q.T, q.H, q.W, C);
     float* S = (float*)alloc((size_t)frames * tokens * tokens * sizeof(float));
     bf16* P = (bf16*)alloc((size_t)frames * tokens * tokens * dtype_size(ta));
     bf16* Vt = (bf16*)alloc((size_t)frames * tokens * C * dtype_size(ta));
     if (ok() && !dry) {
       // per-frame "weights": K of the frame ([tokens][C], split: [tokens][hi C | lo C]) and V^T ([C][tokens])
-      cuda(launch_conv_tc(ps, (const bf16*)q.p, (const bf16*)k.p, C, S, DT_F32, s, frames, (long long)tokens * C * cw), conv_tc_last_error());
+      cuda(launch_conv_tc(pls, (const bf16*)q.p, (const bf16*)k.p, S, s, (long long)tokens * C * cw), conv_tc_last_error());
       cuda(launch_softmax_rows(ta, S, P, (long long)frames * tokens, tokens, s), "attn softmax");
       cuda(launch_transpose_bf16((const bf16*)v.p, Vt, frames, tokens, C, s, split), "attn transpose V");
-      cuda(launch_conv_tc(pv, P, Vt, tokens, o.p, ta, s, frames, (long long)tokens * C * cw), conv_tc_last_error());
+      cuda(launch_conv_tc(plv, P, Vt, o.p, s, (long long)tokens * C * cw), conv_tc_last_error());
     }
     ar.release(Vt);
     ar.release(P);
@@ -866,8 +896,7 @@ struct Exec {
   // up to 1024 tokens keep the two-GEMM path above, whose launch plans the production-plan table pins.
   bool attention_fused(const Act& q, const Act& k, const Act& v, Act& o) {
     const long long frames = (long long)q.B * q.T, tokens = (long long)q.H * q.W;
-    if (!tcm || tokens <= 1024 || q.C % 64 != 0 || q.C > 512) return false;
-    if (!attn_tc_supported(frames, tokens, q.C, split, true)) return false;
+    if (!tcm || tokens <= 1024 || !attn_tc_supported(frames, tokens, q.C, split)) return false;
     o = new_act(q.B, q.T, q.H, q.W, q.C);
     void* vt = alloc(attn_tc_workspace(frames, tokens, q.C, split));
     if (ok() && !dry)
@@ -942,10 +971,6 @@ struct Exec {
   }
   bool fold_upsample() const { return prec == VT_PREC_FMA32; }
 
-  bool phase_ln_ok(const ConvW& ph) const {
-    return tcm && m->desc.norm_type == VT_NORM_LAYERNORM && ph.Co % 32 == 0 && ph.Co <= 256 &&
-           (!split || split_ln_fusion_keeps_kparts(ph.Co, ph.taps() * (ph.Ci / 64)));
-  }
   // Downsample: pad (0,1,0,1) + conv3x3 stride 2 (model_3dcausal.py:223-227)
   void down(const LevelW& lv, Stream& st, const NormW* next, bool next_silu) {
     ConvOpt o; o.sh = 2; o.sw = 2; o.ph0 = 0; o.ph1 = 1; o.pw0 = 0; o.pw1 = 1;
@@ -973,23 +998,27 @@ struct Exec {
     } else if (lv.has_up_phase && tcm) {
       // four parity classes of the 2x-upsampled output, each a 1x2x2 conv on the low-resolution input
       Act y = new_act(h.B, h.T, 2 * h.H, 2 * h.W, lv.resample.Co);
-      const bool fuse = next && phase_ln_ok(lv.up_ph[0]);
+      const long long C = lv.resample.Co, Wo2 = 2 * h.W, Ho2 = 2 * h.H;
+      auto phase = [&](int py, int px, const Act* n) {   // n: where the fused LayerNorm of the next stage goes
+        ConvOpt o;
+        o.ph0 = py == 0 ? 1 : 0; o.ph1 = 1 - o.ph0; o.pw0 = px == 0 ? 1 : 0; o.pw1 = 1 - o.pw0;
+        const size_t off = (size_t)((py * Wo2 + px) * C) * dtype_size(ta);
+        o.out_view = dry ? y.p : (void*)((char*)y.p + off);
+        o.ov_sW = 2 * C * cw; o.ov_sH = 2 * Wo2 * C * cw; o.ov_sT = Ho2 * Wo2 * C * cw; o.ov_sB = o.ov_sT * h.T;
+        if (n) { o.ln2 = next; o.ln2_silu = next_silu; o.ln2_view = dry ? n->p : (void*)((char*)n->p + off); }
+        return o;
+      };
+      // the next stage's LayerNorm is fused when the first phase conv's plan takes it (else that stage normalises)
+      const bool fuse = fuses_ln(lv.up_ph[0], h, phase(0, 0, nullptr), next, next_silu);
       Act n;
       if (fuse) n = new_act(h.B, h.T, 2 * h.H, 2 * h.W, lv.resample.Co);
-      const long long C = lv.resample.Co, Wo2 = 2 * h.W, Ho2 = 2 * h.H;
-      ConvOpt last;
       for (int py = 0; py < 2 && ok(); ++py)
         for (int px = 0; px < 2 && ok(); ++px) {
-          ConvOpt o;
-          o.ph0 = py == 0 ? 1 : 0; o.ph1 = 1 - o.ph0; o.pw0 = px == 0 ? 1 : 0; o.pw1 = 1 - o.pw0;
-          const size_t off = (size_t)((py * Wo2 + px) * C) * dtype_size(ta);
-          o.out_view = dry ? y.p : (void*)((char*)y.p + off);
-          o.ov_sW = 2 * C * cw; o.ov_sH = 2 * Wo2 * C * cw; o.ov_sT = Ho2 * Wo2 * C * cw; o.ov_sB = o.ov_sT * h.T;
-          if (fuse) { o.ln2 = next; o.ln2_silu = next_silu; o.ln2_view = dry ? n.p : (void*)((char*)n.p + off); }
+          ConvOpt o = phase(py, px, fuse ? &n : nullptr);
           conv(lv.up_ph[py * 2 + px], h, o);
           if (fuse && ok() && !o.fused2) rc = fail(VT_ERR_INVALID, "upsample phase conv did not fuse its LayerNorm");
         }
-      set_stream(st, y, last);
+      set_stream(st, y, ConvOpt());
       if (fuse) { st.n = n; st.n_of = next; }
     } else {
       Act hu = upsample_mat(h, 1, 2, 2);
@@ -1019,20 +1048,24 @@ struct Exec {
       if (lv.has_tup_phase && tcm) {
         // even / odd output frames: 2x3x3 convs on the un-upsampled input, mixed with x[t/2] in the epilogue
         Act out = new_act(x.B, 2 * x.T, x.H, x.W, lv.tconv.Co);
-        const bool fuse = next && phase_ln_ok(lv.tup_ph[0]);
-        Act n;
-        if (fuse) n = new_act(x.B, 2 * x.T, x.H, x.W, lv.tconv.Co);
         const long long fr = (long long)x.H * x.W * lv.tconv.Co;
-        for (int pt = 0; pt < 2 && ok(); ++pt) {
+        const std::string pk[2] = {ckey + "#ph0", ckey + "#ph1"};   // streaming: each parity keeps its own copy of x[-1]
+        auto phase = [&](int pt, const Act* n) {   // n: where the fused LayerNorm of the next stage goes
           ConvOpt op;
           op.ra = lv.alpha; op.rb = 1.f - lv.alpha; op.res_mode = 1; op.res = &x;
           if (m->desc.noncausal) { op.pt_front = pt == 0 ? 1 : 0; op.pt_back = pt == 0 ? 0 : 1; }   // frames (i-1, i) / (i, i+1)
-          const std::string pk = ckey + (pt ? "#ph1" : "#ph0");   // streaming: each parity keeps its own copy of x[-1]
-          op.cache_key = pk.c_str();
+          op.cache_key = pk[pt].c_str();
           const size_t off = (size_t)(pt * fr) * dtype_size(ta);
           op.out_view = dry ? out.p : (void*)((char*)out.p + off);
           op.ov_sW = (long long)lv.tconv.Co * cw; op.ov_sH = (long long)x.W * lv.tconv.Co * cw; op.ov_sT = 2 * fr * cw; op.ov_sB = 2 * fr * x.T * cw;
-          if (fuse) { op.ln2 = next; op.ln2_silu = next_silu; op.ln2_view = dry ? n.p : (void*)((char*)n.p + off); }
+          if (n) { op.ln2 = next; op.ln2_silu = next_silu; op.ln2_view = dry ? n->p : (void*)((char*)n->p + off); }
+          return op;
+        };
+        const bool fuse = fuses_ln(lv.tup_ph[0], x, phase(0, nullptr), next, next_silu);
+        Act n;
+        if (fuse) n = new_act(x.B, 2 * x.T, x.H, x.W, lv.tconv.Co);
+        for (int pt = 0; pt < 2 && ok(); ++pt) {
+          ConvOpt op = phase(pt, fuse ? &n : nullptr);
           conv(lv.tup_ph[pt], x, op);
           if (fuse && ok() && !op.fused2) rc = fail(VT_ERR_INVALID, "time-upsample phase conv did not fuse its LayerNorm");
         }
@@ -1172,8 +1205,7 @@ static void run_encoder(Exec& ex, const float* x_ext, int B, int T, int H, int W
   Act xin;
   xin.p = (void*)x_ext; xin.B = B; xin.T = T; xin.H = H; xin.W = W; xin.C = d.in_channels;
   Exec::Stream st;
-  const bf16* stem_w = ex.split ? e.conv_in.w_stem3 : e.conv_in.w_stem;
-  if (ex.streaming() && ex.tcm && stem_w && T + t_rep >= 2 && e.conv_in.Ci * 27 <= 128) {
+  if (ex.streaming() && ex.tcm && e.conv_in.stem && T + t_rep >= 2) {
     // chunked v1.1 / streamed v1.0 on the stem kernel: the causal cache (last two padded input frames,
     // model_3dcausal_v1_1.py:230-233) is kept in the caller's layout (fp32 [B,C,2,H,W]) and read by the kernel's patch loader
     CacheBuf* cb = ex.cache("encoder.conv_in#stem", (size_t)B * d.in_channels * 2 * H * W * sizeof(float));
@@ -1185,7 +1217,7 @@ static void run_encoder(Exec& ex, const float* x_ext, int B, int T, int H, int W
       p.t_mode = ex.ck->first ? (d.version == 1 ? 1 : 0) : 2;   // first chunk: replicate (v1.1) / zero (v1.0) padding
       p.cache = cb->in(); p.cacheT = 2;
       if (!conv_stem_supported(p)) { ex.rc = fail(VT_ERR_INVALID, "stem kernel rejected the chunk geometry"); return; }
-      ex.cuda(launch_conv_stem(p, x_ext, stem_w, (bf16*)st.x.p, ex.s), "conv_stem");
+      ex.cuda(launch_conv_stem(p, x_ext, ex.split ? e.conv_in.w_stem3 : e.conv_in.w_stem, (bf16*)st.x.p, ex.s), "conv_stem");
       ex.cuda(launch_stem_cache_update(x_ext, (float*)cb->out(), B, d.in_channels, T, t_rep, H, W, ex.s), "stem cache");
       ex.commit(cb);
     }
@@ -1490,21 +1522,12 @@ int32_t vt_model_finalize(vt_model* m, void* stream) {
   // sizes
   size_t kn = 0, nk = 0;
   for (ConvW* c : m->convs) {
-    const int K = c->taps() * c->Ci;
-    kn += align_up((size_t)K * c->Co, 64);
-    c->Kpad = 0;
-    c->Co_pad = (c->Co + 31) / 32 * 32;
-    if (c->Ci % 64 == 0) {
-      c->Kpad = K;
-      nk += align_up((size_t)c->Co_pad * K, 512);
-    }
+    kn += align_up((size_t)c->taps() * c->Ci * c->Co, 64);
+    if (c->Kpad) nk += align_up((size_t)c->Co_pad * c->Kpad, 512);
   }
-  // phase-collapsed weights for "nearest 2x upsample then conv" (decoder Upsample / v1.0 TimeUpsampleResCausal2x)
   for (auto& lv : m->dec.levels) {
-    lv.has_up_phase = lv.has_resample && lv.resample.Ci % 64 == 0 && lv.resample.Co % 32 == 0;
-    lv.has_tup_phase = lv.has_tres && m->desc.version == 0 && lv.tconv.Ci % 64 == 0 && lv.tconv.Co % 32 == 0;
-    if (lv.has_up_phase) nk += 4 * align_up((size_t)lv.resample.Co * 4 * lv.resample.Ci, 512);
-    if (lv.has_tup_phase) nk += 2 * align_up((size_t)lv.tconv.Co * 18 * lv.tconv.Ci, 512);
+    if (lv.has_up_phase) nk += 4 * align_up((size_t)lv.up_ph[0].Co_pad * lv.up_ph[0].Kpad, 512);
+    if (lv.has_tup_phase) nk += 2 * align_up((size_t)lv.tup_ph[0].Co_pad * lv.tup_ph[0].Kpad, 512);
   }
   if (!m->packed_kn) VT_CUDA(cudaMalloc(&m->packed_kn, kn * sizeof(float)));
   if (!m->packed_nk && nk) VT_CUDA(cudaMalloc(&m->packed_nk, nk * sizeof(bf16)));
@@ -1535,7 +1558,7 @@ int32_t vt_model_finalize(vt_model* m, void* stream) {
     if (c->Kpad) {
       c->w_nk = m->packed_nk + onk;
       c->w_nk3 = m->packed_nk3 + 2 * onk;
-      onk += align_up((size_t)c->Co_pad * K, 512);
+      onk += align_up((size_t)c->Co_pad * c->Kpad, 512);
       VT_CUDA(launch_pack_w_nk_bf16(w, c->w_nk, c->Co, c->Co_pad, c->Ci, c->taps(), c->Kpad, s));
       VT_CUDA(launch_pack_w_nk_bf16(w, c->w_nk3, c->Co, c->Co_pad, c->Ci, c->taps(), c->Kpad, s, c->wscale3));
     }
@@ -1549,10 +1572,8 @@ int32_t vt_model_finalize(vt_model* m, void* stream) {
       for (int py = 0; py < 2; ++py)
         for (int px = 0; px < 2; ++px) {
           ConvW& ph = lv.up_ph[py * 2 + px];
-          ph = ConvW();
-          ph.Co = c.Co; ph.Ci = c.Ci; ph.kt = 1; ph.kh = 2; ph.kw = 2; ph.Co_pad = c.Co; ph.Kpad = 4 * c.Ci;
           ph.bias = c.bias; ph.w_nk = m->packed_nk + onk; ph.w_nk3 = m->packed_nk3 + 2 * onk; ph.wscale3 = c.wscale3;
-          onk += align_up((size_t)c.Co * 4 * c.Ci, 512);
+          onk += align_up((size_t)ph.Co_pad * ph.Kpad, 512);
           VT_CUDA(launch_pack_w_collapsed(w, ph.w_nk, c.Co, c.Co, c.Ci, 1, 3, 3, id1, py == 0 ? lo : hi, px == 0 ? lo : hi, 1, 2, 2, s));
           VT_CUDA(launch_pack_w_collapsed(w, ph.w_nk3, c.Co, c.Co, c.Ci, 1, 3, 3, id1, py == 0 ? lo : hi, px == 0 ? lo : hi, 1, 2, 2, s, c.wscale3));
         }
@@ -1562,10 +1583,8 @@ int32_t vt_model_finalize(vt_model* m, void* stream) {
       const float* w = m->pool + m->params[c.pw].offset;
       for (int pt = 0; pt < 2; ++pt) {
         ConvW& ph = lv.tup_ph[pt];
-        ph = ConvW();
-        ph.Co = c.Co; ph.Ci = c.Ci; ph.kt = 2; ph.kh = 3; ph.kw = 3; ph.Co_pad = c.Co; ph.Kpad = 18 * c.Ci;
         ph.bias = c.bias; ph.w_nk = m->packed_nk + onk; ph.w_nk3 = m->packed_nk3 + 2 * onk; ph.wscale3 = c.wscale3;
-        onk += align_up((size_t)c.Co * 18 * c.Ci, 512);
+        onk += align_up((size_t)ph.Co_pad * ph.Kpad, 512);
         // even frames t'=2i read x'[2i-2..2i] = x[i-1],x[i-1],x[i]; odd frames read x[i-1],x[i],x[i]
         // non-causal (pad 1 on both sides): even frames read x'[2i-1..2i+1] = x[i-1],x[i],x[i]; odd frames x[i],x[i],x[i+1]
         const int* tmap = m->desc.noncausal ? (pt == 0 ? lo : hi) : (pt == 0 ? hi : lo);
@@ -1576,7 +1595,7 @@ int32_t vt_model_finalize(vt_model* m, void* stream) {
   }
   {
     ConvW& c = m->enc.conv_in;
-    if (c.Ci * 27 <= 128 && c.Co % 64 == 0 && c.Co <= 256 && c.kt == 3 && c.kh == 3 && c.kw == 3) {
+    if (c.stem) {
       if (!m->packed_stem) VT_CUDA(cudaMalloc(&m->packed_stem, (size_t)c.Co * 128 * 3 * sizeof(bf16)));
       c.w_stem = m->packed_stem;
       c.w_stem3 = m->packed_stem + (size_t)c.Co * 128;
@@ -1584,17 +1603,11 @@ int32_t vt_model_finalize(vt_model* m, void* stream) {
       VT_CUDA(launch_pack_w_nk_bf16(m->pool + m->params[c.pw].offset, c.w_stem3, c.Co, c.Co, c.Ci, 27, 128, s, c.wscale3));
     }
   }
-  {
-    // decoder head as tap planes (v1.0 only: zero causal padding, no chunk caches)
+  if (m->head_planes.Kpad) {
     const ConvW& c = m->dec.conv_out;
-    m->head_planes = ConvW();
-    if (m->desc.version == 0 && c.kt == 3 && c.kh == 3 && c.kw == 3 && c.Co <= 4 && c.Ci % 64 == 0) {
-      if (!m->packed_planes) VT_CUDA(cudaMalloc(&m->packed_planes, (size_t)128 * c.Ci * sizeof(bf16)));
-      VT_CUDA(launch_pack_w_tap_planes(m->pool + m->params[c.pw].offset, m->packed_planes, c.Co, c.Ci, 128, s));
-      ConvW& hp = m->head_planes;
-      hp.Co = 128; hp.Ci = c.Ci; hp.kt = hp.kh = hp.kw = 1; hp.Co_pad = 128; hp.Kpad = c.Ci; hp.w_nk = m->packed_planes;
-      hp.bias = nullptr;
-    }
+    if (!m->packed_planes) VT_CUDA(cudaMalloc(&m->packed_planes, (size_t)128 * c.Ci * sizeof(bf16)));
+    VT_CUDA(launch_pack_w_tap_planes(m->pool + m->params[c.pw].offset, m->packed_planes, c.Co, c.Ci, 128, s));
+    m->head_planes.w_nk = m->packed_planes;
   }
   for (NormW* n : m->norms) {
     n->gamma = m->pool + m->params[n->pg].offset;
@@ -2235,7 +2248,6 @@ static int op_conv_impl(int precision, int force_simt, const vt_conv_desc* d, co
   if (e && e->ln_mode) {
     if (!gamma || !beta || (e->ln_mode == 2 && !out2)) return fail(VT_ERR_INVALID, "fused LayerNorm needs gamma, beta (and out2 for mode 2)");
     if (precision == VT_PREC_FMA32 || force_simt) return fail(VT_ERR_INVALID, "the LayerNorm epilogue exists on the wgmma path only");
-    if (!conv_tc_can_fuse_ln(p)) return fail(VT_ERR_INVALID, "LayerNorm cannot be fused for this Cout");
     lf.mode = e->ln_mode; lf.silu = e->ln_silu != 0; lf.gamma = gamma; lf.beta = beta; lf.out2 = out2;
   }
   float* wkn = nullptr;
@@ -2243,18 +2255,19 @@ static int op_conv_impl(int precision, int force_simt, const vt_conv_desc* d, co
   cudaError_t er;
   const bool want_tc = precision != VT_PREC_FMA32 && !force_simt;
   if (want_tc) {
-    if (d->Ci % 64 != 0 || !conv_tc_supported(p, tout))
-      return fail(VT_ERR_INVALID, "wgmma conv does not support this geometry: %s", d->Ci % 64 ? "Cin % 64 != 0" : conv_tc_last_error());
-    const int Co_pad = (d->Co + 31) / 32 * 32;
-    VT_CUDA(cudaMalloc(&wnk, (size_t)K * Co_pad * sizeof(bf16) * cw));
     float wsc = 0.f;
     if (ta == DT_SPLIT) {
       int rc = op_weight_scale(w, (long long)d->Co * K, kModelWeightHeadroom, s, &wsc);
-      if (rc) { cudaFree(wnk); return rc; }
+      if (rc) return rc;
       p.acc_scale = 1.0f / wsc;
     }
+    TcPlan pl;
+    if (!conv_tc_plan(p, tout, &lf, reg, 1, &pl)) return fail(VT_ERR_INVALID, "wgmma conv does not support this geometry: %s", conv_tc_last_error());
+    if (pl.ln.mode != lf.mode || (reg && reg->mode && !pl.reg.mode)) return fail(VT_ERR_INVALID, "epilogue cannot be fused: %s", conv_tc_last_error());
+    const int Co_pad = (d->Co + 31) / 32 * 32;
+    VT_CUDA(cudaMalloc(&wnk, (size_t)K * Co_pad * sizeof(bf16) * cw));
     VT_CUDA(launch_pack_w_nk_bf16(w, wnk, d->Co, Co_pad, d->Ci, taps, K, s, wsc));
-    er = launch_conv_tc(p, (const bf16*)x, wnk, K, out, tout, s, 1, 0, lf.mode ? &lf : nullptr, reg);
+    er = launch_conv_tc(pl, (const bf16*)x, wnk, out, s);
   } else {
     VT_CUDA(cudaMalloc(&wkn, (size_t)K * d->Co * sizeof(float)));
     VT_CUDA(launch_pack_w_kn(w, wkn, d->Co, d->Ci, taps, s));
@@ -2371,9 +2384,9 @@ int32_t vt_op_head_planes(const void* x, const float* w, const float* bias, floa
   set_out(p, cl_strides(T, H, W, 128, 1));
   p.kt = p.kh = p.kw = 1;
   p.ra = 0.f; p.rb = 1.f;
-  cudaError_t er = cudaSuccess;
-  if (!conv_tc_supported(p, DT_BF16)) er = cudaErrorInvalidValue;
-  if (er == cudaSuccess) er = launch_conv_tc(p, (const bf16*)x, wp, Ci, P, DT_BF16, s);
+  TcPlan pl;
+  cudaError_t er = conv_tc_plan(p, DT_BF16, nullptr, nullptr, 1, &pl) ? cudaSuccess : cudaErrorInvalidValue;
+  if (er == cudaSuccess) er = launch_conv_tc(pl, (const bf16*)x, wp, P, s);
   if (er == cudaSuccess) er = launch_tap_planes_gather(P, bias, out, B, T, H, W, 128, Co, to_off, s);
   cudaError_t e2 = cudaStreamSynchronize(s);
   cudaFree(wp); cudaFree(P);
@@ -2410,24 +2423,20 @@ int32_t vt_op_upsample_conv(int32_t precision, int32_t kind, const void* x, cons
     int rcw = op_weight_scale(w, (long long)Co * Ci * (kind == 0 ? 9 : 27), kModelWeightHeadroom, s, &wsc);
     if (rcw) { cudaFree(wp); return rcw; }
   }
+  lv.resample.Co = Co; lv.resample.Ci = Ci; lv.tconv.Co = Co; lv.tconv.Ci = Ci;
   for (int i = 0; i < nph; ++i) {
     ConvW& ph = kind == 0 ? lv.up_ph[i] : lv.tup_ph[i];
-    ph = ConvW();
-    ph.Co = Co; ph.Ci = Ci; ph.Co_pad = Co; ph.Kpad = taps2 * Ci; ph.bias = bias;
+    if (kind == 0) phase_conv(ph, lv.resample, 1, 2, 2);
+    else phase_conv(ph, lv.tconv, 2, 3, 3);
+    ph.bias = bias;
     if (split) ph.wscale3 = wsc;
     bf16* dst = wp + per * i * (split ? 2 : 1);
     if (split) ph.w_nk3 = dst; else ph.w_nk = dst;
-    if (kind == 0) {
-      ph.kt = 1; ph.kh = 2; ph.kw = 2;
-      VT_CUDA(launch_pack_w_collapsed(w, dst, Co, Co, Ci, 1, 3, 3, id1, (i >> 1) == 0 ? lo : hi, (i & 1) == 0 ? lo : hi, 1, 2, 2, s, wsc));
-    } else {
-      ph.kt = 2; ph.kh = 3; ph.kw = 3;
-      VT_CUDA(launch_pack_w_collapsed(w, dst, Co, Co, Ci, 3, 3, 3, i == 0 ? hi : lo, id3, id3, 2, 3, 3, s, wsc));
-    }
+    if (kind == 0) VT_CUDA(launch_pack_w_collapsed(w, dst, Co, Co, Ci, 1, 3, 3, id1, (i >> 1) == 0 ? lo : hi, (i & 1) == 0 ? lo : hi, 1, 2, 2, s, wsc));
+    else VT_CUDA(launch_pack_w_collapsed(w, dst, Co, Co, Ci, 3, 3, 3, i == 0 ? hi : lo, id3, id3, 2, 3, 3, s, wsc));
   }
   lv.has_resample = kind == 0; lv.has_up_phase = kind == 0;
   lv.has_tres = kind == 1; lv.has_tup_phase = kind == 1;
-  lv.resample.Co = Co; lv.resample.Ci = Ci; lv.tconv.Co = Co; lv.tconv.Ci = Ci;
   lv.alpha = alpha;
   lv.tkey = "op";
   NormW nw;

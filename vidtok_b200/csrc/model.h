@@ -27,9 +27,10 @@ struct ConvW {
   bf16* w_nk = nullptr;      // [Co_pad][Kpad] bf16 (wgmma B operand), may be null
   bf16* w_nk3 = nullptr;     // [Co_pad][hi(Kpad) | lo(Kpad)] fp16 planes of w * wscale3: split operand of the EXACT_TC mode
   float wscale3 = 1.f;       // power of two (kernels.h: split_weight_scale); the epilogue multiplies the accumulator by 1/wscale3
-  int Kpad = 0;
+  int Kpad = 0;              // > 0: the conv has wgmma weights (Cin % 64 == 0); set with the geometry, before the weights
   int Co_pad = 0;            // Cout rounded up to 32 (zero rows)
-  bf16* w_stem = nullptr;    // [Co][128] bf16 (conv_stem.cu), only for the Cin<=4 stem
+  bool stem = false;         // the encoder's conv_in runs on conv_stem (Cin <= 4)
+  bf16* w_stem = nullptr;    // [Co][128] bf16 (conv_stem.cu), only for the stem
   bf16* w_stem3 = nullptr;   // [Co][hi 128 | lo 128] (EXACT_TC)
   const float* bias = nullptr;
   int taps() const { return kt * kh * kw; }

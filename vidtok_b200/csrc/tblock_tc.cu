@@ -405,13 +405,12 @@ bool strip_box(int H, int W, int& BW, int& BH) {
 
 const char* tblock_tc_last_error() { return g_tb_err.c_str(); }
 
-bool tblock_tc_supported(int B, int T, int H, int W, int C, bool planning) {
+bool tblock_tc_supported(int B, int T, int H, int W, int C) {
   g_tb_err.clear();
   if (C != kC) { g_tb_err = "C != 128"; return false; }
   if (B <= 0 || T <= 0) { g_tb_err = "empty"; return false; }
   int BW, BH;
   if (!strip_box(H, W, BW, BH)) { g_tb_err = "H x W not tileable by a 128-position box"; return false; }
-  if (!planning && !tmap_encoder()) { g_tb_err = "cuTensorMapEncodeTiled unavailable"; return false; }
   return true;
 }
 
