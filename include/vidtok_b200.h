@@ -161,6 +161,15 @@ int64_t vt_chunk_workspace_bytes(const vt_chunk_state* s, int32_t T_chunk);
 int32_t vt_encode_chunk(vt_chunk_state* s, int32_t is_first, const float* x_chunk, int32_t C, int32_t Tc, const float* noise,
                         float* z, int32_t* indices, float* kl_loss, void* workspace, int64_t workspace_bytes,
                         void* stream);
+/* vt_encode_chunk of an FSQ model that also writes this chunk's partials of the FSQ aux loss (see vt_fsq_aux_partials):
+ * stats fp32 [2] and avg_prob fp32 [J], J = prod(levels), over the chunk's B * Tz * Hz * Wz tokens -- the per-chunk step of
+ * vt_encode_video_fsq_aux.  The workspace holds the chunk's pre-bound latent and the partials' scratch on top of
+ * vt_chunk_workspace_bytes; vt_chunk_fsq_aux_workspace_bytes returns -1 (and records why) for a decoder state, a KL model or
+ * a level list vt_fsq_aux_partials does not support, and vt_encode_chunk_fsq_aux fails with VT_ERR_INVALID before any launch. */
+int64_t vt_chunk_fsq_aux_workspace_bytes(const vt_chunk_state* s, int32_t T_chunk);
+int32_t vt_encode_chunk_fsq_aux(vt_chunk_state* s, int32_t is_first, const float* x_chunk, int32_t C, int32_t Tc, float* z,
+                                int32_t* indices, float inv_temperature, float* stats, float* avg_prob, void* workspace,
+                                int64_t workspace_bytes, void* stream);
 /* z_chunk: device fp32 [B,Cz,Tzc,Hz,Wz] (Cz == z_channels) including the look-ahead frame when overlap applies; x_out receives
  * all decoded frames of this chunk (the caller trims the look-ahead tail as autoencoder_v1_1.py:327-328). */
 int32_t vt_decode_chunk(vt_chunk_state* s, int32_t is_first, const float* z_chunk, int32_t Cz, int32_t Tzc, float* x_out,

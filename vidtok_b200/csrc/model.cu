@@ -1977,7 +1977,42 @@ long long video_max_chunk_tokens(const vt_model* m, int B, int T, int H, int W, 
   }
   return best;
 }
+// what a chunk's aux partials write and read: stats [2], avg_prob [J], the pre-bound latent h fp32 [B,Cz,Tz,Hz,Wz] and the
+// partials' scratch (fsq_aux_workspace of the chunk's tokens)
+struct ChunkAux {
+  float inv_t;
+  float* stats;
+  float* avg_prob;
+  float* h;
+  void* ws;
+};
 }  // namespace
+
+// One chunk of an encode stream or of vt_encode_video: the encoder and the regularizer, then (aux != NULL) the FSQ aux
+// partials of the chunk's tokens from its pre-bound latent.  The aux geometry is checked before anything is launched.
+static int encode_chunk_aux(vt_chunk_state* cs, int32_t is_first, const float* x_chunk, int32_t C, int32_t Tc, const float* noise,
+                            float* z, int32_t* indices, float* kl_loss, const ChunkAux* aux, void* workspace, int64_t workspace_bytes,
+                            void* stream) {
+  FsqAuxGeom ag;
+  long long P = 0;
+  if (aux) {
+    if (!cs) return fail(VT_ERR_INVALID, "null argument");
+    const vt_model_desc& d = cs->m->desc;
+    if (d.regularizer != VT_REG_FSQ) return fail(VT_ERR_INVALID, "the FSQ aux loss needs an FSQ model");
+    if (Tc <= 0) return fail(VT_ERR_INVALID, "bad shape");
+    int Tz, Hz, Wz;
+    latent_shape(cs->m, Tc, cs->H, cs->W, &Tz, &Hz, &Wz);
+    P = (long long)Tz * Hz * Wz;
+    const char* why = fsq_aux_geometry(d.z_channels, d.fsq_levels, (long long)cs->B * P, &ag);
+    if (why) return fail(VT_ERR_INVALID, "%s", why);
+  }
+  int rc = encode_chunk(cs, is_first, x_chunk, C, Tc, noise, z, indices, kl_loss, aux ? aux->h : nullptr, workspace, workspace_bytes,
+                        stream);
+  if (rc || !aux) return rc;
+  VT_CUDA(launch_fsq_aux_partials(aux->h, ag, cs->m->desc.fsq_levels, P, aux->inv_t, aux->stats, aux->avg_prob, aux->ws,
+                                  (cudaStream_t)stream));
+  return VT_OK;
+}
 
 static int encode_video(vt_model* m, int32_t precision, const float* x, int32_t x_on_host, int32_t B, int32_t C, int32_t T,
                         int32_t H, int32_t W, int32_t t_chunk_enc, const float* noise, float* z, int32_t* indices,
@@ -2055,16 +2090,11 @@ static int encode_video(vt_model* m, int32_t precision, const float* x, int32_t 
     if (ce == cudaSuccess && noise)
       ce = copy_frames_2d(noise_c, tzc, 0, noise, TzTot, tz0, (size_t)B * d.z_channels, tzc, fr_z, cudaMemcpyDeviceToDevice, s);
     if (ce != cudaSuccess) break;
-    rc = encode_chunk(st, i == 0, stage[cur], C, n, noise ? noise_c : nullptr, z_c, indices ? idx_c : nullptr,
-                      d.regularizer == VT_REG_KL ? kl_c + i : nullptr, h_c, w, ws_left, stream);
+    const ChunkAux ca{aux ? aux->inv_t : 0.f, aux ? aux->stats + 2 * i : nullptr, aux ? aux->avg_prob + (size_t)i * ag.J : nullptr,
+                      h_c, aux_ws};
+    rc = encode_chunk_aux(st, i == 0, stage[cur], C, n, noise ? noise_c : nullptr, z_c, indices ? idx_c : nullptr,
+                          d.regularizer == VT_REG_KL ? kl_c + i : nullptr, aux ? &ca : nullptr, w, ws_left, stream);
     if (rc) break;
-    if (aux) {
-      const char* why = fsq_aux_geometry(d.z_channels, d.fsq_levels, (long long)B * tzc * Hz * Wz, &ag);
-      if (why) { rc = fail(VT_ERR_INVALID, "%s", why); break; }
-      ce = launch_fsq_aux_partials(h_c, ag, d.fsq_levels, (long long)tzc * Hz * Wz, aux->inv_t, aux->stats + 2 * i,
-                                   aux->avg_prob + (size_t)i * ag.J, aux_ws, s);
-      if (ce != cudaSuccess) break;
-    }
     ce = cudaEventRecord(m->ev_free[cur], s);
     if (ce == cudaSuccess) ce = copy_frames_2d(z, TzTot, tz0, z_c, tzc, 0, (size_t)B * d.z_channels, tzc, fr_z, cudaMemcpyDeviceToDevice, s);
     if (ce == cudaSuccess && indices)
@@ -2115,6 +2145,44 @@ int32_t vt_encode_video_fsq_aux(vt_model* m, int32_t precision, const float* x, 
   const VideoAux aux{inv_temperature, aux_stats, aux_avg_prob};
   return encode_video(m, precision, x, x_on_host, B, C, T, H, W, t_chunk_enc, nullptr, z, indices, nullptr, &aux, workspace,
                       workspace_bytes, stream);
+}
+
+// vt_encode_chunk_fsq_aux's workspace: [h | aux scratch | vt_chunk_workspace_bytes]
+static int chunk_aux_layout(const vt_chunk_state* cs, int32_t Tc, size_t* h_bytes, size_t* aux_bytes) {
+  if (!cs) return fail(VT_ERR_INVALID, "null state");
+  if (cs->is_decoder) return fail(VT_ERR_INVALID, "decoder state passed to vt_encode_chunk_fsq_aux");
+  const vt_model_desc& d = cs->m->desc;
+  if (d.regularizer != VT_REG_FSQ) return fail(VT_ERR_INVALID, "the FSQ aux loss needs an FSQ model");
+  if (Tc <= 0) return fail(VT_ERR_INVALID, "bad shape");
+  int Tz, Hz, Wz;
+  latent_shape(cs->m, Tc, cs->H, cs->W, &Tz, &Hz, &Wz);
+  FsqAuxGeom ag;
+  const char* why = fsq_aux_geometry(d.z_channels, d.fsq_levels, (long long)cs->B * Tz * Hz * Wz, &ag);
+  if (why) return fail(VT_ERR_INVALID, "%s", why);
+  *h_bytes = up1k((size_t)cs->B * d.z_channels * Tz * Hz * Wz * 4);
+  *aux_bytes = up1k(fsq_aux_workspace(ag));
+  return VT_OK;
+}
+
+int64_t vt_chunk_fsq_aux_workspace_bytes(const vt_chunk_state* cs, int32_t Tc) {
+  size_t hb, ab;
+  if (chunk_aux_layout(cs, Tc, &hb, &ab)) return -1;
+  const int64_t base = vt_chunk_workspace_bytes(cs, Tc);
+  if (base < 0) return -1;
+  return (int64_t)(hb + ab) + base;
+}
+
+int32_t vt_encode_chunk_fsq_aux(vt_chunk_state* cs, int32_t is_first, const float* x_chunk, int32_t C, int32_t Tc, float* z,
+                                int32_t* indices, float inv_temperature, float* stats, float* avg_prob, void* workspace,
+                                int64_t workspace_bytes, void* stream) {
+  size_t hb, ab;
+  if (int rc = chunk_aux_layout(cs, Tc, &hb, &ab)) return rc;
+  if (!stats || !avg_prob || !workspace) return fail(VT_ERR_INVALID, "null argument");
+  if (workspace_bytes <= (int64_t)(hb + ab)) return fail(VT_ERR_WORKSPACE, "workspace too small for the FSQ aux loss");
+  char* w = (char*)workspace;
+  const ChunkAux aux{inv_temperature, stats, avg_prob, (float*)w, w + hb};
+  return encode_chunk_aux(cs, is_first, x_chunk, C, Tc, nullptr, z, indices, nullptr, &aux, w + hb + ab,
+                          workspace_bytes - (int64_t)(hb + ab), stream);
 }
 
 int32_t vt_decode_video(vt_model* m, int32_t precision, const float* z, int32_t B, int32_t Cz, int32_t Tz, int32_t Hz, int32_t Wz,

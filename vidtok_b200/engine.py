@@ -132,9 +132,16 @@ class NativeModel:
         N.check(self.lib.vt_model_create(C.byref(desc), device_index, C.byref(self.handle)))
         self.device_index = device_index
         self._ws: Optional[torch.Tensor] = None
+        # handles of the open chunk states: a state returns its caches to the model when destroyed, so any still open go
+        # first (the garbage collector finalises a cycle holding both in no particular order)
+        self._chunk_handles: Dict[int, C.c_void_p] = {}
 
     def __del__(self):
         try:
+            for h in list(getattr(self, "_chunk_handles", {}).values()):
+                if h.value:
+                    self.lib.vt_chunk_state_destroy(h)
+                    h.value = None
             if getattr(self, "handle", None) and self.handle.value:
                 self.lib.vt_model_destroy(self.handle)
                 self.handle = C.c_void_p()
@@ -235,9 +242,11 @@ class ChunkState:
         self.handle = C.c_void_p()
         N.check(native.lib.vt_chunk_state_create(native.handle, precision, B, H, W, int(is_decoder), int(use_overlap),
                                                  C.byref(self.handle)))
+        native._chunk_handles[id(self)] = self.handle
 
     def close(self):
-        if self.handle and self.handle.value:
+        self.native._chunk_handles.pop(id(self), None)
+        if self.handle and self.handle.value:   # cleared when the model went first
             self.native.lib.vt_chunk_state_destroy(self.handle)
             self.handle = C.c_void_p()
 
@@ -249,6 +258,10 @@ class ChunkState:
 
     def workspace(self, Tc: int) -> torch.Tensor:
         return self.native._workspace(int(self.native.lib.vt_chunk_workspace_bytes(self.handle, Tc)))
+
+    def aux_workspace(self, Tc: int) -> torch.Tensor:
+        """workspace of vt_encode_chunk_fsq_aux for a chunk of Tc frames"""
+        return self.native._workspace(int(self.native.lib.vt_chunk_fsq_aux_workspace_bytes(self.handle, Tc)))
 
 
 # --------------------------------------------------------------------------------------------------
