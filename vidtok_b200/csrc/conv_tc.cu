@@ -15,9 +15,12 @@
 // B operand: TMA box {64, BN} of the pre-packed K-major bf16 weights [Cout][taps*Cin].
 // Both land in shared memory in the canonical K-major SWIZZLE_128B layout and feed wgmma.mma_async m64nBNk16.
 // Warp roles (persistent CTA, one per SM): warps 0-7 = two consumer warpgroups (wgmma, then the epilogue straight from the
-// accumulator registers: bias / residual / mix / LayerNorm / regularizer -> global memory), warp 8 = TMA producer, which
-// runs up to `stages` K steps ahead, across tile boundaries too, so that the next tile's operands load while the epilogue
-// runs.  The consumers follow one of two schedules (ping_pong()): cooperative, both warpgroups on every tile (rows
+// accumulator registers: bias / residual / mix / LayerNorm / regularizer), warp 8 = TMA producer, which runs up to `stages`
+// K steps ahead, across tile boundaries too, so that the next tile's operands load while the epilogue runs.  The bf16
+// output tiles of the 256-channel schedule leave through shared memory: each warpgroup packs 64 rows x 64 channels at a
+// time into its own swizzled staging buffer and one thread sends it with a bulk tensor store (TcParams::stage_out); all
+// other outputs are stored per thread.
+// The consumers follow one of two schedules (ping_pong()): cooperative, both warpgroups on every tile (rows
 // [64 g, 64 g + 64)), or ping-pong, each warpgroup on every second tile (all 128 rows), their main loops taking turns so
 // that one warpgroup's epilogue runs while the other one's MMAs issue.
 #include <cuda.h>
@@ -98,6 +101,13 @@ struct TcParams {
   FsqConst reg_fsq;
   uint32_t misc_off;         // byte offset of [bias | gamma | beta] x 2 (x 2 warpgroups in ping-pong) and the regularizer
                              // row buffer from the aligned base
+  // bf16 outputs through shared memory: a warpgroup writes 64 rows x 64 channels of out (or out2) into its staging buffer
+  // in the swizzled row layout and one bulk tensor store (maps o / o2) sends them, clipped at the tensor's edge.  The 64
+  // rows are one half of the CTA tile: the box of the tile halved along dimension half_dim (1 w, 2 h, 3 t), half_ext long.
+  int stage_out;             // the epilogue stores through the staging buffers
+  uint32_t stage_smem;       // bytes of the staging buffers between the stage ring and the barriers (0: none in the plan)
+  uint32_t stage_off;        // their byte offset from the aligned base
+  int half_dim, half_ext;
 };
 
 struct TcMaps {
@@ -106,6 +116,7 @@ struct TcMaps {
   CUtensorMap b;             // weights
   CUtensorMap r;             // residual tensor (output geometry), box = A box
   CUtensorMap e;             // 256 x 256 bf16 identity
+  CUtensorMap o, o2;         // out / out2 (stage_out), box = 64 channels x one 64-row half of the CTA tile
 };
 
 constexpr int kConsumerWarps = 8;       // warps 0-7: two wgmma warpgroups
@@ -116,7 +127,9 @@ constexpr int kThreads = (kConsumerWarps + 4) * 32;
 constexpr int kABytes = 128 * 128;      // 128 rows x 64 bf16
 // consumer named barriers (0 is __syncthreads): 1 = bias buffer switch (cooperative), 2 = regularizer rows,
 // kBarTurn + g = warpgroup g may start its next main loop, kBarBias + g = bias buffer switch of warpgroup g (ping-pong)
-constexpr uint32_t kBarTurn = 3, kBarBias = 5;
+// kBarStage + g = staging buffer of warpgroup g written / free again
+constexpr uint32_t kBarTurn = 3, kBarBias = 5, kBarStage = 7;
+constexpr uint32_t kStageOutBytes = 64 * 128;   // staging buffer of one warpgroup: 64 rows x 64 bf16
 
 // Ping-pong consumer schedule: with short K and a heavy epilogue (bf16 N tiles of 64 and 128 channels: 18-20 K steps
 // against LayerNorm and one or two stored tiles) the cooperative schedule leaves the tensor pipe idle for the whole
@@ -170,7 +183,9 @@ __device__ __forceinline__ float quad_sum(float v) {
   return v;
 }
 
-template <int BN, bool kSplit>
+// kStage: bf16 output tiles leave through the staging buffers (TcParams::stage_out); an instantiation of its own, so that
+// neither way of storing holds registers for the other next to the accumulators
+template <int BN, bool kSplit, bool kStage = false>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_tc_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -184,7 +199,8 @@ conv_tc_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
   const uint32_t stage_bytes = kPl * (p.halo ? b_bytes : a_bytes + b_bytes);
   const uint32_t win_bytes = kPl * p.halo_bytes;           // one halo window slot: [hi window | lo window]
   const uint32_t ring_base = smem_base + (p.halo ? (uint32_t)p.a_stages * win_bytes : 0u);
-  const uint32_t bar_base = ring_base + p.stages * stage_bytes;
+  // (the staging buffers of the bf16 output tiles lie between the ring and the barriers, 1024-byte aligned as every tile is)
+  const uint32_t bar_base = ring_base + p.stages * stage_bytes + p.stage_smem;
   // barriers: full[stages], empty[stages], fullA[a_stages], emptyA[a_stages]
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (p.stages + s); };
@@ -658,6 +674,93 @@ conv_tc_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
         continue;
       }
 
+      if constexpr (kStage) {
+        static_assert(!kSplit && BN == 256, "staged stores: the cooperative bf16 schedule");
+        {
+          // bf16 tiles through the warpgroup's staging buffer, 64 channels at a time.  The arithmetic is that of the
+          // per-thread path below; packing the bf16-rounded values a second time reproduces the same words.
+          float rstd[2], nmr[2];
+#pragma unroll
+          for (int r = 0; r < 2; ++r) {
+            float s = 0.f, q = 0.f;
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+              const float f0 = acc_h[4 * j + 2 * r], f1 = acc_h[4 * j + 2 * r + 1];
+              s += f0 + f1;
+              q = fmaf(f0, f0, q);
+              q = fmaf(f1, f1, q);
+              const uint32_t kp = pack_bf16x2(f0, f1);
+              acc_h[4 * j + 2 * r] = bf16_lo(kp);
+              acc_h[4 * j + 2 * r + 1] = bf16_hi(kp);
+            }
+            const float mean = quad_sum(s) * inv_n;
+            float var = fmaf(-mean, mean, quad_sum(q) * inv_n);
+            var = var < 0.f ? 0.f : var;
+            rstd[r] = rsqrtf(var + 1e-6f);
+            nmr[r] = -mean * rstd[r];
+          }
+          // this thread's words of a 64-channel chunk: rows lrow and lrow + 8 of the half (the same swizzle phase, 1024
+          // bytes apart), 16-byte unit u, bytes 2 cq .. 2 cq + 3 of it.  A warp's 32 words fall into 32 banks.
+          // (addresses derived from the opaque row0, so that they are formed here and not carried through the main loop)
+          const uint32_t sbuf = smem_base + p.stage_off + (uint32_t)(row0 >> 6) * kStageOutBytes;
+          const uint32_t sw = sbuf + swz128_unit(row0 & 63, 0) + 2u * cq;
+          auto put_s = [&](int r, int u, uint32_t word) {
+            asm volatile("st.shared.b32 [%0], %1;" ::"r"((sw ^ ((uint32_t)u << 4)) + 1024u * r), "r"(word) : "memory");
+          };
+          const bool issuer = (threadIdx.x & 127) == 0;   // bulk groups belong to the thread that commits them
+          // the previous store has read the buffer: the warpgroup may write it again
+          auto reserve = [&]() {
+            if (issuer) bulk_wait_read<0>();
+            named_bar_sync(kBarStage + g, 128);
+          };
+          // every thread's words are visible to the async proxy: send chunk k of this half to m
+          auto send = [&](const CUtensorMap* m, int k) {
+            fence_async_smem();
+            named_bar_sync(kBarStage + g, 128);
+            if (issuer) {
+              const int ho = g * p.half_ext;   // this warpgroup's half: its offset along half_dim
+              tma_store_5d(m, sbuf, tc.n0 + 64 * k, tc.w0 + (p.half_dim == 1 ? ho : 0), tc.h0 + (p.half_dim == 2 ? ho : 0),
+                           tc.t0 + (p.half_dim == 3 ? ho : 0), tc.b);
+              bulk_commit();
+            }
+          };
+          if (store_a) {
+#pragma unroll
+            for (int k = 0; k < BN / 64; ++k) {
+              reserve();
+#pragma unroll
+              for (int r = 0; r < 2; ++r)
+#pragma unroll
+                for (int u = 0; u < 8; ++u) put_s(r, u, pack_bf16x2(acc_h[4 * (8 * k + u) + 2 * r], acc_h[4 * (8 * k + u) + 2 * r + 1]));
+              send(&maps.o, k);
+            }
+          }
+          if (p.ln_mode) {
+            const CUtensorMap* nmap = p.ln_mode == 1 ? &maps.o : &maps.o2;
+#pragma unroll
+            for (int k = 0; k < BN / 64; ++k) {
+              reserve();
+#pragma unroll
+              for (int r = 0; r < 2; ++r)
+#pragma unroll
+                for (int u = 0; u < 8; ++u) {
+                  const int j = 8 * k + u, c = 8 * j + cq;
+                  float y0 = fmaf(fmaf(acc_h[4 * j + 2 * r], rstd[r], nmr[r]), gamma_s[c], beta_s[c]);
+                  float y1 = fmaf(fmaf(acc_h[4 * j + 2 * r + 1], rstd[r], nmr[r]), gamma_s[c + 1], beta_s[c + 1]);
+                  if (p.ln_silu) {
+                    // y holds h = LN(v)/2 (gamma, beta were halved): silu = h + h * tanh(h)
+                    y0 = fmaf(y0, tanh_approx(y0), y0);
+                    y1 = fmaf(y1, tanh_approx(y1), y1);
+                  }
+                  put_s(r, u, pack_bf16x2(y0, y1));
+                }
+              send(nmap, k);
+            }
+          }
+          continue;
+        }
+      }
+
       // 16-bit outputs: bf16 pairs, or hi | lo fp16 planes (split)
       auto put = [&](void* optr, int r, int c, float y0, float y1) {
         bf16* o = reinterpret_cast<bf16*>(optr) + ooff[r] + tc.n0 + c;
@@ -747,6 +850,8 @@ conv_tc_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
       }
     }
   }
+  // the last bulk stores of this warpgroup have read its staging buffer, and are complete, before the CTA can exit
+  if (kStage && (threadIdx.x & 127) == 0) bulk_wait<0>();
 }
 
 // 256 x 256 diagonal matrix `value` * I (bf16, or fp16 for the split mode)
@@ -860,9 +965,18 @@ bool conv_tc_plan(const ConvP& p, DType tout, const TcLnFusion* ln, const TcRegF
     static const int cap = [] { const char* e = getenv("VT_TC_STAGES"); return e ? atoi(e) : 0; }();
     if (cap >= 2 && stages > cap) stages = cap;
     t.stages = stages;
-    // smem layout from the 1024-aligned base: [halo windows] [stages x (A | B)] [barriers] [bias/gamma/beta | regularizer rows]
+    // smem layout from the 1024-aligned base:
+    //   [halo windows] [stages x (A | B)] [staging buffers] [barriers] [bias/gamma/beta | regularizer rows]
     const size_t bars = 8 * (2 * (size_t)stages + 2 * (size_t)t.a_stages);
-    t.misc_off = (uint32_t)((a_ring + stages * stage_bytes + bars + 15) & ~(size_t)15);
+    // bf16 output tiles of the cooperative 256-channel schedule leave through one staging buffer per warpgroup
+    // (TcParams::stage_out) where the two fit next to the ring as planned above: the ring's depth is never traded for
+    // them, and the budget above leaves 2 KB of the SM's 227 KB for this.  Not in ping-pong: there the epilogue already
+    // runs under the other warpgroup's MMAs, and the staged one measured slower (DESIGN.md section 8).
+    const size_t staging = 2 * (size_t)kStageOutBytes;
+    const bool staged = !split && tout == DT_BF16 && t.BN == 256 &&
+                        1024 + ((a_ring + stages * stage_bytes + staging + bars + 15) & ~(size_t)15) + misc <= 227 * 1024;
+    t.stage_out = staged ? 1 : 0;
+    t.misc_off = (uint32_t)((a_ring + stages * stage_bytes + (staged ? staging : 0) + bars + 15) & ~(size_t)15);
     t.smem = 1024 + t.misc_off + misc;
     // split + long K: the K steps of a tile are summed in groups (TcParams::kparts; needs BN <= 128)
     t.kparts = (split && t.BN <= 128 && nk >= 16) ? (nk >= 64 ? 8 : 4) : 1;
@@ -908,6 +1022,10 @@ cudaError_t launch_conv_tc(const TcPlan& pl, const bf16* x, const bf16* w_nk, vo
   t.BW = pl.BW; t.BH = pl.BH; t.BT = pl.BT; t.BN = pl.BN;
   t.halo = pl.halo; t.hP = pl.hP; t.a_stages = pl.a_stages; t.halo_bytes = pl.halo_bytes;
   t.stages = pl.stages; t.misc_off = pl.misc_off; t.kparts = pl.kparts; t.res_mma = pl.res_mma;
+  // a bulk tensor store needs a 16-byte aligned tensor, which the per-thread stores do not
+  t.stage_smem = pl.stage_out ? 2 * kStageOutBytes : 0;
+  t.stage_off = (uint32_t)pl.a_stages * pl.halo_bytes + (uint32_t)pl.stages * (uint32_t)((pl.halo ? 0 : kABytes) + pl.BN * 128);
+  t.stage_out = (pl.stage_out && ((uintptr_t)out & 15) == 0 && ((uintptr_t)pl.ln.out2 & 15) == 0) ? 1 : 0;
   t.tilesW = (p.Wo + t.BW - 1) / t.BW; t.tilesH = (p.Ho + t.BH - 1) / t.BH; t.tilesT = (p.To + t.BT - 1) / t.BT;
   t.num_n_tiles = Co_pad / t.BN;
   t.num_tiles = (long long)p.B * t.tilesT * t.tilesH * t.tilesW * t.num_n_tiles;
@@ -997,11 +1115,22 @@ cudaError_t launch_conv_tc(const TcPlan& pl, const bf16* x, const bf16* w_nk, vo
     cuuint32_t box[3] = {64, (cuuint32_t)t.BN, 1};
     if (!encode_tmap_16b(&maps.e, 3, ident, dims, strides, box, "identity", g_tc_err)) return cudaErrorInvalidValue;
   }
+  if (t.stage_out) {
+    // one 64-row half of the CTA tile: its box halved along the outermost dimension that is longer than one position
+    int hb[3] = {t.BW, t.BH, t.BT};
+    t.half_dim = t.BT > 1 ? 3 : (t.BH > 1 ? 2 : 1);
+    t.half_ext = (hb[t.half_dim - 1] /= 2);
+    if (!encode_out(&maps.o, out, p.To, p.osW, p.osH, p.osT, p.osB, hb[0], hb[1], hb[2])) return cudaErrorInvalidValue;
+    maps.o2 = maps.o;
+    if (t.ln_mode == 2 && !encode_out(&maps.o2, t.out2, p.To, p.osW, p.osH, p.osT, p.osB, hb[0], hb[1], hb[2])) return cudaErrorInvalidValue;
+  } else {
+    maps.o = maps.o2 = maps.a[0];
+  }
   {
     static SmemLimitOnce smem_limit;
     cudaError_t e = smem_limit.ensure(dev, 227 * 1024, conv_tc_kernel<32, false>, conv_tc_kernel<64, false>, conv_tc_kernel<128, false>,
                                       conv_tc_kernel<256, false>, conv_tc_kernel<32, true>, conv_tc_kernel<64, true>,
-                                      conv_tc_kernel<128, true>, conv_tc_kernel<256, true>);
+                                      conv_tc_kernel<128, true>, conv_tc_kernel<256, true>, conv_tc_kernel<256, false, true>);
     if (e != cudaSuccess) { g_tc_err = "cudaFuncSetAttribute(smem)"; return e; }
   }
   const int num_sms = device_sms(dev);
@@ -1014,7 +1143,8 @@ cudaError_t launch_conv_tc(const TcPlan& pl, const bf16* x, const bf16* w_nk, vo
   ProfScope _ps(split ? "conv_tc3" : "conv_tc", 2.0 * Mrows * p.kt * p.kh * p.kw * p.Ci * p.Co,
                 2.0 * cw * ((double)p.B * p.Ti * p.Hi * p.Wi * p.Ci) + Mrows * p.Co * (pl.tout == DT_F32 ? 4.0 : 2.0 * cw), s, det);
   auto launch = [&](auto kern) { kern<<<grid, kThreads, pl.smem, s>>>(maps, t); };
-  switch (t.BN * 2 + (split ? 1 : 0)) {
+  if (t.stage_out) launch(conv_tc_kernel<256, false, true>);
+  else switch (t.BN * 2 + (split ? 1 : 0)) {
     case 64: launch(conv_tc_kernel<32, false>); break;
     case 65: launch(conv_tc_kernel<32, true>); break;
     case 128: launch(conv_tc_kernel<64, false>); break;

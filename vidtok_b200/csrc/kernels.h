@@ -140,6 +140,7 @@ struct TcPlan {
   ConvP p;
   DType tout;
   int w_batches, BN, BW, BH, BT, halo, hP, a_stages, stages, kparts, res_mma, ident_s;
+  int stage_out;                 // bf16 output tiles leave through shared-memory staging buffers and bulk tensor stores
   uint32_t halo_bytes, misc_off;
   size_t smem;
   TcLnFusion ln;                 // the requested epilogues that are taken (mode 0 otherwise)

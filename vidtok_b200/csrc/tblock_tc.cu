@@ -211,7 +211,7 @@ __global__ void __launch_bounds__(kThreadsTb, 1) tblock_tc_kernel(const __grid_c
   auto slot_of = [&](int tv) { return h_base + (uint32_t)((tv + kHSlots) % kHSlots) * kKc * kTile; };
   // 16-byte unit (8 channels from c) of ring row `row` in the canonical K-major SWIZZLE_128B layout
   auto ring_unit = [&](uint32_t slot, int row, int c) {
-    return reinterpret_cast<uint4*>(smem_gen + (slot - smem_base) + (c >> 6) * kTile + row * 128 + ((((c & 63) >> 3) ^ (row & 7)) << 4));
+    return reinterpret_cast<uint4*>(smem_gen + (slot - smem_base) + (c >> 6) * kTile + swz128_unit(row, (c & 63) >> 3));
   };
 
   for (long long strip = blockIdx.x; strip < p.num_strips; strip += gridDim.x) {
@@ -286,7 +286,7 @@ __global__ void __launch_bounds__(kThreadsTb, 1) tblock_tc_kernel(const __grid_c
         const float rstd = rsqrtf(var + 1e-6f);
         const float nmr = -mean * rstd;
         const int row = rbase + 8 * r;
-        uint8_t* hrow = smem_gen + (slot - smem_base) + row * 128;
+        uint8_t* hslot = smem_gen + (slot - smem_base);
 #pragma unroll
         for (int j = 0; j < kC / 8; ++j) {
           const int c = 8 * j + cq;
@@ -294,9 +294,8 @@ __global__ void __launch_bounds__(kThreadsTb, 1) tblock_tc_kernel(const __grid_c
           float y1 = fmaf(fmaf(acc[4 * j + 2 * r + 1], rstd, nmr), g2[c + 1], b2[c + 1]);
           y0 = fmaf(y0, tanh_approx(y0), y0);
           y1 = fmaf(y1, tanh_approx(y1), y1);
-          // canonical K-major SWIZZLE_128B: 16-byte unit u of row r lives at unit u ^ (r & 7)
-          const int cc = c & 63, u = cc >> 3;
-          *reinterpret_cast<uint32_t*>(hrow + (c >> 6) * kTile + ((u ^ (row & 7)) << 4) + (cc & 7) * 2) = pack_bf16x2(y0, y1);
+          const int cc = c & 63;
+          *reinterpret_cast<uint32_t*>(hslot + (c >> 6) * kTile + swz128_unit(row, cc >> 3) + (cc & 7) * 2) = pack_bf16x2(y0, y1);
         }
       }
       fence_async_smem();
@@ -326,13 +325,13 @@ __global__ void __launch_bounds__(kThreadsTb, 1) tblock_tc_kernel(const __grid_c
       for (int r = 0; r < 2; ++r) {
         const long long off = (pos0[r] + (long long)t * frame) * kC;
         const int row = rbase + 8 * r;
-        uint8_t* xrow = smem_gen + (xslot - smem_base) + row * 128;
+        uint8_t* xs = smem_gen + (xslot - smem_base);
         float s = 0.f, q = 0.f;
 #pragma unroll
         for (int j = 0; j < kC / 8; ++j) {
           const int c = 8 * j + cq;
-          const int cc = c & 63, u = cc >> 3;
-          uint32_t* xo = reinterpret_cast<uint32_t*>(xrow + (c >> 6) * kTile + ((u ^ (row & 7)) << 4) + (cc & 7) * 2);
+          const int cc = c & 63;
+          uint32_t* xo = reinterpret_cast<uint32_t*>(xs + (c >> 6) * kTile + swz128_unit(row, cc >> 3) + (cc & 7) * 2);
           const uint32_t xw = *xo;
           const float f0 = acc[4 * j + 2 * r] + bias2[c] + bf16_lo(xw), f1 = acc[4 * j + 2 * r + 1] + bias2[c + 1] + bf16_hi(xw);
           s += f0 + f1;

@@ -120,6 +120,10 @@ __device__ __forceinline__ void acc_fence(float (&d)[R]) {
 __device__ __forceinline__ uint32_t desc_lo(uint32_t saddr) { return ((saddr & 0x3FFFFu) >> 4) | (1u << 16); }
 __device__ __forceinline__ uint32_t desc_hi(uint32_t sbo) { return (sbo >> 4) | (1u << 30); }
 __device__ __forceinline__ uint64_t desc(uint32_t lo, uint32_t hi) { return ((uint64_t)hi << 32) | lo; }
+// Byte offset, from the 1024-byte aligned start of a K-major SWIZZLE_128B tile of 128-byte rows, of the 16-byte unit that
+// holds channels [8u, 8u + 8) of row `row`: unit u of a row lives at unit u ^ (row & 7).  What TMA reads and writes and
+// what the descriptors above assume; threads that build or pick apart such a tile themselves address it with this.
+__device__ __forceinline__ uint32_t swz128_unit(int row, int u) { return (uint32_t)row * 128u + (uint32_t)((u ^ (row & 7)) << 4); }
 
 // D[64 x 32] (+)= A[64 x 16] * B[32 x 16]^T, both K-major in shared memory, fp32 accumulators in registers
 __device__ __forceinline__ void wgmma_32_bf16(float (&d)[16], uint64_t da, uint64_t db, uint32_t scale_d) {
