@@ -223,6 +223,29 @@ int32_t vt_video_u8_to_clip_resized(const uint8_t* frames, float* clip, int32_t 
 /* clip: device fp32 [C,T,H,W]; frames: device uint8 [T,H,W,C] = uint8(255 * (clamp(clip,-1,1) + 1) / 2) (tensor_to_uint8). */
 int32_t vt_clip_to_video_u8(const float* clip, uint8_t* frames, int32_t C, int32_t T, int32_t H, int32_t W, void* stream);
 
+/* ---- scoring a reconstruction (scripts/inference_evaluate.py:175-186 with compute_psnr / compute_ssim,
+ *      vidtok/modules/util.py:146-231): clamp to [-1,1], (v+1)/2, then per frame PSNR = -10 log10(mean squared error over
+ *      C x H x W + 1e-8) and SSIM = mean over channels of the mean SSIM map (frames average-pooled by
+ *      max(1, round(min(H,W)/256)) first, round half to even; 11 x 11 Gaussian window, sigma 1.5, no padding; c1 = 1e-4,
+ *      c2 = 9e-4), in one pass over the two clips.  The mean of the per-frame values over a video equals the script's mean
+ *      over its groups of 16 frames, each group value repeated once per frame.  The script clamps only the reconstruction;
+ *      here x is clamped as well, which changes nothing for an input clip in [-1,1].  Every sum runs in a fixed order:
+ *      repeated calls give the same bits. ---- */
+#define VT_DTYPE_F32 0
+#define VT_DTYPE_BF16 1
+#define VT_DTYPE_F16 2
+/* bytes of workspace for one call at this geometry; -1 (and a message) for an empty shape or more tiles than one launch holds */
+int64_t vt_frame_scores_workspace_bytes(int32_t B, int32_t C, int32_t T, int32_t H, int32_t W);
+/* x (the input clip) and y (the reconstruction, not yet clamped): device, dense [B,C,T,H,W], each VT_DTYPE_*; a batch of
+ * frames [N,C,H,W] is B = N, T = 1.  psnr, ssim: device fp32 [B*T], frame (b, t) at b*T + t.  ssim may be NULL (PSNR only);
+ * otherwise the pooled frame must be at least 11 x 11 (VT_ERR_INVALID, as the reference raises ValueError).  running (device,
+ * may be NULL): three doubles that receive += (sum of this call's PSNR values, sum of its SSIM values when ssim is given,
+ * B*T), added frame by frame in order, so a video scored in several calls on one stream needs no host synchronisation
+ * and accumulates the same bits as one call. */
+int32_t vt_frame_scores(const void* x, int32_t x_dtype, const void* y, int32_t y_dtype, int32_t B, int32_t C, int32_t T, int32_t H,
+                        int32_t W, float* psnr, float* ssim, double* running, void* workspace, int64_t workspace_bytes,
+                        void* stream);
+
 /* ---- single operators, exposed for the parity tests (same kernels the model path launches) ---- */
 typedef struct vt_conv_desc {
   int32_t B, Ti, Hi, Wi, Ci;        /* input, channels-last [B,Ti,Hi,Wi,Ci] */

@@ -9,6 +9,7 @@ VT_MAX_LEVELS = 8
 # include/vidtok_b200.h: FMA32 (fp32 FMA kernels), BF16 (wgmma), EXACT_TC (fp16 hi|lo split operands, 3 MMAs per K step, on wgmma), MIXED
 PREC_FMA32, PREC_BF16, PREC_EXACT_TC, PREC_MIXED = 0, 1, 2, 3
 PREC_EXACT = PREC_EXACT_TC  # the parity mode
+DTYPE_F32, DTYPE_BF16, DTYPE_F16 = 0, 1, 2   # VT_DTYPE_*
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libvidtok_b200.so")
 
@@ -74,6 +75,8 @@ _SIGS = {
     "vt_video_u8_to_clip": (_I32, [_P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P]),
     "vt_video_u8_to_clip_resized": (_I32, [_P, _P] + [_I32] * 11 + [_P]),
     "vt_clip_to_video_u8": (_I32, [_P, _P, _I32, _I32, _I32, _I32, _P]),
+    "vt_frame_scores_workspace_bytes": (_I64, [_I32] * 5),
+    "vt_frame_scores": (_I32, [_P, _I32, _P, _I32] + [_I32] * 5 + [_P, _P, _P, _P, _I64, _P]),
     "vt_op_conv": (_I32, [_I32, _I32, C.POINTER(ConvDesc), _P, _P, _P, _P, _P, _P]),
     "vt_op_conv_ex": (_I32, [_I32, C.POINTER(ConvEx), _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "vt_op_conv_regularize": (_I32, [_I32, C.POINTER(ConvDesc), _P, _P, _P, _I32, _I32, C.POINTER(_I32), _P, _P, _P, _P, _P, _P]),

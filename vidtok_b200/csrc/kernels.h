@@ -108,6 +108,14 @@ cudaError_t launch_clip_to_u8_frames(const float* src, uint8_t* dst, int C, int 
 bool u8_frames_resize_fits(int Hs, int Ws, int C, int Hr, int Wr, int h0, int w0, int H, int W);
 cudaError_t launch_u8_frames_resize_to_clip(const uint8_t* src, float* dst, int N, int Hs, int Ws, int C, int Hr, int Wr, int h0,
                                             int w0, int H, int W, int Tc, cudaStream_t s);
+// metrics.cu: per-frame PSNR and SSIM of y against x, both [B,C,T,H,W] in [-1,1] before the clamp (dtype 0 fp32, 1 bf16,
+// 2 fp16 = VT_DTYPE_*).  psnr / ssim fp32 [B*T] (ssim may be null: PSNR only); running (may be null) double [3] receives
+// += (sum of PSNR, sum of SSIM, frames).  ws: frame_scores_workspace bytes (-1: more tiles than one grid holds).
+int frame_scores_pool_factor(int H, int W);   // max(1, round(min(H, W) / 256)), half to even
+bool frame_scores_has_ssim(int H, int W);     // the pooled frame holds at least one 11 x 11 window
+long long frame_scores_workspace(int B, int C, int T, int H, int W);
+cudaError_t launch_frame_scores(const void* x, int x_dtype, const void* y, int y_dtype, int B, int C, int T, int H, int W, float* psnr,
+                                float* ssim, double* running, void* ws, cudaStream_t s);
 // hi|lo split rows [rows][hi(C) | lo(C)] <-> fp32 rows [rows][C]
 cudaError_t launch_split_to_f32(const bf16* x, float* y, long long rows, int C, cudaStream_t s);
 cudaError_t launch_f32_to_split(const float* x, bf16* y, long long rows, int C, cudaStream_t s);

@@ -2642,6 +2642,30 @@ int32_t vt_clip_to_video_u8(const float* clip, uint8_t* frames, int32_t C, int32
   return VT_OK;
 }
 
+// ---- scoring a reconstruction ---------------------------------------------------------------------------
+int64_t vt_frame_scores_workspace_bytes(int32_t B, int32_t C, int32_t T, int32_t H, int32_t W) {
+  if (B <= 0 || C <= 0 || T <= 0 || H <= 0 || W <= 0) { fail(VT_ERR_INVALID, "bad shape"); return -1; }
+  const long long b = frame_scores_workspace(B, C, T, H, W);
+  if (b < 0) fail(VT_ERR_INVALID, "frame scores: %d x %d x %d frames of %d x %d are more tiles than one launch holds; split the batch", B, C, T, H, W);
+  return b;
+}
+int32_t vt_frame_scores(const void* x, int32_t x_dtype, const void* y, int32_t y_dtype, int32_t B, int32_t C, int32_t T, int32_t H,
+                        int32_t W, float* psnr, float* ssim, double* running, void* workspace, int64_t workspace_bytes, void* stream) {
+  if (!x || !y || !psnr || !workspace) return fail(VT_ERR_INVALID, "null argument");
+  if (x_dtype < VT_DTYPE_F32 || x_dtype > VT_DTYPE_F16 || y_dtype < VT_DTYPE_F32 || y_dtype > VT_DTYPE_F16)
+    return fail(VT_ERR_INVALID, "unknown dtype (x %d, y %d): VT_DTYPE_F32, VT_DTYPE_BF16 or VT_DTYPE_F16", x_dtype, y_dtype);
+  const int64_t need = vt_frame_scores_workspace_bytes(B, C, T, H, W);
+  if (need < 0) return VT_ERR_INVALID;
+  if (ssim && !frame_scores_has_ssim(H, W)) {
+    const int f = frame_scores_pool_factor(H, W);
+    return fail(VT_ERR_INVALID, "SSIM kernel size can't be greater than actual input size. Input size: %d x %d (%d x %d pooled by %d). "
+                "Kernel size: 11 x 11", H / f, W / f, H, W, f);
+  }
+  if (workspace_bytes < need) return fail(VT_ERR_WORKSPACE, "workspace too small for the frame scores: %lld < %lld bytes", (long long)workspace_bytes, (long long)need);
+  VT_CUDA(launch_frame_scores(x, x_dtype, y, y_dtype, B, C, T, H, W, psnr, ssim, running, workspace, (cudaStream_t)stream));
+  return VT_OK;
+}
+
 int32_t vt_op_fsq(const float* h, int32_t d, const int32_t* levels, int64_t P, int32_t B, float* codes, int32_t* indices,
                   void* stream) {
   VT_CUDA(launch_fsq(h, d, levels, P, B, codes, indices, (cudaStream_t)stream));

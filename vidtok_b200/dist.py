@@ -71,6 +71,21 @@ def global_psnr(partial: torch.Tensor) -> float:
     return float(p[0] / p[1])
 
 
+def score_partial(x: torch.Tensor, y: torch.Tensor) -> torch.Tensor:
+    """This rank's double [sum of frame PSNR, sum of frame SSIM, n_frames] for CUDA tensors [B,C,T,H,W] (or [N,C,H,W]) in
+    [-1,1]: the fused kernel of vidtok_b200.metrics (clamp + (x+1)/2 inside it), no host synchronisation."""
+    from .metrics import Scorer
+    scorer = Scorer()
+    scorer.update(x, y)
+    return scorer.sums()
+
+
+def global_scores(partial: torch.Tensor) -> dict:
+    """{"psnr", "ssim", "frames"} of the partials of score_partial summed over the ranks (one all-reduce of 3 doubles)."""
+    from .metrics import _means
+    return _means(allreduce_sum(partial.clone()))
+
+
 def gather_clips(local: torch.Tensor, counts: List[int]) -> Optional[torch.Tensor]:
     """All-gather of per-rank reconstructions with possibly different clip counts (pads to the max count)."""
     if not (dist.is_initialized() and dist.get_world_size() > 1):
