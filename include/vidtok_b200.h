@@ -246,6 +246,38 @@ int32_t vt_frame_scores(const void* x, int32_t x_dtype, const void* y, int32_t y
                         int32_t W, float* psnr, float* ssim, double* running, void* workspace, int64_t workspace_bytes,
                         void* stream);
 
+/* ---- LPIPS of a reconstruction (vidtok/modules/lpips.py, scripts/inference_evaluate.py:175-186): per frame, the script's
+ *      clamp of the reconstruction, (v+1)/2 then *2-1, LPIPS's ScalingLayer, VGG16 features[0:30] (13 3x3 ReLU convolutions
+ *      and four 2x2 max-pools) and the head of the five taps relu1_2 .. relu5_3 (channel-normalised squared difference,
+ *      lin_k, mean over the tap's H x W, the five layers added).  One handle holds the weights, built like vt_model.  The
+ *      frame pairs run in passes of vt_lpips_pass_frames(H, W) pairs; a frame's value does not depend on the pass or the
+ *      call it falls into, and every sum runs in a fixed order: repeated calls give the same bits. ---- */
+typedef struct vt_lpips_model vt_lpips_model;
+int32_t vt_lpips_create(int32_t device, vt_lpips_model** out);
+void vt_lpips_destroy(vt_lpips_model* h);
+/* The reference's state-dict keys and shapes: net.slice{1..5}.{i}.weight [Co,Ci,3,3] / .bias [Co] for i in 0, 2 | 5, 7 |
+ * 10, 12, 14 | 17, 19, 21 | 24, 26, 28, and lin{0..4}.model.1.weight [1,C,1,1].  The ScalingLayer's constant buffers are not
+ * parameters. */
+int32_t vt_lpips_num_params(const vt_lpips_model* h);
+int32_t vt_lpips_param_info(const vt_lpips_model* h, int32_t index, char* name, int32_t name_cap, int64_t* shape4, int32_t* ndim);
+int32_t vt_lpips_load_param(vt_lpips_model* h, const char* name, const float* data, int64_t numel, int32_t is_device, void* stream);
+/* repacks the convolutions for the kernels (bf16, and the split copy of EXACT_TC); after the last load, before vt_lpips_model */
+int32_t vt_lpips_finalize(vt_lpips_model* h, void* stream);
+/* frame pairs per pass at H x W: 16, or fewer where relu1_2 of a pass (2 images per pair x H x W x 64) would exceed 2^31
+ * elements; 0 when not even one pair fits */
+int32_t vt_lpips_pass_frames(int32_t H, int32_t W);
+/* workspace of vt_lpips for this geometry (one pass: two activation buffers and the heads' partials); -1 and a message for a
+ * geometry vt_lpips refuses */
+int64_t vt_lpips_workspace_bytes(const vt_lpips_model* h, int32_t precision, int32_t B, int32_t C, int32_t T, int32_t H, int32_t W);
+/* x (the input clip) and y (the reconstruction, not yet clamped): device, dense [B,C,T,H,W], each VT_DTYPE_*; frames [N,C,H,W]
+ * are B = N, T = 1.  precision: VT_PREC_BF16 or VT_PREC_EXACT_TC.  C must be 3 and H, W at least 16 (relu5_3 at least 1 x 1);
+ * otherwise VT_ERR_INVALID and nothing is launched.  lpips: device fp32 [B*T]; per_layer (device, may be NULL): fp32
+ * [B*T][5], the five layers' terms; running (device, may be NULL): two doubles that receive += (sum of this call's values,
+ * B*T), frame by frame in order. */
+int32_t vt_lpips(vt_lpips_model* h, int32_t precision, const void* x, int32_t x_dtype, const void* y, int32_t y_dtype, int32_t B, int32_t C,
+                 int32_t T, int32_t H, int32_t W, float* lpips, float* per_layer, double* running, void* workspace,
+                 int64_t workspace_bytes, void* stream);
+
 /* ---- single operators, exposed for the parity tests (same kernels the model path launches) ---- */
 typedef struct vt_conv_desc {
   int32_t B, Ti, Hi, Wi, Ci;        /* input, channels-last [B,Ti,Hi,Wi,Ci] */
@@ -292,6 +324,12 @@ int32_t vt_op_conv_regularize(int32_t precision, const vt_conv_desc* d, const vo
 int32_t vt_op_conv_regularize_ex(int32_t precision, const vt_conv_ex* e, const void* x, const void* cache, const float* w,
                                  const float* bias, int32_t reg_mode, int32_t zc, const int32_t* fsq_levels, const float* noise,
                                  float* h_out, float* z, int32_t* indices, float* kl_loss, void* stream);
+/* A convolution followed by ReLU, as the LPIPS stack runs it (BF16 / EXACT_TC; d->res_mode must be 0).  Operands as vt_op_conv. */
+int32_t vt_op_conv_relu(int32_t precision, const vt_conv_desc* d, const void* x, const float* w, const float* bias, void* out,
+                        void* stream);
+/* 2x2 / stride-2 max-pool (floor) of channels-last x [N,H,W,C] -> y [N,H/2,W/2,C] in the precision's activation type (bf16, or
+ * hi|lo split rows compared as hi + lo); C % 8 == 0. */
+int32_t vt_op_maxpool2x2(int32_t precision, const void* x, void* y, int64_t N, int32_t H, int32_t W, int32_t C, void* stream);
 /* Encoder stem from the caller's fp32 [B,Ci,T,H,W] (t_rep replicated leading frames); out channels-last
  * [B,T+t_rep,H,W,Co] in the precision's activation type (BF16 / EXACT_TC). */
 int32_t vt_op_conv_stem(int32_t precision, const float* x, const float* w, const float* bias, void* out, int32_t B,

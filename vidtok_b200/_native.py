@@ -77,6 +77,17 @@ _SIGS = {
     "vt_clip_to_video_u8": (_I32, [_P, _P, _I32, _I32, _I32, _I32, _P]),
     "vt_frame_scores_workspace_bytes": (_I64, [_I32] * 5),
     "vt_frame_scores": (_I32, [_P, _I32, _P, _I32] + [_I32] * 5 + [_P, _P, _P, _P, _I64, _P]),
+    "vt_lpips_create": (_I32, [_I32, C.POINTER(_P)]),
+    "vt_lpips_destroy": (None, [_P]),
+    "vt_lpips_num_params": (_I32, [_P]),
+    "vt_lpips_param_info": (_I32, [_P, _I32, C.c_char_p, _I32, C.POINTER(_I64), C.POINTER(_I32)]),
+    "vt_lpips_load_param": (_I32, [_P, C.c_char_p, _P, _I64, _I32, _P]),
+    "vt_lpips_finalize": (_I32, [_P, _P]),
+    "vt_lpips_pass_frames": (_I32, [_I32, _I32]),
+    "vt_lpips_workspace_bytes": (_I64, [_P] + [_I32] * 6),
+    "vt_lpips": (_I32, [_P, _I32, _P, _I32, _P, _I32] + [_I32] * 5 + [_P, _P, _P, _P, _I64, _P]),
+    "vt_op_conv_relu": (_I32, [_I32, C.POINTER(ConvDesc), _P, _P, _P, _P, _P]),
+    "vt_op_maxpool2x2": (_I32, [_I32, _P, _P, _I64, _I32, _I32, _I32, _P]),
     "vt_op_conv": (_I32, [_I32, _I32, C.POINTER(ConvDesc), _P, _P, _P, _P, _P, _P]),
     "vt_op_conv_ex": (_I32, [_I32, C.POINTER(ConvEx), _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "vt_op_conv_regularize": (_I32, [_I32, C.POINTER(ConvDesc), _P, _P, _P, _I32, _I32, C.POINTER(_I32), _P, _P, _P, _P, _P, _P]),

@@ -17,7 +17,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libvidtok_b200.so")
-SOURCES = ["conv_simt.cu", "conv_tc.cu", "conv_stem.cu", "tblock_tc.cu", "attn_tc.cu", "elementwise.cu", "fsq_aux.cu", "video_io.cu", "metrics.cu", "model.cu"]
+SOURCES = ["conv_simt.cu", "conv_tc.cu", "conv_stem.cu", "tblock_tc.cu", "attn_tc.cu", "elementwise.cu", "fsq_aux.cu", "video_io.cu", "metrics.cu", "lpips.cu", "model.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v",

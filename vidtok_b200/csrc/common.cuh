@@ -186,6 +186,8 @@ struct ConvP {
   // channel ci of a position is the FSQ code digit ((idx / basis_ci) % L_ci - L_ci/2) / (L_ci/2).  0 = off.
   int fsq_d;
   int fsq_levels[VT_MAX_FSQ];
+  // epilogue: out = max(v, 0) after the bias and residual (the VGG16 feature stack of LPIPS); wgmma path only
+  int relu;
 };
 
 }  // namespace vt

@@ -8,6 +8,7 @@
 // accumulators.  The epilogue adds the bias and writes the bf16 channels-last activation.  The patch loads of tile i+1 are
 // in flight (registers) during the MMAs and the epilogue of tile i.
 #include <cstdio>
+#include <cstring>
 
 #include "common.cuh"
 #include "kernels.h"
@@ -31,6 +32,28 @@ struct StemParams {
   int tilesW, tilesH;
   float acc_scale;   // split: 2^-s of the pre-scaled weights (1 otherwise)
 };
+// LPIPS stem (kLp): a 1x3x3 convolution over To = 2 G images; image f < G is frame n0 + f of the clip x, image G + f the same
+// frame of y, both [Bc,3,Tc,H,W] of dtype VT_DTYPE_* (frame n = b * Tc + t).  A kernel parameter of its own, behind the others,
+// so that the encoder's instantiations keep their parameter layout and code.
+struct LpStemParams {
+  const void* x;
+  const void* y;
+  int x_dt, y_dt, G, Tc;
+  long long n0;
+};
+
+// The LPIPS input of one element: the evaluation script's clamp of the reconstruction (y only), (v + 1) / 2, * 2 - 1, then
+// LPIPS's ScalingLayer (v - shift) / scale, each step rounded in fp32 as torch rounds it (lpips.py:98-105)
+__device__ __forceinline__ float lpips_in(const void* src, int dt, long long i, bool clamp, int c) {
+  float v = dt == 0 ? static_cast<const float*>(src)[i]
+                    : dt == 1 ? __bfloat162float(static_cast<const bf16*>(src)[i]) : __half2float(static_cast<const __half*>(src)[i]);
+  if (clamp) v = fminf(fmaxf(v, -1.0f), 1.0f);
+  v = __fdiv_rn(__fadd_rn(v, 1.0f), 2.0f);
+  v = __fsub_rn(__fmul_rn(v, 2.0f), 1.0f);
+  const float shift = c == 0 ? -0.030f : (c == 1 ? -0.088f : -0.188f);
+  const float scale = c == 0 ? 0.458f : (c == 1 ? 0.448f : 0.450f);
+  return __fdiv_rn(__fsub_rn(v, shift), scale);
+}
 
 constexpr int BW = 16, BH = 8;
 constexpr int PW = BW + 2, PH = BH + 2;
@@ -40,8 +63,10 @@ constexpr int kPatchIt = 9;            // patch values per thread: Ci * 3 * PH *
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 // kSplit (EXACT_TC mode): the im2col rows and the weights are hi|lo fp16 pairs, every K=16 step issues hi*hi + lo*hi +
 // hi*lo into the same accumulator, and the output is written as hi | lo planes ([..., 2*Co]).
-template <int CO, bool kSplit>
-__global__ void __launch_bounds__(256, 1) conv_stem_kernel(const StemParams p, const bf16* __restrict__ wpk /*[Co][128] or [Co][hi 128 | lo 128]*/) {
+// kLp: the LPIPS stem (LpStemParams): one input frame per image, the script's preprocessing while loading, ReLU after the bias.
+template <int CO, bool kSplit, bool kLp = false>
+__global__ void __launch_bounds__(256, 1) conv_stem_kernel(const StemParams p, const bf16* __restrict__ wpk /*[Co][128] or [Co][hi 128 | lo 128]*/,
+                                                           const LpStemParams lp) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* gen = smem_raw + (base - smem_u32(smem_raw));
@@ -49,14 +74,15 @@ __global__ void __launch_bounds__(256, 1) conv_stem_kernel(const StemParams p, c
   // layout: A[planes] (32 KB each) | B[planes] (Co x 256 B each) | patch (Ci*3*PH*PW floats) | bias | im2col lut
   const uint32_t offA = 0, offB = kPl * kATile;
   const uint32_t offP = offB + kPl * (uint32_t)CO * 256u;
-  const uint32_t patch_floats = (uint32_t)p.Ci * 3 * PH * PW;
+  constexpr int kTimeTaps = kLp ? 1 : 3;
+  const uint32_t patch_floats = (uint32_t)p.Ci * kTimeTaps * PH * PW;
   const uint32_t offBias = offP + ((patch_floats * 4 + 15) & ~15u);
   const uint32_t offLut = offBias + 256 * 4;   // im2col k -> patch offset (or -1)
   float* patch = reinterpret_cast<float*>(gen + offP);
   float* sbias = reinterpret_cast<float*>(gen + offBias);
   int* lut = reinterpret_cast<int*>(gen + offLut);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int K = p.Ci * 27;
+  const int K = p.Ci * 9 * kTimeTaps;
   const int units = (K + 7) / 8;  // 16-byte units of real data per im2col row (11 for Ci = 3)
 
   // ---- one-time setup: zero the A tile, stage weights (swizzled) and bias
@@ -73,7 +99,7 @@ __global__ void __launch_bounds__(256, 1) conv_stem_kernel(const StemParams p, c
     if (tid < K) {
       const int ci = tid % p.Ci, tap = tid / p.Ci;
       const int c = tap % 3, bb = (tap / 3) % 3, a = tap / 9;
-      off = ((ci * 3 + a) * PH + bb) * PW + c;
+      off = ((ci * kTimeTaps + a) * PH + bb) * PW + c;
     }
     lut[tid] = off;
   }
@@ -95,6 +121,26 @@ __global__ void __launch_bounds__(256, 1) conv_stem_kernel(const StemParams p, c
   auto load_patch = [&](long long tile, float (&pv)[kPatchIt]) {
     int b, t, h0, w0;
     decode(tile, b, t, h0, w0);
+    if constexpr (kLp) {
+      // image t of the pass: x or y, frame n0 + t % G of the clip; zero padding outside the frame (after the scaling)
+      const bool from_y = t >= lp.G;
+      const long long n = lp.n0 + (from_y ? t - lp.G : t);
+      const long long fb = (n / lp.Tc) * 3 * lp.Tc + n % lp.Tc;   // (b * 3 + 0) * Tc + t
+      const long long plane = (long long)lp.Tc * p.H * p.W;
+#pragma unroll
+      for (int k = 0; k < kPatchIt; ++k) {
+        const uint32_t i = (uint32_t)tid + (uint32_t)k * 256u;
+        float v = 0.f;
+        if (i < patch_floats) {
+          const int ww = i % PW, hh = (i / PW) % PH, ci = i / (PW * PH);
+          const int hv = h0 + hh - 1, wv = w0 + ww - 1;
+          if (hv >= 0 && hv < p.H && wv >= 0 && wv < p.W)
+            v = lpips_in(from_y ? lp.y : lp.x, from_y ? lp.y_dt : lp.x_dt, fb * p.H * p.W + ci * plane + (long long)hv * p.W + wv, from_y, ci);
+        }
+        pv[k] = v;
+      }
+      return;
+    }
 #pragma unroll
     for (int k = 0; k < kPatchIt; ++k) {
       const uint32_t i = (uint32_t)tid + (uint32_t)k * 256u;
@@ -200,7 +246,20 @@ __global__ void __launch_bounds__(256, 1) conv_stem_kernel(const StemParams p, c
 #pragma unroll
       for (int j = 0; j < CO / 8; ++j) {
         const int c = 8 * j + cq;
-        if constexpr (kSplit) {
+        if constexpr (kLp) {
+          float f0 = kSplit ? fmaf(acc[4 * j + 2 * r], p.acc_scale, sbias[c]) : acc[4 * j + 2 * r] + sbias[c];
+          float f1 = kSplit ? fmaf(acc[4 * j + 2 * r + 1], p.acc_scale, sbias[c + 1]) : acc[4 * j + 2 * r + 1] + sbias[c + 1];
+          f0 = f0 < 0.f ? 0.f : f0;
+          f1 = f1 < 0.f ? 0.f : f1;
+          if constexpr (kSplit) {
+            const __half2 h2 = __floats2half2_rn(split_sat(f0), split_sat(f1));
+            const float2 hf = __half22float2(h2);
+            *reinterpret_cast<__half2*>(orow + c) = h2;
+            *reinterpret_cast<__half2*>(orow + CO + c) = __floats2half2_rn(split_sat(f0 - hf.x), split_sat(f1 - hf.y));
+          } else {
+            *reinterpret_cast<__nv_bfloat162*>(orow + c) = __floats2bfloat162_rn(f0, f1);
+          }
+        } else if constexpr (kSplit) {
           const float f0 = fmaf(acc[4 * j + 2 * r], p.acc_scale, sbias[c]);
           const float f1 = fmaf(acc[4 * j + 2 * r + 1], p.acc_scale, sbias[c + 1]);
           const __half2 h2 = __floats2half2_rn(split_sat(f0), split_sat(f1));
@@ -316,12 +375,50 @@ cudaError_t launch_conv_stem(const ConvP& p, const float* x, const bf16* wpk, bf
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 256, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
     const long long slots = (long long)per_sm * num_sms;
     const unsigned grid = (unsigned)(t.num_tiles < slots ? t.num_tiles : slots);
-    kern<<<grid, 256, smem, s>>>(t, wpk);
+    kern<<<grid, 256, smem, s>>>(t, wpk, LpStemParams());
     return cudaSuccess;
   };
   cudaError_t e;
   if (p.split) e = p.Co == 64 ? launch(conv_stem_kernel<64, true>) : launch(conv_stem_kernel<128, true>);
   else e = p.Co == 64 ? launch(conv_stem_kernel<64, false>) : p.Co == 128 ? launch(conv_stem_kernel<128, false>) : launch(conv_stem_kernel<256, false>);
+  if (e != cudaSuccess) return e;
+  count_launch();
+  return cudaGetLastError();
+}
+
+cudaError_t launch_lpips_stem(const void* x, int x_dtype, const void* y, int y_dtype, int Tc, long long n0, int G, int H, int W,
+                              bool split, const bf16* wpk, const float* bias, float acc_scale, bf16* out, cudaStream_t s) {
+  StemParams t;
+  memset(&t, 0, sizeof(t));
+  LpStemParams lp;
+  lp.x = x; lp.y = y; lp.x_dt = x_dtype; lp.y_dt = y_dtype; lp.Tc = Tc; lp.n0 = n0; lp.G = G;
+  t.B = 1; t.Ci = 3; t.T = 2 * G; t.H = H; t.W = W; t.To = 2 * G;
+  t.Co = 64; t.bias = bias; t.out = out;
+  t.acc_scale = split ? acc_scale : 1.0f;
+  t.tilesW = (W + BW - 1) / BW; t.tilesH = (H + BH - 1) / BH;
+  t.num_tiles = (long long)t.To * t.tilesH * t.tilesW;
+  const size_t pl = split ? 2 : 1;
+  const size_t smem = 1024 + pl * kATile + pl * 64 * 256 + (((size_t)3 * PH * PW * 4 + 15) & ~(size_t)15) + 256 * 4 + 128 * 4;
+  int dev = 0;
+  const cudaError_t dev_err = current_device(dev);
+  if (dev_err != cudaSuccess) return dev_err;
+  const int num_sms = device_sms(dev);
+  const double M = (double)2 * G * H * W;
+  auto esz = [](int dt) { return dt == 0 ? 4.0 : 2.0; };
+  char det[96] = "";
+  if (prof_enabled()) snprintf(det, sizeof(det), "k133 3->64 @%dx%dx%d%s", 2 * G, H, W, split ? " split" : "");
+  ProfScope _ps("lpips_stem", 2.0 * M * 27 * 64, (double)G * 3 * H * W * (esz(x_dtype) + esz(y_dtype)) + M * 64 * 2.0 * pl, s, det);
+  auto launch = [&](auto kern) -> cudaError_t {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    int per_sm = 1;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 256, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
+    const long long slots = (long long)per_sm * num_sms;
+    const unsigned grid = (unsigned)(t.num_tiles < slots ? t.num_tiles : slots);
+    kern<<<grid, 256, smem, s>>>(t, wpk, lp);
+    return cudaSuccess;
+  };
+  cudaError_t e = split ? launch(conv_stem_kernel<64, true, true>) : launch(conv_stem_kernel<64, false, true>);
   if (e != cudaSuccess) return e;
   count_launch();
   return cudaGetLastError();

@@ -108,6 +108,7 @@ struct TcParams {
   uint32_t stage_smem;       // bytes of the staging buffers between the stage ring and the barriers (0: none in the plan)
   uint32_t stage_off;        // their byte offset from the aligned base
   int half_dim, half_ext;
+  int relu;                  // ConvP::relu: a uniform flag, applied to the fp32 values before any store
 };
 
 struct TcMaps {
@@ -602,6 +603,11 @@ conv_tc_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
           }
         }
       }
+      if (p.relu) {
+        // (v < 0 ? 0 : v keeps a NaN, as torch's ReLU does)
+#pragma unroll
+        for (int i = 0; i < R; ++i) acc_h[i] = acc_h[i] < 0.f ? 0.f : acc_h[i];
+      }
 
       if (p.out_f32) {
         // external fp32 heads / attention scores: direct stores, only the real output channels
@@ -917,6 +923,7 @@ bool conv_tc_plan(const ConvP& p, DType tout, const TcLnFusion* ln, const TcRegF
   if (p.t_mode == 2 && p.sh != 1) return no("cache mode with spatial stride");
   if (p.Wi > 65535 || p.Hi > 65535) return no("extent");
   if (w_batches > 1 && w_batches != p.B) return no("batched weights need one weight matrix per batch element");
+  if (p.relu && ((ln && ln->mode) || (reg && reg->mode))) return no("ReLU with a fused LayerNorm or regularizer epilogue");
   TcPlan t = TcPlan();
   t.p = p; t.tout = tout; t.w_batches = w_batches;
   const int nk = p.kt * p.kh * p.kw * (p.Ci / 64);   // K steps
@@ -1048,6 +1055,7 @@ cudaError_t launch_conv_tc(const TcPlan& pl, const bf16* x, const bf16* w_nk, vo
     if (reg.mode == 2) t.reg_fsq = make_fsq_const(reg.zc, reg.fsq_levels);
   }
   t.w_batched = pl.w_batches > 1 ? 1 : 0;
+  t.relu = p.relu ? 1 : 0;
 
   TcMaps maps;
   // activation view: element (c, w, h, t, b) at base + c + w*sw_ + h*sh_ + t*isT + b*bs  (elements)
@@ -1137,9 +1145,10 @@ cudaError_t launch_conv_tc(const TcPlan& pl, const bf16* x, const bf16* w_nk, vo
   const unsigned grid = (unsigned)(t.num_tiles < num_sms ? t.num_tiles : num_sms);
   const double Mrows = (double)p.B * p.To * p.Ho * p.Wo;
   // plan key of the launch (profiler detail): geometry, tile, N tile, halo windows, fused LayerNorm, residual mode (m: through
-  // the MMA), kparts, time padding (t0 zeros / t1 replicate / t2 cache) and pipeline stages
+  // the MMA), kparts, time padding (t0 zeros / t1 replicate / t2 cache) and pipeline stages; " relu" only when ReLU is on, so
+  // the keys of every other plan stay as they were
   char det[160] = "";
-  if (prof_enabled()) snprintf(det, sizeof(det), "k%d%d%d s%d%d %d->%d @%dx%dx%d tile%dx%dx%d bn%d%s ln%d r%d%s p%d t%d st%d", p.kt, p.kh, p.kw, p.st, p.sh, p.Ci, p.Co, p.To, p.Ho, p.Wo, t.BT, t.BH, t.BW, t.BN, t.halo ? " halo" : "", t.ln_mode, p.res_mode, t.res_mma ? "m" : "", split ? t.kparts : 1, p.t_mode, t.stages);
+  if (prof_enabled()) snprintf(det, sizeof(det), "k%d%d%d s%d%d %d->%d @%dx%dx%d tile%dx%dx%d bn%d%s ln%d r%d%s p%d t%d st%d%s", p.kt, p.kh, p.kw, p.st, p.sh, p.Ci, p.Co, p.To, p.Ho, p.Wo, t.BT, t.BH, t.BW, t.BN, t.halo ? " halo" : "", t.ln_mode, p.res_mode, t.res_mma ? "m" : "", split ? t.kparts : 1, p.t_mode, t.stages, p.relu ? " relu" : "");
   ProfScope _ps(split ? "conv_tc3" : "conv_tc", 2.0 * Mrows * p.kt * p.kh * p.kw * p.Ci * p.Co,
                 2.0 * cw * ((double)p.B * p.Ti * p.Hi * p.Wi * p.Ci) + Mrows * p.Co * (pl.tout == DT_F32 ? 4.0 : 2.0 * cw), s, det);
   auto launch = [&](auto kern) { kern<<<grid, kThreads, pl.smem, s>>>(maps, t); };

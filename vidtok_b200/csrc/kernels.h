@@ -201,5 +201,28 @@ const char* attn_tc_last_error();
 bool conv_stem_supported(const ConvP& p);
 cudaError_t launch_conv_stem(const ConvP& p, const float* x, const bf16* wpk, bf16* out, cudaStream_t s);
 cudaError_t launch_stem_cache_update(const float* x, float* cache, int B, int Ci, int T, int t_rep, int H, int W, cudaStream_t s);
+// LPIPS stem: conv1_1 (3 -> 64, 1x3x3, ReLU) of 2 G images, frames [n0, n0 + G) of x then of y ([Bc,3,Tc,H,W], VT_DTYPE_*),
+// with the evaluation script's preprocessing and LPIPS's ScalingLayer applied while loading; out channels-last [2G,H,W,64]
+// (split: [2G,H,W,hi 64 | lo 64]); wpk as for launch_conv_stem (Kpad = 128, 9 taps)
+cudaError_t launch_lpips_stem(const void* x, int x_dtype, const void* y, int y_dtype, int Tc, long long n0, int G, int H, int W,
+                              bool split, const bf16* wpk, const float* bias, float acc_scale, bf16* out, cudaStream_t s);
+
+// lpips.cu: the pooling and the per-position head of LPIPS (vidtok/modules/lpips.py) on channels-last features
+// 2x2 / stride-2 max-pool (floor) of [N,H,W,C] (split: [N,H,W,hi C | lo C], compared as hi + lo) -> [N,H/2,W/2,C]
+cudaError_t launch_maxpool2x2(const bf16* x, bf16* y, long long N, int H, int W, int C, bool split, cudaStream_t s);
+// positions of one head tile, and the tiles of an H x W feature map
+constexpr int kLpipsHeadPos = 64;
+inline long long lpips_head_tiles(int H, int W) { return ((long long)H * W + kLpipsHeadPos - 1) / kLpipsHeadPos; }
+// f [2G,H,W,C]: images [0,G) against [G,2G); part[g * tiles + tile] = sum over the tile's positions of
+// sum_c w[c] (f_x / (|f_x| + 1e-10) - f_y / (|f_y| + 1e-10))^2, in fp32
+cudaError_t launch_lpips_head(const bf16* f, int G, int H, int W, int C, bool split, const float* w, float* part, cudaStream_t s);
+// per image g < G: layer k's partials (tiles[k] each, part + off[k]) added in order in double, / (H_k W_k), the five layers
+// added in order; lpips[g] (fp32), per_layer[g][5] (may be null); running (may be null) += (sum of lpips[0..G), G)
+struct LpipsFinish {
+  long long off[5], tiles[5];
+  double area[5];
+};
+cudaError_t launch_lpips_finish(const float* part, const LpipsFinish& f, int G, float* lpips, float* per_layer, double* running,
+                                cudaStream_t s);
 
 }  // namespace vt

@@ -2270,7 +2270,8 @@ static int op_weight_scale(const float* w, long long n, float headroom, cudaStre
 // precision, with temporary weight repacks.
 static int op_conv_impl(int precision, int force_simt, const vt_conv_desc* d, const vt_conv_ex* e, const void* x,
                         const void* cache, const float* w, const float* bias, const void* res, const float* gamma,
-                        const float* beta, void* out, void* out2, cudaStream_t s, const TcRegFusion* reg = nullptr) {
+                        const float* beta, void* out, void* out2, cudaStream_t s, const TcRegFusion* reg = nullptr,
+                        bool relu = false) {
   if (!d || !x || !w || (!out && !reg)) return fail(VT_ERR_INVALID, "null argument");
   if (precision != VT_PREC_FMA32 && precision != VT_PREC_BF16 && precision != VT_PREC_EXACT_TC)
     return fail(VT_ERR_INVALID, "operator precision must be FMA32, BF16 or EXACT_TC");
@@ -2293,6 +2294,7 @@ static int op_conv_impl(int precision, int force_simt, const vt_conv_desc* d, co
     p.t_mode = e->t_mode; p.cache = cache; p.cacheT = e->cacheT;
   }
   p.bias = bias;
+  p.relu = relu ? 1 : 0;
   p.res_mode = d->res_mode;
   p.res = res;
   if (d->res_mode && !res) return fail(VT_ERR_INVALID, "residual mode without residual tensor");
@@ -2322,6 +2324,7 @@ static int op_conv_impl(int precision, int force_simt, const vt_conv_desc* d, co
   bf16* wnk = nullptr;
   cudaError_t er;
   const bool want_tc = precision != VT_PREC_FMA32 && !force_simt;
+  if (relu && !want_tc) return fail(VT_ERR_INVALID, "the ReLU epilogue exists on the wgmma path only");
   if (want_tc) {
     float wsc = 0.f;
     if (ta == DT_SPLIT) {
@@ -2714,6 +2717,307 @@ int32_t vt_op_kl(const float* h, const float* noise, int32_t zc, int64_t P, int3
   cudaStreamSynchronize((cudaStream_t)stream);
   cudaFree(scratch);
   if (e != cudaSuccess) return fail(VT_ERR_CUDA, "kl: %s", cudaGetErrorString(e));
+  return VT_OK;
+}
+
+
+// ---- LPIPS (vidtok/modules/lpips.py; scripts/inference_evaluate.py:175-186) --------------------------------------------
+// VGG16 features[0:30] as 13 ReLU convolutions (conv1_1 on the LPIPS stem, the rest on conv_tc), four 2x2 max-pools, and the
+// head of each of the five taps, walked over the frame pairs in passes of at most lpips_pass_frames() pairs.  Image f < g of a
+// pass is frame n0 + f of x, image g + f the same frame of y, so each layer runs both images in one launch.
+}  // extern "C"
+namespace {
+struct LpipsConv { int Ci, Co, pw, pb; };
+// the reference's state-dict indices of the 13 convolutions, their slices and channels; taps after conv 1, 3, 6, 9, 12, a
+// max-pool in front of conv 2, 4, 7, 10
+constexpr int kLpConvIdx[13] = {0, 2, 5, 7, 10, 12, 14, 17, 19, 21, 24, 26, 28};
+constexpr int kLpSlice[13] = {1, 1, 2, 2, 3, 3, 3, 4, 4, 4, 5, 5, 5};
+constexpr int kLpCo[13] = {64, 64, 128, 128, 256, 256, 256, 512, 512, 512, 512, 512, 512};
+constexpr int kLpChns[5] = {64, 128, 256, 512, 512};
+inline bool lp_tap(int i) { return i == 1 || i == 3 || i == 6 || i == 9 || i == 12; }
+inline bool lp_pool_before(int i) { return i == 2 || i == 4 || i == 7 || i == 10; }
+// 2^31: the kernels are not audited for activations of more elements (DESIGN.md section 6)
+constexpr long long kLpMaxElems = 1LL << 31;
+}  // namespace
+
+struct vt_lpips_model {
+  int device = 0;
+  std::vector<vt::Param> params;
+  std::map<std::string, int> index;
+  float* pool = nullptr;
+  int64_t pool_elems = 0;
+  bool finalized = false;
+  vt::bf16* packed = nullptr;          // every conv's bf16 [Co][Kpad], then its split copy [Co][hi Kpad | lo Kpad]
+  LpipsConv conv[13];
+  vt::bf16* w[13] = {nullptr};
+  vt::bf16* w3[13] = {nullptr};
+  float wscale3[13] = {0.f};
+  int plin[5] = {0};
+};
+
+extern "C" {
+
+// frame pairs of one pass: 16, or fewer where relu1_2 of the pass (2 g images x H x W x 64) would exceed 2^31 elements;
+// 0 when not even one pair fits
+static int lpips_pass_frames(int H, int W) {
+  const long long per = 2LL * H * W * 64;
+  int g = 16;
+  while (g > 0 && g * per > kLpMaxElems) --g;
+  return g;
+}
+// the spatial extents of the five levels (floor halving)
+static void lpips_levels(int H, int W, int (&Hl)[5], int (&Wl)[5]) {
+  Hl[0] = H; Wl[0] = W;
+  for (int l = 1; l < 5; ++l) { Hl[l] = Hl[l - 1] / 2; Wl[l] = Wl[l - 1] / 2; }
+}
+struct LpipsLayout {
+  int G, Hl[5], Wl[5];
+  size_t act_bytes, part_bytes;
+};
+static int lpips_check(int precision, int B, int C, int T, int H, int W, LpipsLayout* L) {
+  if (precision != VT_PREC_BF16 && precision != VT_PREC_EXACT_TC) return fail(VT_ERR_INVALID, "LPIPS runs in BF16 or EXACT_TC, got precision %d", precision);
+  if (C != 3) return fail(VT_ERR_INVALID, "LPIPS takes RGB clips (C == 3), got C = %d", C);
+  if (B <= 0 || T <= 0) return fail(VT_ERR_INVALID, "empty clip (B = %d, T = %d)", B, T);
+  if (H < 16 || W < 16) return fail(VT_ERR_INVALID, "frames of %d x %d are smaller than 16 x 16, where relu5_3 is 1 x 1", H, W);
+  const int Gmax = lpips_pass_frames(H, W);
+  if (Gmax < 1) return fail(VT_ERR_INVALID, "frames of %d x %d give activations beyond 2^31 elements", H, W);
+  const long long frames = (long long)B * T;
+  L->G = (int)(frames < Gmax ? frames : Gmax);
+  lpips_levels(H, W, L->Hl, L->Wl);
+  const size_t esz = precision == VT_PREC_EXACT_TC ? 4 : 2;
+  L->act_bytes = align_up((size_t)2 * L->G * H * W * 64 * esz, 1024);
+  long long tiles = 0;
+  for (int k = 0; k < 5; ++k) tiles += lpips_head_tiles(L->Hl[k], L->Wl[k]);
+  L->part_bytes = align_up((size_t)L->G * tiles * sizeof(float), 1024);
+  return VT_OK;
+}
+
+// The conv_tc plan of conv i (i >= 1) for a pass of g pairs at level extent H x W
+static bool lpips_conv_plan(const vt_lpips_model* h, int i, int g, int H, int W, bool split, TcPlan* pl) {
+  const LpipsConv& c = h->conv[i];
+  const long long cw = split ? 2 : 1;
+  ConvP p = conv_p(2 * g, 1, H, W, c.Ci);
+  p.split = split ? 1 : 0;
+  set_in(p, cl_strides(1, H, W, c.Ci, cw));
+  p.kt = 1; p.kh = p.kw = 3; p.ph = p.pw = 1;
+  p.Co = c.Co;
+  conv_out_size(p, 0, 1, 1);
+  set_out(p, cl_strides(1, p.Ho, p.Wo, c.Co, cw));
+  p.bias = h->finalized ? h->pool + h->params[c.pb].offset : nullptr;
+  p.ra = 0.f; p.rb = 1.f;
+  p.relu = 1;
+  p.acc_scale = split ? 1.0f / h->wscale3[i] : 0.f;
+  return conv_tc_plan(p, split ? DT_SPLIT : DT_BF16, nullptr, nullptr, 1, pl);
+}
+
+int32_t vt_lpips_create(int32_t device, vt_lpips_model** out) {
+  if (!out) return fail(VT_ERR_INVALID, "null argument");
+  vt_lpips_model* h = new vt_lpips_model();
+  h->device = device;
+  auto add = [&](const std::string& name, std::vector<int64_t> shape) {
+    Param p;
+    p.name = name;
+    p.shape = shape;
+    p.numel = 1;
+    for (auto d : shape) p.numel *= d;
+    p.offset = h->pool_elems;
+    h->pool_elems += (p.numel + 3) / 4 * 4;
+    h->index[name] = (int)h->params.size();
+    h->params.push_back(p);
+    return (int)h->params.size() - 1;
+  };
+  int Ci = 3;
+  for (int i = 0; i < 13; ++i) {
+    const std::string key = "net.slice" + std::to_string(kLpSlice[i]) + "." + std::to_string(kLpConvIdx[i]);
+    h->conv[i].Ci = Ci;
+    h->conv[i].Co = kLpCo[i];
+    h->conv[i].pw = add(key + ".weight", {kLpCo[i], Ci, 3, 3});
+    h->conv[i].pb = add(key + ".bias", {kLpCo[i]});
+    Ci = kLpCo[i];
+  }
+  for (int k = 0; k < 5; ++k) h->plin[k] = add("lin" + std::to_string(k) + ".model.1.weight", {1, kLpChns[k], 1, 1});
+  *out = h;
+  return VT_OK;
+}
+
+void vt_lpips_destroy(vt_lpips_model* h) {
+  if (!h) return;
+  if (h->pool) cudaFree(h->pool);
+  if (h->packed) cudaFree(h->packed);
+  delete h;
+}
+
+int32_t vt_lpips_num_params(const vt_lpips_model* h) { return h ? (int32_t)h->params.size() : 0; }
+
+int32_t vt_lpips_param_info(const vt_lpips_model* h, int32_t i, char* name, int32_t cap, int64_t* shape4, int32_t* ndim) {
+  if (!h || i < 0 || i >= (int)h->params.size()) return fail(VT_ERR_INVALID, "bad parameter index");
+  const Param& p = h->params[i];
+  if (name && cap > 0) {
+    strncpy(name, p.name.c_str(), cap - 1);
+    name[cap - 1] = 0;
+  }
+  if (ndim) *ndim = (int)p.shape.size();
+  if (shape4)
+    for (size_t k = 0; k < 4; ++k) shape4[k] = k < p.shape.size() ? p.shape[k] : 1;
+  return VT_OK;
+}
+
+static int lpips_device(vt_lpips_model* h) {
+  int n = 0;
+  if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) {
+    cudaGetLastError();
+    return fail(VT_ERR_NO_DEVICE, "no CUDA device visible: vidtok_b200 has no CPU fallback");
+  }
+  VT_CUDA(cudaSetDevice(h->device));
+  if (!h->pool) VT_CUDA(cudaMalloc(&h->pool, (size_t)h->pool_elems * sizeof(float)));
+  return VT_OK;
+}
+
+int32_t vt_lpips_load_param(vt_lpips_model* h, const char* name, const float* data, int64_t numel, int32_t is_device, void* stream) {
+  if (!h || !name || !data) return fail(VT_ERR_INVALID, "null argument");
+  auto it = h->index.find(name);
+  if (it == h->index.end()) return fail(VT_ERR_INVALID, "unknown LPIPS parameter %s", name);
+  Param& p = h->params[it->second];
+  if (p.numel != numel) return fail(VT_ERR_INVALID, "parameter %s: expected %lld elements, got %lld", name, (long long)p.numel, (long long)numel);
+  int rc = lpips_device(h);
+  if (rc) return rc;
+  VT_CUDA(cudaMemcpyAsync(h->pool + p.offset, data, (size_t)numel * sizeof(float), is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice,
+                          (cudaStream_t)stream));
+  p.loaded = true;
+  h->finalized = false;
+  return VT_OK;
+}
+
+// Repacks the convolutions' weights: bf16 [Co][K = tap * Ci + ci] (conv1_1: K padded to 128 for the stem) and the split copy
+// of w * 2^s, s from max |w| of each convolution.
+int32_t vt_lpips_finalize(vt_lpips_model* h, void* stream) {
+  if (!h) return fail(VT_ERR_INVALID, "null argument");
+  for (auto& p : h->params)
+    if (!p.loaded) return fail(VT_ERR_NOT_READY, "LPIPS parameter %s was never loaded", p.name.c_str());
+  int rc = lpips_device(h);
+  if (rc) return rc;
+  cudaStream_t s = (cudaStream_t)stream;
+  auto kpad = [&](int i) { return i == 0 ? 128 : 9 * h->conv[i].Ci; };
+  size_t total = 0;
+  for (int i = 0; i < 13; ++i) total += 3 * align_up((size_t)h->conv[i].Co * kpad(i), 512);
+  if (!h->packed) VT_CUDA(cudaMalloc(&h->packed, total * sizeof(bf16)));
+  {
+    float* d_max = nullptr;
+    VT_CUDA(cudaMalloc(&d_max, 13 * sizeof(float)));
+    cudaError_t e = cudaSuccess;
+    for (int i = 0; i < 13 && e == cudaSuccess; ++i)
+      e = launch_absmax(h->pool + h->params[h->conv[i].pw].offset, (long long)h->conv[i].Co * h->conv[i].Ci * 9, d_max + i, s);
+    float h_max[13];
+    if (e == cudaSuccess) e = cudaMemcpyAsync(h_max, d_max, sizeof(h_max), cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    cudaFree(d_max);
+    if (e != cudaSuccess) return fail(VT_ERR_CUDA, "LPIPS weight scales: %s", cudaGetErrorString(e));
+    for (int i = 0; i < 13; ++i) h->wscale3[i] = split_weight_scale(h_max[i]);
+  }
+  size_t off = 0;
+  for (int i = 0; i < 13; ++i) {
+    const LpipsConv& c = h->conv[i];
+    const size_t n = align_up((size_t)c.Co * kpad(i), 512);
+    h->w[i] = h->packed + off;
+    h->w3[i] = h->packed + off + n;
+    off += 3 * n;
+    const float* w = h->pool + h->params[c.pw].offset;
+    VT_CUDA(launch_pack_w_nk_bf16(w, h->w[i], c.Co, c.Co, c.Ci, 9, kpad(i), s));
+    VT_CUDA(launch_pack_w_nk_bf16(w, h->w3[i], c.Co, c.Co, c.Ci, 9, kpad(i), s, h->wscale3[i]));
+  }
+  VT_CUDA(cudaStreamSynchronize(s));
+  h->finalized = true;
+  return VT_OK;
+}
+
+int32_t vt_lpips_pass_frames(int32_t H, int32_t W) { return H > 0 && W > 0 ? lpips_pass_frames(H, W) : 0; }
+
+int64_t vt_lpips_workspace_bytes(const vt_lpips_model* h, int32_t precision, int32_t B, int32_t C, int32_t T, int32_t H, int32_t W) {
+  if (!h) { fail(VT_ERR_INVALID, "null handle"); return -1; }
+  LpipsLayout L;
+  if (lpips_check(precision, B, C, T, H, W, &L)) return -1;
+  return (int64_t)(2 * L.act_bytes + L.part_bytes);
+}
+
+int32_t vt_lpips(vt_lpips_model* h, int32_t precision, const void* x, int32_t x_dtype, const void* y, int32_t y_dtype, int32_t B, int32_t C,
+                 int32_t T, int32_t H, int32_t W, float* lpips, float* per_layer, double* running, void* workspace, int64_t workspace_bytes,
+                 void* stream) {
+  if (!h || !x || !y || !lpips) return fail(VT_ERR_INVALID, "null argument");
+  auto dt_ok = [](int d) { return d == VT_DTYPE_F32 || d == VT_DTYPE_BF16 || d == VT_DTYPE_F16; };
+  if (!dt_ok(x_dtype) || !dt_ok(y_dtype)) return fail(VT_ERR_INVALID, "unknown dtype (x %d, y %d)", x_dtype, y_dtype);
+  LpipsLayout L;
+  int rc = lpips_check(precision, B, C, T, H, W, &L);
+  if (rc) return rc;
+  if (!workspace || workspace_bytes < (int64_t)(2 * L.act_bytes + L.part_bytes))
+    return fail(VT_ERR_WORKSPACE, "LPIPS workspace: %lld bytes given, %lld needed", (long long)workspace_bytes,
+                (long long)(2 * L.act_bytes + L.part_bytes));
+  if (!h->finalized) return fail(VT_ERR_NOT_READY, "vt_lpips_finalize has not been called");
+  const bool split = precision == VT_PREC_EXACT_TC;
+  const long long frames = (long long)B * T;
+  // every plan of both pass sizes first: a geometry conv_tc refuses launches nothing
+  const int g_tail = (int)(frames % L.G == 0 ? L.G : frames % L.G);
+  for (int g : {L.G, g_tail}) {
+    int lvl = 0;
+    for (int i = 1; i < 13; ++i) {
+      if (lp_pool_before(i)) ++lvl;
+      TcPlan pl;
+      if (!lpips_conv_plan(h, i, g, L.Hl[lvl], L.Wl[lvl], split, &pl))
+        return fail(VT_ERR_INVALID, "LPIPS conv %d at %d x %d: the wgmma conv does not take it: %s", kLpConvIdx[i], L.Hl[lvl], L.Wl[lvl],
+                    conv_tc_last_error());
+    }
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  bf16* buf[2] = {(bf16*)workspace, (bf16*)((char*)workspace + L.act_bytes)};
+  float* part = (float*)((char*)workspace + 2 * L.act_bytes);
+  for (long long n0 = 0; n0 < frames; n0 += L.G) {
+    const int g = (int)std::min<long long>(L.G, frames - n0);
+    LpipsFinish fin;
+    long long off = 0;
+    for (int k = 0; k < 5; ++k) {
+      fin.tiles[k] = lpips_head_tiles(L.Hl[k], L.Wl[k]);
+      fin.off[k] = off;
+      fin.area[k] = (double)L.Hl[k] * L.Wl[k];
+      off += (long long)g * fin.tiles[k];
+    }
+    int cur = 0, lvl = 0, tap = 0;
+    VT_CUDA(launch_lpips_stem(x, x_dtype, y, y_dtype, T, n0, g, H, W, split, split ? h->w3[0] : h->w[0], h->pool + h->params[h->conv[0].pb].offset,
+                              1.0f / h->wscale3[0], buf[cur], s));
+    for (int i = 1; i < 13; ++i) {
+      if (lp_pool_before(i)) {
+        VT_CUDA(launch_maxpool2x2(buf[cur], buf[cur ^ 1], 2LL * g, L.Hl[lvl], L.Wl[lvl], h->conv[i].Ci, split, s));
+        cur ^= 1;
+        ++lvl;
+      }
+      TcPlan pl;
+      lpips_conv_plan(h, i, g, L.Hl[lvl], L.Wl[lvl], split, &pl);
+      cudaError_t e = launch_conv_tc(pl, buf[cur], split ? h->w3[i] : h->w[i], buf[cur ^ 1], s);
+      if (e != cudaSuccess) return fail(VT_ERR_CUDA, "LPIPS conv %d: %s %s", kLpConvIdx[i], cudaGetErrorString(e), conv_tc_last_error());
+      cur ^= 1;
+      if (lp_tap(i)) {
+        VT_CUDA(launch_lpips_head(buf[cur], g, L.Hl[lvl], L.Wl[lvl], h->conv[i].Co, split, h->pool + h->params[h->plin[tap]].offset,
+                                  part + fin.off[tap], s));
+        ++tap;
+      }
+    }
+    VT_CUDA(launch_lpips_finish(part, fin, g, lpips + n0, per_layer ? per_layer + n0 * 5 : nullptr, running, s));
+  }
+  return VT_OK;
+}
+
+// One ReLU convolution of the LPIPS stack as the executor runs it (vt_conv_desc with res_mode 0)
+int32_t vt_op_conv_relu(int32_t precision, const vt_conv_desc* d, const void* x, const float* w, const float* bias, void* out, void* stream) {
+  if (!d) return fail(VT_ERR_INVALID, "null argument");
+  if (d->res_mode != 0) return fail(VT_ERR_INVALID, "vt_op_conv_relu takes no residual (res_mode 0)");
+  if (precision != VT_PREC_BF16 && precision != VT_PREC_EXACT_TC) return fail(VT_ERR_INVALID, "the ReLU epilogue exists on the wgmma path only");
+  return op_conv_impl(precision, 0, d, nullptr, x, nullptr, w, bias, nullptr, nullptr, nullptr, out, nullptr, (cudaStream_t)stream,
+                      nullptr, true);
+}
+
+int32_t vt_op_maxpool2x2(int32_t precision, const void* x, void* y, int64_t N, int32_t H, int32_t W, int32_t C, void* stream) {
+  if (!x || !y) return fail(VT_ERR_INVALID, "null argument");
+  if (precision != VT_PREC_BF16 && precision != VT_PREC_EXACT_TC) return fail(VT_ERR_INVALID, "maxpool2x2 takes bf16 or split activations");
+  if (N <= 0 || H < 2 || W < 2 || C <= 0 || C % 8 != 0) return fail(VT_ERR_INVALID, "maxpool2x2 needs N > 0, H, W >= 2 and C %% 8 == 0");
+  VT_CUDA(launch_maxpool2x2((const bf16*)x, (bf16*)y, N, H, W, C, precision == VT_PREC_EXACT_TC, (cudaStream_t)stream));
   return VT_OK;
 }
 
