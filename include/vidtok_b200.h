@@ -278,6 +278,38 @@ int32_t vt_lpips(vt_lpips_model* h, int32_t precision, const void* x, int32_t x_
                  int32_t T, int32_t H, int32_t W, float* lpips, float* per_layer, double* running, void* workspace,
                  int64_t workspace_bytes, void* stream);
 
+/* ---- I3D features for the Frechet video distance (FVD).  The definition (vidtok_b200/metrics.py, README "FVD"): each clip
+ *      clamped to [-1,1], (v+1)/2, every frame resized bilinearly (align_corners=False, no antialias) to short side 224 and
+ *      long side ceil(long * 224 / short), centre-cropped to 224 x 224, (v-0.5)*2; I3D (Inception-v1 inflated, Kinetics-400,
+ *      the PyTorch port's InceptionI3d layout); the 400 logits averaged over the remaining time steps.  One handle holds the
+ *      weights, built like vt_lpips_model.  Clips run in passes of vt_i3d_pass_clips(T, H, W); a clip's features do not depend
+ *      on the pass or the call, and every sum runs in a fixed order. ---- */
+typedef struct vt_i3d_model vt_i3d_model;
+int32_t vt_i3d_create(int32_t device, vt_i3d_model** out);
+void vt_i3d_destroy(vt_i3d_model* h);
+/* The port's state-dict keys: <unit>.conv3d.weight [Co,Ci,k,k,k] and <unit>.bn.{weight,bias,running_mean,running_var} [Co]
+ * for Conv3d_1a_7x7, Conv3d_2b_1x1, Conv3d_2c_3x3 and Mixed_{3b,3c,4b,4c,4d,4e,4f,5b,5c}.{b0,b1a,b1b,b2a,b2b,b3b};
+ * logits.conv3d.weight [400,1024,1,1,1] and logits.conv3d.bias [400].  shape5: five extents (1 beyond ndim). */
+int32_t vt_i3d_num_params(const vt_i3d_model* h);
+int32_t vt_i3d_param_info(const vt_i3d_model* h, int32_t index, char* name, int32_t name_cap, int64_t* shape5, int32_t* ndim);
+int32_t vt_i3d_load_param(vt_i3d_model* h, const char* name, const float* data, int64_t numel, int32_t is_device, void* stream);
+/* folds BatchNorm (eps 1e-3) into the weights, packs them for the kernels (bf16 and the split copy of EXACT_TC); synchronises */
+int32_t vt_i3d_finalize(vt_i3d_model* h, void* stream);
+/* clips per pass for T frames: 8, or fewer where an activation of the pass would exceed 2^31 elements; 0 for T < 9 */
+int32_t vt_i3d_pass_clips(const vt_i3d_model* h, int32_t T, int32_t H, int32_t W);
+/* workspace of vt_i3d_features for this geometry (one pass); -1 and a message for a geometry it refuses */
+int64_t vt_i3d_workspace_bytes(const vt_i3d_model* h, int32_t precision, int32_t B, int32_t C, int32_t T, int32_t H, int32_t W);
+/* x: device, dense [B,C,T,H,W] of VT_DTYPE_*, in [-1,1].  precision VT_PREC_BF16 or VT_PREC_EXACT_TC; C must be 3 and T at
+ * least 9, otherwise VT_ERR_INVALID and nothing is launched.  features: device fp32 [B,400].  stats (device, may be NULL):
+ * doubles [n, sum f (400), sum f f^T (400 x 400)] that receive += this call's clips, clip by clip in index order. */
+int32_t vt_i3d_features(vt_i3d_model* h, int32_t precision, const void* x, int32_t x_dtype, int32_t B, int32_t C, int32_t T, int32_t H,
+                        int32_t W, float* features, double* stats, void* workspace, int64_t workspace_bytes, void* stream);
+/* For the tests: the activation at end point `name` (Conv3d_1a_7x7 ... Mixed_5c, the port's names) of up to one pass of
+ * clips, as fp32 [B,C,T,H,W] of the real channels into out.  shape5 (may be NULL) receives that shape; with out NULL only the
+ * shape is computed and nothing is launched. */
+int32_t vt_i3d_endpoint(vt_i3d_model* h, int32_t precision, const void* x, int32_t x_dtype, int32_t B, int32_t C, int32_t T, int32_t H,
+                        int32_t W, const char* name, float* out, int64_t* shape5, void* workspace, int64_t workspace_bytes, void* stream);
+
 /* ---- single operators, exposed for the parity tests (same kernels the model path launches) ---- */
 typedef struct vt_conv_desc {
   int32_t B, Ti, Hi, Wi, Ci;        /* input, channels-last [B,Ti,Hi,Wi,Ci] */

@@ -1036,7 +1036,7 @@ cudaError_t launch_conv_tc(const TcPlan& pl, const bf16* x, const bf16* w_nk, vo
   t.tilesW = (p.Wo + t.BW - 1) / t.BW; t.tilesH = (p.Ho + t.BH - 1) / t.BH; t.tilesT = (p.To + t.BT - 1) / t.BT;
   t.num_n_tiles = Co_pad / t.BN;
   t.num_tiles = (long long)p.B * t.tilesT * t.tilesH * t.tilesW * t.num_n_tiles;
-  t.split = split ? 1 : 0; t.a_lo = p.Ci; t.b_lo = Kpad; t.o_lo = p.Co;
+  t.split = split ? 1 : 0; t.a_lo = p.Ci; t.b_lo = Kpad; t.o_lo = pl.o_lo ? pl.o_lo : p.Co;
   t.acc_scale = (split && p.acc_scale != 0.f) ? p.acc_scale : 1.0f;
   t.B = p.B; t.To = p.To; t.Ho = p.Ho; t.Wo = p.Wo; t.Co = p.Co; t.Ti = p.Ti;
   t.kt = p.kt; t.kh = p.kh; t.kw = p.kw; t.Ci = p.Ci; t.num_kc = p.Ci / 64;

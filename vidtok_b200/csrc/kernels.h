@@ -149,6 +149,8 @@ struct TcPlan {
   DType tout;
   int w_batches, BN, BW, BH, BT, halo, hP, a_stages, stages, kparts, res_mma, ident_s;
   int stage_out;                 // bf16 output tiles leave through shared-memory staging buffers and bulk tensor stores
+  int o_lo;                      // split output: channel offset of the lo plane from the output pointer (0: Co); a conv
+                                 // that writes a channel slice of a wider tensor sets it to that tensor's channel count
   uint32_t halo_bytes, misc_off;
   size_t smem;
   TcLnFusion ln;                 // the requested epilogues that are taken (mode 0 otherwise)
@@ -224,5 +226,45 @@ struct LpipsFinish {
 };
 cudaError_t launch_lpips_finish(const float* part, const LpipsFinish& f, int G, float* lpips, float* per_layer, double* running,
                                 cudaStream_t s);
+
+// Max-pool of channels-last [N,T,H,W,C] (split: hi C | lo C, compared as hi + lo) with SAME front padding (zeros) ->
+// [N,To,Ho,Wo,C]; C % 8 == 0 (lpips.cu)
+struct MaxPool3d {
+  int T, H, W, C, To, Ho, Wo;
+  int kt, kh, kw, st, sh, sw, pt, ph, pw;
+};
+cudaError_t launch_maxpool3d(const bf16* x, bf16* y, long long N, const MaxPool3d& q, bool split, cudaStream_t s);
+
+// i3d.cu: the FVD feature network's own kernels.  Frames are resized so that the short side is 224 and centre-cropped to
+// 224 x 224; Mixed_5c has 1024 channels and the logits 400.
+constexpr int kI3dSize = 224, kI3dFeatC = 1024, kI3dClasses = 400;
+struct I3dCrop { int Hr, Wr, oh, ow; };
+inline I3dCrop i3d_crop(int H, int W) {
+  I3dCrop c;
+  // short side 224, long side ceil(long * 224 / short) in integers
+  if (H <= W) { c.Hr = kI3dSize; c.Wr = (int)(((long long)W * kI3dSize + H - 1) / H); }
+  else { c.Wr = kI3dSize; c.Hr = (int)(((long long)H * kI3dSize + W - 1) / W); }
+  c.oh = (c.Hr - kI3dSize) / 2;
+  c.ow = (c.Wr - kI3dSize) / 2;
+  return c;
+}
+// clips [n0, n0 + G) of x [Bc,3,T,H,W] (VT_DTYPE_*) -> fp32 [G,3,T,224,224]: clamp, (v+1)/2, bilinear resize, crop, (v-0.5)*2
+cudaError_t launch_i3d_resize(const void* x, int x_dtype, long long n0, int G, int T, int H, int W, float* out, cudaStream_t s);
+// Conv3d_1a_7x7 with folded BatchNorm and ReLU: x [G,3,T,224,224] fp32 -> channels-last [G,To,112,112,64] (split: hi|lo);
+// wpk [64][1088] (launch_pack_w_nk_bf16, 343 taps, Kpad 1088) or its split copy
+size_t i3d_stem_smem(bool split);
+cudaError_t launch_i3d_stem(const float* x, int G, int T, int To, int pt, int ph, int pw, bool split, const bf16* wpk, const float* bias,
+                            float acc_scale, bf16* out, cudaStream_t s);
+// Mixed_5c [G,T5,7,7,1024] -> features [G,400]: AvgPool3d [2,7,7], the logits (wt [1024][400] fp32, bias [400]), mean over time
+cudaError_t launch_i3d_head(const bf16* f, int G, int T5, bool split, const float* wt, const float* bias, float* feat, cudaStream_t s);
+// stats [1 + 400 + 400 * 400] doubles += (G, sum f, sum f f^T), clip by clip in index order
+cudaError_t launch_i3d_stats(const float* feat, int G, double* stats, cudaStream_t s);
+// Real channel c of a stored layout: in segment k (real0 <= c < real0 + count) it is stored at stored0 + c - real0
+struct I3dSegs {
+  int n, real;
+  int real0[4], stored0[4], count[4];
+};
+cudaError_t launch_i3d_unpack(const bf16* x, bool split, long long N, int T, int H, int W, int Cs, const I3dSegs& segs, float* out,
+                              cudaStream_t s);
 
 }  // namespace vt

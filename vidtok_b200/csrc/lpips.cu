@@ -80,6 +80,56 @@ __global__ void __launch_bounds__(kThreads) maxpool2x2_kernel(const bf16* __rest
   }
 }
 
+// The max-pools of I3D (metrics FVD): window kt x kh x kw, strides st x sh x sw, front padding pt, ph, pw ("SAME"), over
+// channels-last [N,T,H,W,C] (split: [.., hi C | lo C], compared as hi + lo) -> [N,To,Ho,Wo,C].  A padded position counts as a
+// zero, which is what ignoring it gives on the ReLU outputs this pools.  Window order (t, h, w); the first maximum wins, a
+// NaN wins.
+template <bool kSplit>
+__global__ void __launch_bounds__(kThreads) maxpool3d_kernel(const bf16* __restrict__ x, bf16* __restrict__ y, long long total, MaxPool3d q) {
+  const int U = q.C / 8;
+  const long long cs = kSplit ? 2LL * q.C : (long long)q.C;
+  for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < total; i += (long long)gridDim.x * kThreads) {
+    const int u = (int)(i % U);
+    long long r = i / U;
+    const int wo = (int)(r % q.Wo);
+    r /= q.Wo;
+    const int ho = (int)(r % q.Ho);
+    r /= q.Ho;
+    const int to = (int)(r % q.To);
+    const long long n = r / q.To;
+    float best[8], v[8];
+    uint4 bh = make_uint4(0, 0, 0, 0), bl = make_uint4(0, 0, 0, 0), h, l;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) best[e] = -INFINITY;
+    uint16_t* bhs = reinterpret_cast<uint16_t*>(&bh);
+    uint16_t* bls = reinterpret_cast<uint16_t*>(&bl);
+    for (int a = 0; a < q.kt; ++a)
+      for (int b = 0; b < q.kh; ++b)
+        for (int c = 0; c < q.kw; ++c) {
+          const int ti = to * q.st + a - q.pt, hi = ho * q.sh + b - q.ph, wi = wo * q.sw + c - q.pw;
+          if (ti >= 0 && ti < q.T && hi >= 0 && hi < q.H && wi >= 0 && wi < q.W) {
+            load8<kSplit>(x + (((n * q.T + ti) * q.H + hi) * q.W + wi) * cs + 8 * u, q.C, v, h, l);
+          } else {
+            h = l = make_uint4(0, 0, 0, 0);
+#pragma unroll
+            for (int e = 0; e < 8; ++e) v[e] = 0.f;
+          }
+          const uint16_t* hs = reinterpret_cast<const uint16_t*>(&h);
+          const uint16_t* ls = reinterpret_cast<const uint16_t*>(&l);
+#pragma unroll
+          for (int e = 0; e < 8; ++e)
+            if (v[e] > best[e] || v[e] != v[e]) {
+              best[e] = v[e];
+              bhs[e] = hs[e];
+              if constexpr (kSplit) bls[e] = ls[e];
+            }
+        }
+    bf16* dst = y + (((n * q.To + to) * q.Ho + ho) * q.Wo + wo) * cs + 8 * u;
+    *reinterpret_cast<uint4*>(dst) = bh;
+    if constexpr (kSplit) *reinterpret_cast<uint4*>(dst + q.C) = bl;
+  }
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
   // xor butterfly: every lane ends with the same value (fp addition is commutative)
 #pragma unroll
@@ -186,6 +236,19 @@ cudaError_t launch_maxpool2x2(const bf16* x, bf16* y, long long N, int H, int W,
   ProfScope _ps("maxpool2x2", 3.0 * N * Ho * Wo * C, esz * ((double)N * H * W * C + (double)N * Ho * Wo * C), s, det);
   if (split) maxpool2x2_kernel<true><<<grid_for(total), kThreads, 0, s>>>(x, y, total, H, W, Ho, Wo, C);
   else maxpool2x2_kernel<false><<<grid_for(total), kThreads, 0, s>>>(x, y, total, H, W, Ho, Wo, C);
+  count_launch();
+  return cudaGetLastError();
+}
+
+cudaError_t launch_maxpool3d(const bf16* x, bf16* y, long long N, const MaxPool3d& q, bool split, cudaStream_t s) {
+  if (q.C % 8 != 0 || q.To < 1 || q.Ho < 1 || q.Wo < 1) return cudaErrorInvalidValue;
+  const long long total = N * q.To * q.Ho * q.Wo * (q.C / 8);
+  const double esz = split ? 4.0 : 2.0, out = (double)N * q.To * q.Ho * q.Wo * q.C;
+  char det[96] = "";
+  if (prof_enabled()) snprintf(det, sizeof(det), "k%d%d%d s%d%d%d %lldx%dx%dx%dx%d%s", q.kt, q.kh, q.kw, q.st, q.sh, q.sw, N, q.T, q.H, q.W, q.C, split ? " split" : "");
+  ProfScope _ps("maxpool3d", out * q.kt * q.kh * q.kw, esz * ((double)N * q.T * q.H * q.W * q.C + out), s, det);
+  if (split) maxpool3d_kernel<true><<<grid_for(total), kThreads, 0, s>>>(x, y, total, q);
+  else maxpool3d_kernel<false><<<grid_for(total), kThreads, 0, s>>>(x, y, total, q);
   count_launch();
   return cudaGetLastError();
 }

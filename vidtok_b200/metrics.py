@@ -94,15 +94,25 @@ class Scorer:
             scorer.update(x, recon)            # enqueues the kernels; no host synchronisation
         scorer.result()                        # {"psnr", "ssim", "frames"[, "lpips"]}: the one synchronisation
 
+    With an I3D model (Scorer(i3d=I3D.from_files())) each update also adds the input clips' I3D features to the "real"
+    statistics and the reconstructions' to the "generated" ones, and result() adds "fvd" and "fvd_clips".  fvd_frames=k cuts
+    every clip of an update into consecutive windows of k frames (a shorter tail is dropped); otherwise a clip is one sample.
+
     The sums live in doubles on the device, so result() equals the script's np.mean over its per-frame lists (see the module
     docstring for why no grouping by 16 is needed).  The workspaces are kept and regrown only for a larger geometry."""
 
-    def __init__(self, lpips: "LPIPS | None" = None):
+    def __init__(self, lpips: "LPIPS | None" = None, i3d: "I3D | None" = None, fvd_frames: int | None = None):
         self._acc = None
         self._ws = None
         self._lpips = lpips
         self._lacc = None     # [sum of LPIPS, frames]
         self._lws = None
+        if fvd_frames is not None and (i3d is None or fvd_frames < I3D_MIN_FRAMES):
+            raise ValueError(f"fvd_frames needs an I3D model and at least {I3D_MIN_FRAMES} frames, got {fvd_frames}")
+        self._i3d = i3d
+        self._fvd_frames = fvd_frames
+        self._facc = None     # [2, n + sum f + sum f f^T]: the input clips' features, then the reconstructions'
+        self._fws = None
 
     def update(self, x: torch.Tensor, y: torch.Tensor):
         """Scores one piece (as frame_scores, and lpips_scores when the Scorer has an LPIPS model) and adds its frames to the
@@ -123,6 +133,15 @@ class Scorer:
             if self._lws is None or self._lws.numel() < lneed:
                 self._lws = torch.empty(lneed, dtype=torch.uint8, device=x.device)
             self._lpips._launch(x, y, geom, self._lacc, self._lws)
+        if self._i3d is not None:
+            if self._facc is None:
+                self._facc = torch.zeros(2, _STATS_LEN, dtype=torch.float64, device=x.device)
+            for k, clips in enumerate((x, y)):
+                clips = fvd_windows(clips, self._fvd_frames)
+                fneed = self._i3d._workspace_bytes(_clip_geometry(clips))
+                if self._fws is None or self._fws.numel() < fneed:
+                    self._fws = torch.empty(fneed, dtype=torch.uint8, device=x.device)
+                self._i3d._launch(clips, self._facc[k], self._fws)
         return out
 
     def sums(self) -> torch.Tensor:
@@ -137,6 +156,8 @@ class Scorer:
         Before any frame was scored: frames 0 and NaN scores."""
         from .dist import allreduce_sum, global_scores
         acc = self.sums()
+        if self._i3d is not None:
+            return self._result_fvd(acc, reduce)
         if self._lpips is None:
             if not reduce:
                 return _means(acc)
@@ -150,11 +171,37 @@ class Scorer:
         out["lpips"] = s / n if n > 0 else math.nan
         return out
 
+    def _result_fvd(self, acc: torch.Tensor, reduce: bool) -> dict:
+        """result() with FVD: the score sums, the LPIPS sums and both feature accumulators in one all-reduce."""
+        from .dist import allreduce_sum
+        lacc = self._lacc if self._lacc is not None else torch.zeros(2, dtype=torch.float64, device=acc.device)
+        facc = self._facc if self._facc is not None else torch.zeros(2, _STATS_LEN, dtype=torch.float64, device=acc.device)
+        both = torch.cat([acc, lacc.to(acc.device), facc.to(acc.device).flatten()])
+        if reduce:
+            both = allreduce_sum(both)
+        out = _means(both[:3])
+        if self._lpips is not None:
+            s, n = both[3:5].tolist()
+            out["lpips"] = s / n if n > 0 else math.nan
+        f = both[5:].view(2, _STATS_LEN).cpu()
+        n = int(round(float(f[0, 0])))
+        out["fvd"] = fvd_from_stats(f[0], f[1]) if n >= 2 else math.nan
+        out["fvd_clips"] = n
+        return out
+
+    def fvd_sums(self) -> torch.Tensor:
+        """A copy of the feature accumulators, float64 [2, n + sum f + sum f f^T] (input clips, reconstructions)."""
+        if self._facc is not None:
+            return self._facc.clone()
+        return torch.zeros(2, _STATS_LEN, dtype=torch.float64)
+
     def reset(self):
         if self._acc is not None:
             self._acc.zero_()
         if self._lacc is not None:
             self._lacc.zero_()
+        if self._facc is not None:
+            self._facc.zero_()
 
 
 def _means(sums: torch.Tensor) -> dict:
@@ -308,3 +355,224 @@ def lpips_scores(model: LPIPS, x: torch.Tensor, y: torch.Tensor, per_layer: bool
     geom = _geometry(x, y, False)
     ws = torch.empty(model._workspace_bytes(geom), dtype=torch.uint8, device=x.device)
     return model._launch(x, y, geom, None, ws, per_layer)
+
+
+# ---- FVD: I3D features and the Frechet distance -------------------------------------------------------------------------------
+# The definition (the common one, VideoGPT's fvd module with TF-GAN's Frechet distance; the reference reports FVD but ships no
+# code for it): clamp to [-1,1], (v+1)/2, bilinear resize (align_corners=False, no antialias) to short side 224 and long side
+# ceil(long * 224 / short), centre crop 224 x 224, (v-0.5)*2; I3D (Inception-v1 inflated, Kinetics-400); the 400 logits averaged
+# over time; FVD = |mu1-mu2|^2 + tr S1 + tr S2 - 2 tr((S1^1/2 S2 S1^1/2)^1/2) with unbiased covariances, in float64.
+I3D_DEFAULT_PATH = os.path.join("checkpoints", "i3d", "i3d_pretrained_400.pt")
+I3D_FEATURES = 400
+I3D_MIN_FRAMES = 9
+_I3D_MODULES = (("Mixed_3b", (64, 96, 128, 16, 32, 32)), ("Mixed_3c", (128, 128, 192, 32, 96, 64)),
+                ("Mixed_4b", (192, 96, 208, 16, 48, 64)), ("Mixed_4c", (160, 112, 224, 24, 64, 64)),
+                ("Mixed_4d", (128, 128, 256, 24, 64, 64)), ("Mixed_4e", (112, 144, 288, 32, 64, 64)),
+                ("Mixed_4f", (256, 160, 320, 32, 128, 128)), ("Mixed_5b", (256, 160, 320, 32, 128, 128)),
+                ("Mixed_5c", (384, 192, 384, 48, 128, 128)))
+I3D_ENDPOINTS = ("Conv3d_1a_7x7", "MaxPool3d_2a_3x3", "Conv3d_2b_1x1", "Conv3d_2c_3x3", "MaxPool3d_3a_3x3", "Mixed_3b", "Mixed_3c",
+                 "MaxPool3d_4a_3x3", "Mixed_4b", "Mixed_4c", "Mixed_4d", "Mixed_4e", "Mixed_4f", "MaxPool3d_5a_2x2", "Mixed_5b",
+                 "Mixed_5c")
+_STATS_LEN = 1 + I3D_FEATURES + I3D_FEATURES * I3D_FEATURES
+
+
+def i3d_units():
+    """[(unit key, Cin, Cout, k)] of every conv + BatchNorm + ReLU unit of I3D, in network order."""
+    units = [("Conv3d_1a_7x7", 3, 64, 7), ("Conv3d_2b_1x1", 64, 64, 1), ("Conv3d_2c_3x3", 64, 192, 3)]
+    cin = 192
+    for name, o in _I3D_MODULES:
+        units += [(f"{name}.b0", cin, o[0], 1), (f"{name}.b1a", cin, o[1], 1), (f"{name}.b1b", o[1], o[2], 3),
+                  (f"{name}.b2a", cin, o[3], 1), (f"{name}.b2b", o[3], o[4], 3), (f"{name}.b3b", cin, o[5], 1)]
+        cin = o[0] + o[2] + o[4] + o[5]
+    return units
+
+
+def i3d_state_shapes() -> dict:
+    """The PyTorch port's (InceptionI3d, i3d_pretrained_400.pt) parameter keys and shapes."""
+    shapes = {}
+    for key, ci, co, k in i3d_units():
+        shapes[f"{key}.conv3d.weight"] = (co, ci, k, k, k)
+        for b in ("weight", "bias", "running_mean", "running_var"):
+            shapes[f"{key}.bn.{b}"] = (co,)
+    shapes["logits.conv3d.weight"] = (I3D_FEATURES, 1024, 1, 1, 1)
+    shapes["logits.conv3d.bias"] = (I3D_FEATURES,)
+    return shapes
+
+
+def i3d_state(sd: dict) -> dict:
+    """The I3D parameters of a state dict in the port's layout.  Raises KeyError naming a missing key and ValueError naming a
+    misshaped one; other keys (num_batches_tracked) are ignored."""
+    out = {}
+    missing = [k for k in i3d_state_shapes() if k not in sd]
+    if missing:
+        raise KeyError("I3D state dict lacks " + ", ".join(missing))
+    for key, shape in i3d_state_shapes().items():
+        v = torch.as_tensor(sd[key])
+        if tuple(v.shape) != shape:
+            raise ValueError(f"I3D parameter {key}: shape {tuple(v.shape)}, expected {shape}")
+        out[key] = v
+    return out
+
+
+def _clip_geometry(x: torch.Tensor):
+    if x.dim() != 5:
+        raise ValueError(f"expected clips [B,3,T,H,W], got {tuple(x.shape)}")
+    if x.dtype not in _DTYPES:
+        raise ValueError(f"expected a float32, bfloat16 or float16 tensor, got {x.dtype}")
+    if x.numel() == 0:
+        raise ValueError(f"empty clip {tuple(x.shape)}")
+    if not x.is_cuda:
+        raise RuntimeError("vidtok_b200: inputs must be CUDA tensors; there is no CPU path")
+    return tuple(int(d) for d in x.shape)
+
+
+class I3D:
+    """The FVD feature network on the device: owns the library's I3D weight handle.  precision "exact" (the default:
+    fp32-class results through the split-fp16 tensor-core operands) or "bf16".  Build it with from_state_dict or from_files;
+    use it with i3d_features or Scorer(i3d=...)."""
+
+    def __init__(self, state: dict, device=None, precision: str = "exact"):
+        if precision not in _LPIPS_PRECISIONS:
+            raise ValueError(f"precision must be one of {sorted(_LPIPS_PRECISIONS)}, got {precision!r}")
+        self.precision = precision
+        self.device = torch.device(device) if device is not None else torch.device("cuda")
+        if self.device.index is None:
+            self.device = torch.device(self.device.type, torch.cuda.current_device())
+        state = i3d_state(state)
+        h = C.c_void_p()
+        N.check(N.lib().vt_i3d_create(self.device.index, C.byref(h)))
+        self._h = h
+        with torch.cuda.device(self.device):
+            stream = torch.cuda.current_stream(self.device)
+            for key, v in state.items():
+                t = v.detach().to("cpu", torch.float32).contiguous()
+                N.check(N.lib().vt_i3d_load_param(h, key.encode(), C.c_void_p(t.data_ptr()), t.numel(), 0, C.c_void_p(stream.cuda_stream)))
+            N.check(N.lib().vt_i3d_finalize(h, C.c_void_p(stream.cuda_stream)))
+
+    @classmethod
+    def from_state_dict(cls, sd: dict, device=None, precision: str = "exact") -> "I3D":
+        return cls(sd, device, precision)
+
+    @classmethod
+    def from_files(cls, path: str | None = None, device=None, precision: str = "exact") -> "I3D":
+        """The port's Kinetics-400 weights (default: checkpoints/i3d/i3d_pretrained_400.pt).  Nothing is downloaded: a missing
+        file raises FileNotFoundError naming the path."""
+        path = path or I3D_DEFAULT_PATH
+        if not os.path.isfile(path):
+            raise FileNotFoundError(f"I3D weights not found: {path}")
+        return cls(torch.load(path, map_location="cpu", weights_only=True), device, precision)
+
+    def close(self):
+        if getattr(self, "_h", None):
+            N.lib().vt_i3d_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def pass_clips(self, T: int, H: int, W: int) -> int:
+        """Clips per pass of the executor: 8, or fewer where an activation of the pass would exceed 2^31 elements."""
+        return int(N.lib().vt_i3d_pass_clips(self._h, T, H, W))
+
+    def _workspace_bytes(self, geom) -> int:
+        need = N.lib().vt_i3d_workspace_bytes(self._h, _LPIPS_PRECISIONS[self.precision], *geom)
+        if need < 0:
+            raise ValueError(N.lib().vt_last_error().decode(errors="replace"))
+        return need
+
+    def _launch(self, x, stats, workspace):
+        geom = _clip_geometry(x)
+        if x.device != self.device:
+            raise ValueError(f"this I3D model lives on {self.device}, got clips on {x.device}")
+        x = x.detach().contiguous()
+        with torch.cuda.device(x.device):
+            feats = torch.empty((geom[0], I3D_FEATURES), dtype=torch.float32, device=x.device)
+            N.check(N.lib().vt_i3d_features(
+                self._h, _LPIPS_PRECISIONS[self.precision], C.c_void_p(x.data_ptr()), _DTYPES[x.dtype], *geom,
+                C.c_void_p(feats.data_ptr()), C.c_void_p(stats.data_ptr()) if stats is not None else None,
+                C.c_void_p(workspace.data_ptr()), workspace.numel(), C.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)))
+        return feats
+
+    def endpoint(self, x: torch.Tensor, name: str, workspace: torch.Tensor | None = None) -> torch.Tensor:
+        """The activation at end point `name` (I3D_ENDPOINTS) as fp32 [B,C,T,H,W], for the tests: one pass of clips at most."""
+        geom = _clip_geometry(x)
+        prec = _LPIPS_PRECISIONS[self.precision]
+        shape = (C.c_int64 * 5)()
+        N.check(N.lib().vt_i3d_endpoint(self._h, prec, None, _DTYPES[x.dtype], *geom, name.encode(), None, shape, None, 0, None))
+        x = x.detach().contiguous()
+        if workspace is None:
+            workspace = torch.empty(self._workspace_bytes(geom), dtype=torch.uint8, device=x.device)
+        with torch.cuda.device(x.device):
+            out = torch.empty(tuple(shape), dtype=torch.float32, device=x.device)
+            N.check(N.lib().vt_i3d_endpoint(self._h, prec, C.c_void_p(x.data_ptr()), _DTYPES[x.dtype], *geom, name.encode(),
+                                            C.c_void_p(out.data_ptr()), None, C.c_void_p(workspace.data_ptr()), workspace.numel(),
+                                            C.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)))
+        return out
+
+
+def i3d_features(model: I3D, clips: torch.Tensor, stats: torch.Tensor | None = None) -> torch.Tensor:
+    """fp32 [B,400] I3D features of clips [B,3,T,H,W] in [-1,1] (float32, bfloat16 or float16, T >= 9), on the current stream,
+    without synchronising.  stats (optional): a float64 device tensor of i3d_stats_empty()'s shape that receives += this
+    call's clips, in clip order."""
+    ws = torch.empty(model._workspace_bytes(_clip_geometry(clips)), dtype=torch.uint8, device=clips.device)
+    return model._launch(clips, stats, ws)
+
+
+def i3d_stats_empty(device=None) -> torch.Tensor:
+    """A zero accumulator [n, sum f (400), sum f f^T (400 x 400)] in float64."""
+    return torch.zeros(_STATS_LEN, dtype=torch.float64, device=device)
+
+
+def features_to_stats(features: torch.Tensor) -> torch.Tensor:
+    """The accumulator of a feature set [n,400], in float64 (host or device)."""
+    f = features.to(torch.float64)
+    return torch.cat([torch.tensor([f.shape[0]], dtype=torch.float64, device=f.device), f.sum(0), (f.T @ f).flatten()])
+
+
+def _psd_eigvals(a: torch.Tensor, rank: int):
+    """eigh of a symmetric PSD matrix of rank <= rank: eigenvalues clamped at 0, all but the rank largest set to 0 (the
+    covariance of n samples has rank n - 1 at most; the square roots of its zero eigenvalues' rounding noise would otherwise
+    add ~1e-8 of the distance per sample set below 400 clips)"""
+    w, v = torch.linalg.eigh((a + a.T) / 2)
+    w = w.clamp(min=0)
+    if rank < w.numel():
+        w[: w.numel() - rank] = 0
+    return w, v
+
+
+def fvd_from_stats(stats_a: torch.Tensor, stats_b: torch.Tensor) -> float:
+    """FVD between the feature sets of two accumulators (each at least two clips), in float64 on the host."""
+    out = []
+    for s in (stats_a, stats_b):
+        s = s.detach().to("cpu", torch.float64)
+        n = float(s[0])
+        if n < 2:
+            raise ValueError(f"FVD needs at least 2 clips per set, got {n:g}")
+        mu = s[1:1 + I3D_FEATURES] / n
+        cov = (s[1 + I3D_FEATURES:].view(I3D_FEATURES, I3D_FEATURES) - n * torch.outer(mu, mu)) / (n - 1)
+        out.append((mu, cov, int(round(n)) - 1))
+    (mu1, s1, r1), (mu2, s2, r2) = out
+    w, v = _psd_eigvals(s1, r1)
+    root = (v * w.sqrt()) @ v.T
+    tr = _psd_eigvals(root @ s2 @ root, min(r1, r2))[0].sqrt().sum()
+    return float(((mu1 - mu2) ** 2).sum() + torch.trace(s1) + torch.trace(s2) - 2 * tr)
+
+
+def fvd(features_a: torch.Tensor, features_b: torch.Tensor) -> float:
+    """FVD between two feature sets [n,400] (as i3d_features returns them)."""
+    return fvd_from_stats(features_to_stats(features_a), features_to_stats(features_b))
+
+
+def fvd_windows(x: torch.Tensor, k: int | None) -> torch.Tensor:
+    """Clips [B,C,T,H,W] cut into consecutive windows of k frames ([B * (T // k), C, k, H, W], a shorter tail dropped), or x
+    itself for k None."""
+    if k is None:
+        return x
+    B, Cc, T, H, W = x.shape
+    nw = T // k
+    if nw == 0:
+        raise ValueError(f"clips of {T} frames hold no window of {k} frames")
+    return x[:, :, :nw * k].reshape(B, Cc, nw, k, H, W).transpose(1, 2).reshape(B * nw, Cc, k, H, W)
