@@ -161,6 +161,11 @@ int64_t vt_chunk_workspace_bytes(const vt_chunk_state* s, int32_t T_chunk);
 int32_t vt_encode_chunk(vt_chunk_state* s, int32_t is_first, const float* x_chunk, int32_t C, int32_t Tc, const float* noise,
                         float* z, int32_t* indices, float* kl_loss, void* workspace, int64_t workspace_bytes,
                         void* stream);
+/* vt_encode_chunk that also writes the chunk's encoder output before the regularizer, h_pre device fp32 [B,2z|z,Tz,Hz,Wz]
+ * (per-sample losses of a batched state: each sample's KL loss or FSQ aux partials); z / indices as vt_encode_chunk. */
+int32_t vt_encode_chunk_pre(vt_chunk_state* s, int32_t is_first, const float* x_chunk, int32_t C, int32_t Tc, const float* noise,
+                            float* z, int32_t* indices, float* kl_loss, float* h_pre, void* workspace, int64_t workspace_bytes,
+                            void* stream);
 /* vt_encode_chunk of an FSQ model that also writes this chunk's partials of the FSQ aux loss (see vt_fsq_aux_partials):
  * stats fp32 [2] and avg_prob fp32 [J], J = prod(levels), over the chunk's B * Tz * Hz * Wz tokens -- the per-chunk step of
  * vt_encode_video_fsq_aux.  The workspace holds the chunk's pre-bound latent and the partials' scratch on top of
@@ -206,6 +211,14 @@ int32_t vt_decode_video_frames(const vt_model* m, int32_t Tz, int32_t t_chunk_de
 int32_t vt_decode_video(vt_model* m, int32_t precision, const float* z, int32_t B, int32_t Cz, int32_t Tz, int32_t Hz, int32_t Wz,
                         int32_t t_chunk_dec, int32_t use_overlap, float* x_out, int32_t out_on_host, void* workspace,
                         int64_t workspace_bytes, void* stream);
+
+/* Temporal reach R of a causal v1.1 model under the tile_encode / tile_decode chunking: an output frame depends on no input
+ * more than R frames before it.  Encoder (is_decoder 0): latent l depends on input frames >= f - R, f = its group's first
+ * frame (0 for l = 0, else 1 + (l-1) * tdf).  Decoder: decoded frame t depends on latent frames >= t / tdf - R; use_overlap
+ * selects the look-ahead chunking (its caches hold the frames before each chunk; without overlap the trilinear time
+ * upsample's cache reaches further back).  Composed from the layer list the executor runs; no device is touched.
+ * VT_ERR_INVALID for v1.0 and non-causal models, and for use_overlap on the encoder. */
+int32_t vt_temporal_reach(const vt_model* m, int32_t is_decoder, int32_t use_overlap, int32_t* frames);
 
 /* ---- video I/O adjacent steps (scripts/inference_reconstruct.py:41-47,71-82,231-239): the tokenizer runs at > 1000
  *      frames/s, so the uint8 <-> float conversions around it belong on the device too ---- */

@@ -62,6 +62,7 @@ _SIGS = {
     "vt_chunk_state_destroy": (None, [_P]),
     "vt_chunk_workspace_bytes": (_I64, [_P, _I32]),
     "vt_encode_chunk": (_I32, [_P, _I32, _P, _I32, _I32, _P, _P, _P, _P, _P, _I64, _P]),
+    "vt_encode_chunk_pre": (_I32, [_P, _I32, _P, _I32, _I32, _P, _P, _P, _P, _P, _P, _I64, _P]),
     "vt_chunk_fsq_aux_workspace_bytes": (_I64, [_P, _I32]),
     "vt_encode_chunk_fsq_aux": (_I32, [_P, _I32, _P, _I32, _I32, _P, _P, C.c_float, _P, _P, _P, _I64, _P]),
     "vt_decode_chunk": (_I32, [_P, _I32, _P, _I32, _I32, _P, _P, _I64, _P]),
@@ -72,6 +73,7 @@ _SIGS = {
     "vt_decode_video_workspace_bytes": (_I64, [_P, _I32, _I32, _I32, _I32, _I32, _I32, _I32]),
     "vt_decode_video_frames": (_I32, [_P, _I32, _I32, _I32]),
     "vt_decode_video": (_I32, [_P, _I32, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _I32, _P, _I64, _P]),
+    "vt_temporal_reach": (_I32, [_P, _I32, _I32, C.POINTER(_I32)]),
     "vt_video_u8_to_clip": (_I32, [_P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P]),
     "vt_video_u8_to_clip_resized": (_I32, [_P, _P] + [_I32] * 11 + [_P]),
     "vt_clip_to_video_u8": (_I32, [_P, _P, _I32, _I32, _I32, _I32, _P]),

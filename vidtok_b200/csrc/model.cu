@@ -1172,6 +1172,46 @@ struct Stage {
   }
 };
 
+// The stages between conv_in and conv_out, in the order the stack runs them (run_encoder / run_decoder, vt_temporal_reach).
+static std::vector<Stage> encoder_stages(const StackW& e) {
+  std::vector<Stage> stages;
+  for (size_t l = 0; l < e.levels.size(); ++l) {
+    const LevelW& lv = e.levels[l];
+    for (size_t b = 0; b < lv.blk.size(); ++b) {
+      Stage a; a.kind = Stage::RES2D; a.rb = &lv.blk[b]; stages.push_back(a);
+      Stage t; t.kind = Stage::RES1D; t.rb = &lv.tblk[b]; stages.push_back(t);
+    }
+    if (lv.has_resample) {
+      Stage a; a.kind = Stage::DOWN; a.lv = &lv; stages.push_back(a);
+      if (lv.has_tres) { Stage t; t.kind = Stage::TDOWN; t.lv = &lv; stages.push_back(t); }
+    }
+  }
+  { Stage a; a.kind = Stage::RES3D; a.rb = &e.mid1; stages.push_back(a); }
+  { Stage a; a.kind = Stage::ATTN; a.at = &e.attn; stages.push_back(a); }
+  { Stage a; a.kind = Stage::RES3D; a.rb = &e.mid2; stages.push_back(a); }
+  { Stage a; a.kind = Stage::HEAD; a.head_norm = &e.norm_out; stages.push_back(a); }
+  return stages;
+}
+static std::vector<Stage> decoder_stages(const StackW& g) {
+  std::vector<Stage> stages;
+  { Stage a; a.kind = Stage::RES3D; a.rb = &g.mid1; stages.push_back(a); }
+  { Stage a; a.kind = Stage::ATTN; a.at = &g.attn; stages.push_back(a); }
+  { Stage a; a.kind = Stage::RES3D; a.rb = &g.mid2; stages.push_back(a); }
+  for (int l = (int)g.levels.size() - 1; l >= 0; --l) {
+    const LevelW& lv = g.levels[l];
+    for (size_t b = 0; b < lv.blk.size(); ++b) {
+      Stage a; a.kind = Stage::RES2D; a.rb = &lv.blk[b]; stages.push_back(a);
+      Stage t; t.kind = Stage::RES1D; t.rb = &lv.tblk[b]; stages.push_back(t);
+    }
+    if (lv.has_resample) {
+      Stage a; a.kind = Stage::UP; a.lv = &lv; stages.push_back(a);
+      if (lv.has_tres) { Stage t; t.kind = Stage::TUP; t.lv = &lv; stages.push_back(t); }  // nested as model_3dcausal.py:844-853
+    }
+  }
+  { Stage a; a.kind = Stage::HEAD; a.head_norm = &g.norm_out; stages.push_back(a); }
+  return stages;
+}
+
 static void run_stages(Exec& ex, Exec::Stream& st, const std::vector<Stage>& stages) {
   for (size_t i = 0; i < stages.size() && ex.ok(); ++i) {
     const Stage& sg = stages[i];
@@ -1235,23 +1275,7 @@ static void run_encoder(Exec& ex, const float* x_ext, int B, int T, int H, int W
     ConvOpt o; o.ext_in = x_ext; o.t_rep = t_rep;
     st.x = ex.conv(e.conv_in, xin, o);
   }
-  std::vector<Stage> stages;
-  for (size_t l = 0; l < e.levels.size(); ++l) {
-    const LevelW& lv = e.levels[l];
-    for (size_t b = 0; b < lv.blk.size(); ++b) {
-      Stage a; a.kind = Stage::RES2D; a.rb = &lv.blk[b]; stages.push_back(a);
-      Stage t; t.kind = Stage::RES1D; t.rb = &lv.tblk[b]; stages.push_back(t);
-    }
-    if (lv.has_resample) {
-      Stage a; a.kind = Stage::DOWN; a.lv = &lv; stages.push_back(a);
-      if (lv.has_tres) { Stage t; t.kind = Stage::TDOWN; t.lv = &lv; stages.push_back(t); }
-    }
-  }
-  { Stage a; a.kind = Stage::RES3D; a.rb = &e.mid1; stages.push_back(a); }
-  { Stage a; a.kind = Stage::ATTN; a.at = &e.attn; stages.push_back(a); }
-  { Stage a; a.kind = Stage::RES3D; a.rb = &e.mid2; stages.push_back(a); }
-  { Stage a; a.kind = Stage::HEAD; a.head_norm = &e.norm_out; stages.push_back(a); }
-  run_stages(ex, st, stages);
+  run_stages(ex, st, encoder_stages(e));
   Act n = ex.take_norm(st, e.norm_out, true, false);
   ex.free_act(st.x);
   ConvOpt o; o.ext_out = h_out; o.cache_key = "encoder.conv_out";
@@ -1282,23 +1306,7 @@ static void run_decoder(Exec& ex, const float* z_ext, int B, int Tz, int Hz, int
     ConvOpt o; o.ext_in = z_ext; o.ext_in_indices = z_is_indices;
     st.x = ex.conv(g.conv_in, zin, o);
   }
-  std::vector<Stage> stages;
-  { Stage a; a.kind = Stage::RES3D; a.rb = &g.mid1; stages.push_back(a); }
-  { Stage a; a.kind = Stage::ATTN; a.at = &g.attn; stages.push_back(a); }
-  { Stage a; a.kind = Stage::RES3D; a.rb = &g.mid2; stages.push_back(a); }
-  for (int l = (int)g.levels.size() - 1; l >= 0; --l) {
-    const LevelW& lv = g.levels[l];
-    for (size_t b = 0; b < lv.blk.size(); ++b) {
-      Stage a; a.kind = Stage::RES2D; a.rb = &lv.blk[b]; stages.push_back(a);
-      Stage t; t.kind = Stage::RES1D; t.rb = &lv.tblk[b]; stages.push_back(t);
-    }
-    if (lv.has_resample) {
-      Stage a; a.kind = Stage::UP; a.lv = &lv; stages.push_back(a);
-      if (lv.has_tres) { Stage t; t.kind = Stage::TUP; t.lv = &lv; stages.push_back(t); }  // nested as model_3dcausal.py:844-853
-    }
-  }
-  { Stage a; a.kind = Stage::HEAD; a.head_norm = &g.norm_out; stages.push_back(a); }
-  run_stages(ex, st, stages);
+  run_stages(ex, st, decoder_stages(g));
   Act n = ex.take_norm(st, g.norm_out, true, false);
   ex.free_act(st.x);
   if (ex.prec == VT_PREC_BF16 && m->head_planes.Kpad > 0 && n.W % 8 == 0) {
@@ -1338,6 +1346,45 @@ static void run_decoder(Exec& ex, const float* z_ext, int B, int Tz, int Hz, int
   if (d.version == 0 && !d.noncausal && (!ex.streaming() || ex.ck->first)) o.to_off = d.time_downsample_factor - 1;
   ex.conv(g.conv_out, n, o);
   ex.free_act(n);
+}
+
+// ---- temporal reach (vt_temporal_reach) ----------------------------------------------------------------------------------
+// Composed over the stages the executor runs.  A causal conv of kt taps reads kt-1 frames of its own axis back; spatial
+// blocks and resampling, attention and the norms work within a frame.
+static int res_back(const ResBlockW& r) { return (r.c1.kt - 1) + (r.c2.kt - 1); }   // the nin shortcut is 1x1
+// Encoder: how many input frames before its group's first frame a latent frame reads.  `rate`: input frames per frame of the
+// stage.  The time downsample's output frame o reads frames 2o-1 .. 2o+1 (the stride-2 conv's kt-2 front frames, and the
+// avg pool's one-frame cache).
+static int64_t encoder_reach(const vt_model* m) {
+  const StackW& e = m->enc;
+  int64_t rate = 1, back = e.conv_in.kt - 1;
+  for (const Stage& sg : encoder_stages(e)) {
+    if (sg.kind == Stage::RES1D || sg.kind == Stage::RES3D) back += res_back(*sg.rb) * rate;
+    if (sg.kind == Stage::TDOWN) {
+      back += std::max(sg.lv->tconv.kt - 2, 1) * rate;
+      rate *= 2;
+    }
+  }
+  return back + (e.conv_out.kt - 1) * rate;
+}
+// Decoder: the last frame of each stage's output that latent frame 0 changes, in frames of that stage; the answer is the
+// latent frame the last decoded frame it changes belongs to.  Time upsampling maps input frame i to output frames up to 2i+1
+// (nearest) or 2i+2 (trilinear: output 2i+2 interpolates from frame i).  Without overlap the trilinear cache is x[-2n:-n] of
+// the previous chunk, so the first output frame 2a of a chunk starting at frame a interpolates from frame a-n-1, and frame i
+// reaches 2n frames further when i+1 is a multiple of n (a chunk start for some t_chunk_dec).  With overlap the cache holds
+// the n frames before the chunk (model_3dcausal_v1_1.py:329-340, autoencoder_v1_1.py:307-320).
+static int64_t decoder_reach(const vt_model* m, bool overlap) {
+  const StackW& g = m->dec;
+  const bool tri = m->desc.interpolation_mode == VT_INTERP_TRILINEAR;
+  int64_t last = g.conv_in.kt - 1;
+  for (const Stage& sg : decoder_stages(g)) {
+    if (sg.kind == Stage::RES1D || sg.kind == Stage::RES3D) last += res_back(*sg.rb);
+    if (sg.kind == Stage::TUP) {
+      const int64_t n = sg.lv->num_temp_upsample, i = last - (last + 1) % n;   // the last changed frame a chunk start reads
+      last = (tri ? std::max(2 * last + 2, overlap ? 0 : 2 * i + 2 + 2 * n) : 2 * last + 1) + (sg.lv->tconv.kt - 1);
+    }
+  }
+  return (last + g.conv_out.kt - 1) / m->desc.time_downsample_factor;
 }
 
 static int latent_shape(const vt_model* m, int T, int H, int W, int* Tz, int* Hz, int* Wz) {
@@ -1840,6 +1887,13 @@ int32_t vt_encode_chunk(vt_chunk_state* cs, int32_t is_first, const float* x_chu
   return encode_chunk(cs, is_first, x_chunk, C, Tc, noise, z, indices, kl_loss, nullptr, workspace, workspace_bytes, stream);
 }
 
+int32_t vt_encode_chunk_pre(vt_chunk_state* cs, int32_t is_first, const float* x_chunk, int32_t C, int32_t Tc, const float* noise,
+                            float* z, int32_t* indices, float* kl_loss, float* h_pre, void* workspace, int64_t workspace_bytes,
+                            void* stream) {
+  if (!h_pre) return fail(VT_ERR_INVALID, "null argument");
+  return encode_chunk(cs, is_first, x_chunk, C, Tc, noise, z, indices, kl_loss, h_pre, workspace, workspace_bytes, stream);
+}
+
 int32_t vt_decode_chunk(vt_chunk_state* cs, int32_t is_first, const float* z_chunk, int32_t Cz, int32_t Tzc, float* x_out,
                         void* workspace, int64_t workspace_bytes, void* stream) {
   if (!cs || !z_chunk || !x_out) return fail(VT_ERR_INVALID, "null argument");
@@ -1958,6 +2012,16 @@ int32_t vt_decode_video_frames(const vt_model* m, int32_t Tz, int32_t t_chunk_de
     total += vt_decoded_frames(m, c.e - c.s + (look ? 1 : 0)) - (look ? tdf : 0);
   }
   return total;
+}
+
+int32_t vt_temporal_reach(const vt_model* m, int32_t is_decoder, int32_t use_overlap, int32_t* frames) {
+  if (!m || !frames) return fail(VT_ERR_INVALID, "null argument");
+  if (m->desc.noncausal)
+    return fail(VT_ERR_INVALID, "non-causal models have no one-sided temporal reach: their time padding is symmetric, so a frame depends on later frames");
+  if (m->desc.version != 1) return fail(VT_ERR_INVALID, "the temporal reach is defined for the v1.1 model family (v1.0 models run whole clips)");
+  if (use_overlap && !is_decoder) return fail(VT_ERR_INVALID, "use_overlap is a decoder option");
+  *frames = (int32_t)(is_decoder ? decoder_reach(m, use_overlap != 0) : encoder_reach(m));
+  return VT_OK;
 }
 
 // FSQ aux-loss partials of every chunk (vt_encode_video_fsq_aux): chunk i writes stats[2i..2i+1] and avg_prob[i*J ..)

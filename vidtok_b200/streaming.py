@@ -172,12 +172,17 @@ class _Stream:
 
 
 class EncodeStream(_Stream):
-    def __init__(self, model, batch: int, H: int, W: int, t_chunk: Optional[int] = None):
+    """keep_pre_bound: reg_log also holds "h_pre", the encoder output before the regularizer of this push's latent frames
+    ([B, 2z|z, tz, Hz, Wz]), so that a caller can form per-sample losses of a batched stream; the stream's own FSQ aux loss
+    is then not formed."""
+
+    def __init__(self, model, batch: int, H: int, W: int, t_chunk: Optional[int] = None, keep_pre_bound: bool = False):
         super().__init__(model, batch, H, W, is_decoder=False, t_chunk=t_chunk)
+        self.keep_pre = bool(keep_pre_bound)
         self.pending: Optional[torch.Tensor] = None
         self.Hz, self.Wz = self.native.latent_shape(1, H, W)[1:]
         self.reg = model.regularization
-        self.aux = self.spec.regularizer == "fsq" and self.reg.aux_enabled()
+        self.aux = self.spec.regularizer == "fsq" and self.reg.aux_enabled() and not self.keep_pre
         if self.aux:
             dev, J = self.native.device, self.reg.codebook_size
             self.aux_stats = torch.empty((1, 2), dtype=torch.float32, device=dev)   # one chunk's partials
@@ -245,6 +250,8 @@ class EncodeStream(_Stream):
         z = torch.empty((self.B, s.z_channels, Tz, self.Hz, self.Wz), dtype=torch.float32, device=dev)
         idx = torch.empty((self.B, Tz, self.Hz, self.Wz), dtype=torch.int32, device=dev) if s.regularizer == "fsq" else None
         kls = torch.zeros((max(len(chunks), 1),), dtype=torch.float32, device=dev)
+        hC = (2 if s.double_z else 1) * s.z_channels
+        h = torch.empty((self.B, hC, Tz, self.Hz, self.Wz), dtype=torch.float32, device=dev) if self.keep_pre else None
         lib, stream = self.native.lib, _stream_ptr(dev)
         t0 = tz0 = 0
         for i, (n, tz) in enumerate(zip(chunks, tzs)):
@@ -252,7 +259,14 @@ class EncodeStream(_Stream):
             zc = torch.empty((self.B, s.z_channels, tz, self.Hz, self.Wz), dtype=torch.float32, device=dev)
             ic = torch.empty((self.B, tz, self.Hz, self.Wz), dtype=torch.int32, device=dev) if idx is not None else None
             nc = noise[:, :, tz0:tz0 + tz].contiguous() if kl_noise else None
-            if self.aux:
+            if self.keep_pre:
+                ws = self._workspace(n)
+                hc = torch.empty((self.B, hC, tz, self.Hz, self.Wz), dtype=torch.float32, device=dev)
+                N.check(lib.vt_encode_chunk_pre(self.state.handle, int(self.first), _ptr(xc), s.in_channels, n, _ptr(nc), _ptr(zc),
+                                                _ptr(ic), _ptr(kls[i:i + 1]) if s.regularizer == "kl" else None, _ptr(hc), _ptr(ws),
+                                                ws.numel(), stream))
+                h[:, :, tz0:tz0 + tz] = hc
+            elif self.aux:
                 ws = self.state.aux_workspace(n)
                 N.check(lib.vt_encode_chunk_fsq_aux(self.state.handle, int(self.first), _ptr(xc), s.in_channels, n, _ptr(zc), _ptr(ic),
                                                     100.0, _ptr(self.aux_stats), _ptr(self.aux_avg), _ptr(ws), ws.numel(), stream))
@@ -277,12 +291,16 @@ class EncodeStream(_Stream):
                 self.aux_loss = self.reg.aux_finalize((self.tok_stats / self.tokens).float().view(1, 2),
                                                       (self.tok_avg / self.tokens).float().view(1, -1),
                                                       n_steps=self.model.global_step // 2, world_size=1)
-            return z.to(self.out_dtype), {"indices": idx, "aux_loss": self.aux_loss}
-        if self.t_chunk is None:
-            kl = kls.sum()
+            log = {"indices": idx, "aux_loss": self.aux_loss}
         else:
-            kl = self._mean(self.kl_sum, self.n_chunks) if self.n_chunks else torch.zeros((), dtype=torch.float32, device=dev)
-        return z.to(self.out_dtype), {"kl_loss": kl}
+            if self.t_chunk is None:
+                kl = kls.sum()
+            else:
+                kl = self._mean(self.kl_sum, self.n_chunks) if self.n_chunks else torch.zeros((), dtype=torch.float32, device=dev)
+            log = {"kl_loss": kl}
+        if self.keep_pre:
+            log["h_pre"] = h
+        return z.to(self.out_dtype), log
 
     @staticmethod
     def _mean(total: torch.Tensor, n: int) -> torch.Tensor:
