@@ -101,6 +101,18 @@ def test_latent_geometry_and_workspace_dry_run():
     assert NativeModel(spec5).latent_shape(17, 512, 512) == (5, 32, 32)
 
 
+def test_load_refusals_name_the_parameter():
+    from vidtok_b200 import _native as N
+    from vidtok_b200.engine import NativeModel, TokenizerSpec
+    nm = NativeModel(TokenizerSpec(version=0, ch=128, ch_mult=(1, 2, 4, 4), num_res_blocks=2, z_channels=4, double_z=True,
+                                   norm_type="layernorm"))
+    buf = (C.c_float * 128)()
+    assert N.lib().vt_model_load_param(nm.handle, b"encoder.conv_in.bias", buf, 128, 0, None) == -1
+    assert N.lib().vt_last_error() == b"unknown parameter encoder.conv_in.bias"
+    assert N.lib().vt_model_load_param(nm.handle, b"encoder.conv_in.conv.bias", buf, 127, 0, None) == -1
+    assert N.lib().vt_last_error() == b"parameter encoder.conv_in.conv.bias: expected 128 elements, got 127"
+
+
 @pytest.mark.skipif(torch.cuda.is_available(), reason="checks the no-GPU failure mode")
 def test_product_path_fails_loudly_without_gpu():
     from vidtok_b200.compat_util import instantiate_from_config

@@ -1,5 +1,7 @@
-"""FVD without a GPU: the I3D state-dict layout, the oracle's end-point shapes and preprocessing, the Frechet distance
-against scipy, the feature windows of Scorer and the all-reduce of the feature statistics over two gloo ranks."""
+"""FVD without a GPU: the I3D state-dict layout, the library's I3D parameter table and load refusals, the oracle's end-point
+shapes and preprocessing, the Frechet distance against scipy, the feature windows of Scorer and the all-reduce of the feature
+statistics over two gloo ranks."""
+import ctypes as C
 import math
 import os
 import socket
@@ -11,6 +13,7 @@ import torch.multiprocessing as mp
 import torch.nn.functional as F
 
 from oracle.i3d_oracle import fvd_fp64, i3d_fp64, preprocess, resized_size, synthetic_i3d_state
+from vidtok_b200 import _native as N
 from vidtok_b200.metrics import (I3D, I3D_ENDPOINTS, features_to_stats, fvd, fvd_from_stats, fvd_windows, i3d_state,
                                  i3d_state_shapes)
 
@@ -29,6 +32,30 @@ def test_state_layout():
     bad = dict(sd, **{"Mixed_3c.b1b.conv3d.weight": torch.zeros(192, 128, 3, 3, 1)})
     with pytest.raises(ValueError, match="Mixed_3c.b1b.conv3d.weight"):
         i3d_state(bad)
+
+
+def test_native_manifest_and_load_refusals():
+    lib, h = N.lib(), C.c_void_p()
+    N.check(lib.vt_i3d_create(0, C.byref(h)))
+    try:
+        native = {}
+        for i in range(lib.vt_i3d_num_params(h)):
+            name, shape, nd = C.create_string_buffer(128), (C.c_int64 * 5)(), C.c_int32()
+            N.check(lib.vt_i3d_param_info(h, i, name, 128, shape, C.byref(nd)))
+            native[name.value.decode()] = tuple(shape[:nd.value])
+        assert native == i3d_state_shapes()
+        assert lib.vt_i3d_param_info(h, len(native), None, 0, None, None) == -1
+        assert lib.vt_last_error() == b"bad parameter index"
+        buf = (C.c_float * 64)()
+        assert lib.vt_i3d_load_param(h, b"Conv3d_1a_7x7.bn.scale", buf, 64, 0, None) == -1
+        assert lib.vt_last_error() == b"unknown I3D parameter Conv3d_1a_7x7.bn.scale"
+        assert lib.vt_i3d_load_param(h, b"Conv3d_1a_7x7.bn.bias", buf, 63, 0, None) == -1
+        assert lib.vt_last_error() == b"parameter Conv3d_1a_7x7.bn.bias: expected 64 elements, got 63"
+        N.check(lib.vt_i3d_load_param(h, b"Conv3d_1a_7x7.bn.bias", buf, 64, 0, None))   # host memory: no device needed
+        assert lib.vt_i3d_finalize(h, None) == -3
+        assert lib.vt_last_error() == b"I3D parameter Conv3d_1a_7x7.conv3d.weight was never loaded"
+    finally:
+        lib.vt_i3d_destroy(h)
 
 
 def test_synthetic_state_is_seeded():

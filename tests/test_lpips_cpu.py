@@ -33,6 +33,33 @@ def test_key_table_matches_the_library_and_the_oracle():
     assert len(native) == 31 and native["net.slice5.28.weight"] == (512, 512, 3, 3) and native["lin0.model.1.weight"] == (1, 64, 1, 1)
 
 
+def test_load_refusals_name_the_parameter():
+    lib, h = N.lib(), C.c_void_p()
+    N.check(lib.vt_lpips_create(0, C.byref(h)))
+    buf = (C.c_float * 64)()
+    try:
+        assert lib.vt_lpips_load_param(h, b"net.slice1.1.weight", buf, 64, 0, None) == -1
+        assert lib.vt_last_error() == b"unknown LPIPS parameter net.slice1.1.weight"
+        assert lib.vt_lpips_load_param(h, b"net.slice1.0.bias", buf, 63, 0, None) == -1
+        assert lib.vt_last_error() == b"parameter net.slice1.0.bias: expected 64 elements, got 63"
+        assert lib.vt_lpips_finalize(h, None) == -3
+        assert lib.vt_last_error() == b"LPIPS parameter net.slice1.0.weight was never loaded"
+    finally:
+        lib.vt_lpips_destroy(h)
+
+
+@pytest.mark.skipif(torch.cuda.is_available(), reason="checks the no-GPU failure mode")
+def test_load_fails_loudly_without_gpu():
+    lib, h = N.lib(), C.c_void_p()
+    N.check(lib.vt_lpips_create(0, C.byref(h)))
+    buf = (C.c_float * 64)()
+    try:
+        assert lib.vt_lpips_load_param(h, b"net.slice1.0.bias", buf, 64, 0, None) == -5
+        assert b"no CPU fallback" in lib.vt_last_error()
+    finally:
+        lib.vt_lpips_destroy(h)
+
+
 def test_loader_takes_both_checkpoint_forms_and_refuses_bad_ones():
     ref = synthetic_lpips_state(1)
     ref_full = dict(ref, **{"scaling_layer.shift": torch.tensor([-.030, -.088, -.188])[None, :, None, None],

@@ -1,16 +1,42 @@
 // Internal model representation: parameter manifest, packed weights, layer structure (mirrors the module
-// tree of vidtok/modules/model_3dcausal.py:502-885) and the arena used by the executor.
+// tree of vidtok/modules/model_3dcausal.py:502-885) and the arena used by the executor.  Also the host helpers that the
+// tokenizer (model.cu) and the evaluation networks (eval_nets.cu) share: errors, parameter sets, weight packing and the
+// ConvP layout of their convolutions.
 #pragma once
 #include <cuda_runtime.h>
 
+#include <cstring>
 #include <map>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/vidtok_b200.h"
 #include "kernels.h"
 
 namespace vt {
+
+// ---- errors: fail() sets the message vt_last_error returns and passes the code through ---------------------------------
+int fail(int code, const char* fmt, ...);
+#define VT_CUDA(call)                                                                         \
+  do {                                                                                        \
+    cudaError_t _e = (call);                                                                  \
+    if (_e != cudaSuccess)                                                                    \
+      return fail(VT_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(_e), __FILE__, __LINE__); \
+  } while (0)
+
+inline size_t align_up(size_t n, size_t a) { return (n + a - 1) / a * a; }
+
+// Makes `device` current; VT_ERR_NO_DEVICE when no CUDA device is visible
+inline int use_device(int device) {
+  int n = 0;
+  if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) {
+    cudaGetLastError();
+    return fail(VT_ERR_NO_DEVICE, "no CUDA device visible: vidtok_b200 has no CPU fallback");
+  }
+  VT_CUDA(cudaSetDevice(device));
+  return VT_OK;
+}
 
 struct Param {
   std::string name;
@@ -19,6 +45,144 @@ struct Param {
   int64_t offset = 0;  // element offset into the raw fp32 pool
   bool loaded = false;
 };
+
+// The parameters of one network under the reference's checkpoint keys, with their offsets into an fp32 pool of pool_elems
+// elements.  `net` names the network in the load errors ("LPIPS ", "I3D ", or "" for the tokenizer).
+struct ParamSet {
+  const char* net;
+  std::vector<Param> list;
+  std::map<std::string, int> index;
+  int64_t pool_elems = 0;
+  explicit ParamSet(const char* net) : net(net) {}
+  int size() const { return (int)list.size(); }
+  Param& operator[](int i) { return list[i]; }
+  const Param& operator[](int i) const { return list[i]; }
+  int add(const std::string& name, std::vector<int64_t> shape) {
+    Param p;
+    p.name = name;
+    p.shape = shape;
+    p.numel = 1;
+    for (auto s : shape) p.numel *= s;
+    p.offset = pool_elems;
+    pool_elems += (p.numel + 3) / 4 * 4;  // keep every tensor 16-byte aligned
+    index[name] = size();
+    list.push_back(p);
+    return size() - 1;
+  }
+  // the index of parameter `name` holding numel elements; -1 after fail(VT_ERR_INVALID)
+  int find(const char* name, int64_t numel) const {
+    auto it = index.find(name);
+    if (it == index.end()) {
+      fail(VT_ERR_INVALID, "unknown %sparameter %s", net, name);
+      return -1;
+    }
+    const Param& p = list[it->second];
+    if (p.numel != numel) {
+      fail(VT_ERR_INVALID, "parameter %s: expected %lld elements, got %lld", name, (long long)p.numel, (long long)numel);
+      return -1;
+    }
+    return it->second;
+  }
+  int check_loaded() const {
+    for (const Param& p : list)
+      if (!p.loaded) return fail(VT_ERR_NOT_READY, "%sparameter %s was never loaded", net, p.name.c_str());
+    return VT_OK;
+  }
+  // *_param_info: the shape padded with 1 to shape_len entries
+  int info(int i, char* name, int cap, int64_t* shape, int shape_len, int32_t* ndim) const {
+    if (i < 0 || i >= size()) return fail(VT_ERR_INVALID, "bad parameter index");
+    const Param& p = list[i];
+    if (name && cap > 0) {
+      strncpy(name, p.name.c_str(), cap - 1);
+      name[cap - 1] = 0;
+    }
+    if (ndim) *ndim = (int)p.shape.size();
+    if (shape)
+      for (size_t k = 0; k < (size_t)shape_len; ++k) shape[k] = k < p.shape.size() ? p.shape[k] : 1;
+    return VT_OK;
+  }
+};
+
+// ---- weight packing ------------------------------------------------------------------------------------------------------
+// The power-of-two scales (split_weight_scale) of the split copies of fp32 device tensors {pointer, elements}: one max |w|
+// per tensor on stream s, read back once
+inline int split_weight_scales(const std::vector<std::pair<const float*, long long>>& w, float headroom, cudaStream_t s,
+                               float* scale) {
+  float* d_max = nullptr;
+  VT_CUDA(cudaMalloc(&d_max, w.size() * sizeof(float)));
+  std::vector<float> h_max(w.size());
+  cudaError_t e = cudaSuccess;
+  for (size_t i = 0; i < w.size() && e == cudaSuccess; ++i) e = launch_absmax(w[i].first, w[i].second, d_max + i, s);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(h_max.data(), d_max, h_max.size() * sizeof(float), cudaMemcpyDeviceToHost, s);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+  cudaFree(d_max);
+  if (e != cudaSuccess) return fail(VT_ERR_CUDA, "weight scales: %s", cudaGetErrorString(e));
+  for (size_t i = 0; i < w.size(); ++i) scale[i] = split_weight_scale(h_max[i], headroom);
+  return VT_OK;
+}
+// A convolution's wgmma weights from fp32 w [Co][Ci][taps]: the bf16 copy [Co_pad][Kpad] at nk, the split copy of w * wscale3
+// at nk3
+inline cudaError_t pack_conv_weights(const float* w, bf16* nk, bf16* nk3, int Co, int Co_pad, int Ci, int taps, int Kpad,
+                                     float wscale3, cudaStream_t s) {
+  const cudaError_t e = launch_pack_w_nk_bf16(w, nk, Co, Co_pad, Ci, taps, Kpad, s);
+  return e == cudaSuccess ? launch_pack_w_nk_bf16(w, nk3, Co, Co_pad, Ci, taps, Kpad, s, wscale3) : e;
+}
+
+// ---- ConvP layout: every descriptor the executors and the operator entry points launch is built from these --------------
+// zeroed but for the input extent, unit strides and unit upsampling
+inline ConvP conv_p(int B, int Ti, int Hi, int Wi, int Ci) {
+  ConvP p;
+  memset(&p, 0, sizeof(p));
+  p.B = B; p.Ti = Ti; p.Hi = Hi; p.Wi = Wi; p.Ci = Ci;
+  p.st = p.sh = p.sw = 1; p.ut = p.uh = p.uw = 1;
+  return p;
+}
+// element strides of one operand
+struct Strides { long long B, T, H, W, C; };
+// channels-last [B][T][H][W][C] with cw storage elements per channel (2 for split rows); bs >= 0 overrides the batch stride
+// (views into a larger tensor)
+inline Strides cl_strides(int T, int H, int W, int C, long long cw, long long bs = -1) {
+  const long long sW = cw * C, sH = W * sW, sT = H * sH;
+  return {bs >= 0 ? bs : T * sT, sT, sH, sW, 1};
+}
+inline void set_in(ConvP& p, const Strides& s) { p.isB = s.B; p.isT = s.T; p.isH = s.H; p.isW = s.W; p.isC = s.C; }
+inline void set_out(ConvP& p, const Strides& s) { p.osB = s.B; p.osT = s.T; p.osH = s.H; p.osW = s.W; p.osC = s.C; }
+// To / Ho / Wo from the input extent, taps, strides, upsampling and front padding already in p; pt_back, ph1, pw1: the
+// padding behind the end of each axis.  False when the output is empty.
+inline bool conv_out_size(ConvP& p, int pt_back, int ph1, int pw1) {
+  p.To = (p.t_rep + p.ut * p.Ti + p.pt + pt_back - p.kt) / p.st + 1 - p.to_off;
+  p.Ho = (p.uh * p.Hi + p.ph + ph1 - p.kh) / p.sh + 1;
+  p.Wo = (p.uw * p.Wi + p.pw + pw1 - p.kw) / p.sw + 1;
+  return p.To > 0 && p.Ho > 0 && p.Wo > 0;
+}
+// The conv_tc plan of a stride-1 convolution with bias and ReLU (LPIPS, I3D) over a channels-last input of Ci_s stored
+// channels: kt x ks x ks taps, zero padding pt / pt_back in front of / behind the time axis and ps / ps_back on the spatial
+// axes.  It writes Co channels of a channels-last output of out_Cs channels (a slice when out_Cs > Co: the caller offsets the
+// output pointer); split: acc_scale 1 / wscale3.
+inline bool relu_conv_plan(int B, int T, int H, int W, int Ci_s, int kt, int ks, int pt, int pt_back, int ps, int ps_back, int Co,
+                           int out_Cs, const float* bias, float wscale3, bool split, TcPlan* pl) {
+  const long long cw = split ? 2 : 1;
+  ConvP p = conv_p(B, T, H, W, Ci_s);
+  p.split = split ? 1 : 0;
+  set_in(p, cl_strides(T, H, W, Ci_s, cw));
+  p.kt = kt; p.kh = p.kw = ks;
+  p.pt = pt; p.ph = p.pw = ps;
+  p.Co = Co;
+  conv_out_size(p, pt_back, ps_back, ps_back);
+  set_out(p, cl_strides(p.To, p.Ho, p.Wo, out_Cs, cw));
+  p.bias = bias;
+  p.ra = 0.f; p.rb = 1.f;
+  p.relu = 1;
+  p.acc_scale = split ? 1.0f / wscale3 : 0.f;
+  if (!conv_tc_plan(p, split ? DT_SPLIT : DT_BF16, nullptr, nullptr, 1, pl)) return false;
+  if (out_Cs != Co) pl->o_lo = out_Cs;
+  return true;
+}
+
+// One operator launch of the kernel the model path uses for that precision (vt_op_conv, vt_op_conv_ex, vt_op_conv_relu, ...)
+int op_conv_impl(int precision, int force_simt, const vt_conv_desc* d, const vt_conv_ex* e, const void* x, const void* cache,
+                 const float* w, const float* bias, const void* res, const float* gamma, const float* beta, void* out, void* out2,
+                 cudaStream_t s, const TcRegFusion* reg = nullptr, bool relu = false);
 
 struct ConvW {
   int Co = 0, Ci = 0, kt = 1, kh = 1, kw = 1;
@@ -94,10 +258,8 @@ struct Arena {
 struct vt_model {
   vt_model_desc desc;
   int device = 0;
-  std::vector<vt::Param> params;
-  std::map<std::string, int> index;
+  vt::ParamSet params{""};
   float* pool = nullptr;        // raw fp32 parameters (reference layout)
-  int64_t pool_elems = 0;
   float* packed_kn = nullptr;   // all [K][Co] fp32 repacks
   vt::bf16* packed_nk = nullptr;
   vt::bf16* packed_nk3 = nullptr;      // split (hi|lo) copies of every wgmma weight matrix

@@ -213,7 +213,6 @@ def _means(sums: torch.Tensor) -> dict:
 
 
 # ---- LPIPS (vidtok/modules/lpips.py; scripts/inference_evaluate.py:175-186) ------------------------------------------------
-_LPIPS_PRECISIONS = {"exact": N.PREC_EXACT_TC, "bf16": N.PREC_BF16}
 _LPIPS_CONVS = ((1, 0), (1, 2), (2, 5), (2, 7), (3, 10), (3, 12), (3, 14), (4, 17), (4, 19), (4, 21), (5, 24), (5, 26), (5, 28))
 _LPIPS_COUT = (64, 64, 128, 128, 256, 256, 256, 512, 512, 512, 512, 512, 512)
 _LPIPS_CHNS = (64, 128, 256, 512, 512)
@@ -270,35 +269,70 @@ def lpips_pass_frames(H: int, W: int) -> int:
     return int(N.lib().vt_lpips_pass_frames(H, W))
 
 
-class LPIPS:
-    """LPIPS with VGG16 on the device (vidtok/modules/lpips.py as scripts/inference_evaluate.py calls it): owns the library's
-    weight handle.  precision "exact" (the default: fp32-class results through the split-fp16 tensor-core operands, as the
-    script's fp32 run) or "bf16".  Build it with from_state_dict or from_files; score with lpips_scores or Scorer(lpips=...)."""
+# The precisions of the evaluation networks (LPIPS, I3D)
+_EVAL_PRECISIONS = {"exact": N.PREC_EXACT_TC, "bf16": N.PREC_BF16}
+
+
+class _EvalNet:
+    """The library's weight handle of an evaluation network (the C functions vt_<_net>_*): created on the model's device with
+    every parameter of _state(state) loaded and finalized, released by close().  _host_load: the parameters are loaded from
+    host tensors rather than from copies on the device."""
+    _net: str                # "lpips" or "i3d"
+    _state: staticmethod     # the state-dict check of the network (lpips_state, i3d_state)
+    _host_load = False
 
     def __init__(self, state: dict, device=None, precision: str = "exact"):
-        if precision not in _LPIPS_PRECISIONS:
-            raise ValueError(f"precision must be one of {sorted(_LPIPS_PRECISIONS)}, got {precision!r}")
+        if precision not in _EVAL_PRECISIONS:
+            raise ValueError(f"precision must be one of {sorted(_EVAL_PRECISIONS)}, got {precision!r}")
         self.precision = precision
         self.device = torch.device(device) if device is not None else torch.device("cuda")
         if self.device.index is None:
             self.device = torch.device(self.device.type, torch.cuda.current_device())
-        state = lpips_state(state)
+        state = self._state(state)
         h = C.c_void_p()
-        N.check(N.lib().vt_lpips_create(self.device.index, C.byref(h)))
+        N.check(self._fn("create")(self.device.index, C.byref(h)))
         self._h = h
         with torch.cuda.device(self.device):
-            stream = torch.cuda.current_stream(self.device)
+            stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
             keep = []
             for key, v in state.items():
-                t = v.detach().to(self.device, torch.float32).contiguous()
+                t = v.detach().to("cpu" if self._host_load else self.device, torch.float32).contiguous()
                 keep.append(t)
-                N.check(N.lib().vt_lpips_load_param(h, key.encode(), C.c_void_p(t.data_ptr()), t.numel(), 1, C.c_void_p(stream.cuda_stream)))
-            N.check(N.lib().vt_lpips_finalize(h, C.c_void_p(stream.cuda_stream)))
+                N.check(self._fn("load_param")(h, key.encode(), C.c_void_p(t.data_ptr()), t.numel(), int(not self._host_load), stream))
+            N.check(self._fn("finalize")(h, stream))
             del keep
 
+    def _fn(self, name: str):
+        return getattr(N.lib(), f"vt_{self._net}_{name}")
+
     @classmethod
-    def from_state_dict(cls, sd: dict, device=None, precision: str = "exact") -> "LPIPS":
+    def from_state_dict(cls, sd: dict, device=None, precision: str = "exact"):
         return cls(sd, device, precision)
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._fn("destroy")(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _workspace_bytes(self, geom) -> int:
+        need = self._fn("workspace_bytes")(self._h, _EVAL_PRECISIONS[self.precision], *geom)
+        if need < 0:
+            raise ValueError(N.lib().vt_last_error().decode(errors="replace"))
+        return need
+
+
+class LPIPS(_EvalNet):
+    """LPIPS with VGG16 on the device (vidtok/modules/lpips.py as scripts/inference_evaluate.py calls it): owns the library's
+    weight handle.  precision "exact" (the default: fp32-class results through the split-fp16 tensor-core operands, as the
+    script's fp32 run) or "bf16".  Build it with from_state_dict or from_files; score with lpips_scores or Scorer(lpips=...)."""
+    _net = "lpips"
+    _state = staticmethod(lpips_state)
 
     @classmethod
     def from_files(cls, vgg16_path: str | None = None, lpips_path: str | None = None, device=None, precision: str = "exact") -> "LPIPS":
@@ -314,23 +348,6 @@ class LPIPS:
             sd.update(torch.load(path, map_location="cpu", weights_only=True))
         return cls(sd, device, precision)
 
-    def close(self):
-        if getattr(self, "_h", None):
-            N.lib().vt_lpips_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def _workspace_bytes(self, geom) -> int:
-        need = N.lib().vt_lpips_workspace_bytes(self._h, _LPIPS_PRECISIONS[self.precision], *geom)
-        if need < 0:
-            raise ValueError(N.lib().vt_last_error().decode(errors="replace"))
-        return need
-
     def _launch(self, x, y, geom, running, workspace, per_layer=False):
         B, Cc, T, H, W = geom
         if x.device != self.device:
@@ -341,7 +358,7 @@ class LPIPS:
             out = torch.empty(shape, dtype=torch.float32, device=x.device)
             layers = torch.empty(shape + (5,), dtype=torch.float32, device=x.device) if per_layer else None
             N.check(N.lib().vt_lpips(
-                self._h, _LPIPS_PRECISIONS[self.precision], C.c_void_p(x.data_ptr()), _DTYPES[x.dtype], C.c_void_p(y.data_ptr()),
+                self._h, _EVAL_PRECISIONS[self.precision], C.c_void_p(x.data_ptr()), _DTYPES[x.dtype], C.c_void_p(y.data_ptr()),
                 _DTYPES[y.dtype], B, Cc, T, H, W, C.c_void_p(out.data_ptr()), C.c_void_p(layers.data_ptr()) if per_layer else None,
                 C.c_void_p(running.data_ptr()) if running is not None else None, C.c_void_p(workspace.data_ptr()), workspace.numel(),
                 C.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)))
@@ -426,32 +443,13 @@ def _clip_geometry(x: torch.Tensor):
     return tuple(int(d) for d in x.shape)
 
 
-class I3D:
+class I3D(_EvalNet):
     """The FVD feature network on the device: owns the library's I3D weight handle.  precision "exact" (the default:
     fp32-class results through the split-fp16 tensor-core operands) or "bf16".  Build it with from_state_dict or from_files;
     use it with i3d_features or Scorer(i3d=...)."""
-
-    def __init__(self, state: dict, device=None, precision: str = "exact"):
-        if precision not in _LPIPS_PRECISIONS:
-            raise ValueError(f"precision must be one of {sorted(_LPIPS_PRECISIONS)}, got {precision!r}")
-        self.precision = precision
-        self.device = torch.device(device) if device is not None else torch.device("cuda")
-        if self.device.index is None:
-            self.device = torch.device(self.device.type, torch.cuda.current_device())
-        state = i3d_state(state)
-        h = C.c_void_p()
-        N.check(N.lib().vt_i3d_create(self.device.index, C.byref(h)))
-        self._h = h
-        with torch.cuda.device(self.device):
-            stream = torch.cuda.current_stream(self.device)
-            for key, v in state.items():
-                t = v.detach().to("cpu", torch.float32).contiguous()
-                N.check(N.lib().vt_i3d_load_param(h, key.encode(), C.c_void_p(t.data_ptr()), t.numel(), 0, C.c_void_p(stream.cuda_stream)))
-            N.check(N.lib().vt_i3d_finalize(h, C.c_void_p(stream.cuda_stream)))
-
-    @classmethod
-    def from_state_dict(cls, sd: dict, device=None, precision: str = "exact") -> "I3D":
-        return cls(sd, device, precision)
+    _net = "i3d"
+    _state = staticmethod(i3d_state)
+    _host_load = True   # finalize folds BatchNorm into the weights on the host
 
     @classmethod
     def from_files(cls, path: str | None = None, device=None, precision: str = "exact") -> "I3D":
@@ -462,26 +460,9 @@ class I3D:
             raise FileNotFoundError(f"I3D weights not found: {path}")
         return cls(torch.load(path, map_location="cpu", weights_only=True), device, precision)
 
-    def close(self):
-        if getattr(self, "_h", None):
-            N.lib().vt_i3d_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
     def pass_clips(self, T: int, H: int, W: int) -> int:
         """Clips per pass of the executor: 8, or fewer where an activation of the pass would exceed 2^31 elements."""
         return int(N.lib().vt_i3d_pass_clips(self._h, T, H, W))
-
-    def _workspace_bytes(self, geom) -> int:
-        need = N.lib().vt_i3d_workspace_bytes(self._h, _LPIPS_PRECISIONS[self.precision], *geom)
-        if need < 0:
-            raise ValueError(N.lib().vt_last_error().decode(errors="replace"))
-        return need
 
     def _launch(self, x, stats, workspace):
         geom = _clip_geometry(x)
@@ -491,7 +472,7 @@ class I3D:
         with torch.cuda.device(x.device):
             feats = torch.empty((geom[0], I3D_FEATURES), dtype=torch.float32, device=x.device)
             N.check(N.lib().vt_i3d_features(
-                self._h, _LPIPS_PRECISIONS[self.precision], C.c_void_p(x.data_ptr()), _DTYPES[x.dtype], *geom,
+                self._h, _EVAL_PRECISIONS[self.precision], C.c_void_p(x.data_ptr()), _DTYPES[x.dtype], *geom,
                 C.c_void_p(feats.data_ptr()), C.c_void_p(stats.data_ptr()) if stats is not None else None,
                 C.c_void_p(workspace.data_ptr()), workspace.numel(), C.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)))
         return feats
@@ -499,7 +480,7 @@ class I3D:
     def endpoint(self, x: torch.Tensor, name: str, workspace: torch.Tensor | None = None) -> torch.Tensor:
         """The activation at end point `name` (I3D_ENDPOINTS) as fp32 [B,C,T,H,W], for the tests: one pass of clips at most."""
         geom = _clip_geometry(x)
-        prec = _LPIPS_PRECISIONS[self.precision]
+        prec = _EVAL_PRECISIONS[self.precision]
         shape = (C.c_int64 * 5)()
         N.check(N.lib().vt_i3d_endpoint(self._h, prec, None, _DTYPES[x.dtype], *geom, name.encode(), None, shape, None, 0, None))
         x = x.detach().contiguous()
