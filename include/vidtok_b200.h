@@ -354,6 +354,9 @@ typedef struct vt_conv_ex {
   int32_t out_f32_ncdhw;   /* out is fp32 [B,Co,To,Ho,Wo] */
   int32_t res_mix;         /* res_mode 1 computes alpha*res + (1-alpha)*conv instead of res + conv */
   int32_t res_t_mode;      /* res_mode 3 front pad: 0 zero, 1 frame 0, 2 `cache` = 1 frame [B,1,H,W,C] */
+  int32_t pt_back;         /* zero frames behind the end of x (the non-causal family: symmetric padding, and one frame
+                            * behind the end for the stride-2 time downsample, model_3dnoncausal.py:80,86-87) */
+  int32_t res_pool_off;    /* res_mode 3 avg-pool window: frames 2t-1+off .. 2t+1+off (1: non-causal, zero frame behind the end) */
 } vt_conv_ex;
 int32_t vt_op_conv_ex(int32_t precision, const vt_conv_ex* e, const void* x, const void* cache, const float* w,
                       const float* bias, const void* res, const float* gamma, const float* beta, void* out, void* out2,
@@ -362,7 +365,7 @@ int32_t vt_op_conv_ex(int32_t precision, const vt_conv_ex* e, const void* x, con
  * distributions.py:8-18): reg_mode 1 = KL (Co = 2*zc, zc in {4,8,16}; noise NULL = the mode), 2 = FSQ (Co = zc = len(levels)).
  * h_out (fp32 [B,Co,T,H,W]) may be NULL; z fp32 [B,zc,T,H,W]; indices int32 [B,T,H,W] (FSQ); kl_loss 1 float (KL).
  * vt_op_conv_regularize: v1.0 zero time padding.  vt_op_conv_regularize_ex: e carries the geometry (e->d) and the v1.1
- * time padding (t_mode, cacheT, with `cache` as in vt_op_conv_ex); its other fields are ignored. */
+ * time padding (t_mode, cacheT, with `cache` as in vt_op_conv_ex, and pt_back); its other fields are ignored. */
 int32_t vt_op_conv_regularize(int32_t precision, const vt_conv_desc* d, const void* x, const float* w, const float* bias,
                               int32_t reg_mode, int32_t zc, const int32_t* fsq_levels, const float* noise, float* h_out,
                               float* z, int32_t* indices, float* kl_loss, void* stream);
@@ -375,16 +378,21 @@ int32_t vt_op_conv_relu(int32_t precision, const vt_conv_desc* d, const void* x,
 /* 2x2 / stride-2 max-pool (floor) of channels-last x [N,H,W,C] -> y [N,H/2,W/2,C] in the precision's activation type (bf16, or
  * hi|lo split rows compared as hi + lo); C % 8 == 0. */
 int32_t vt_op_maxpool2x2(int32_t precision, const void* x, void* y, int64_t N, int32_t H, int32_t W, int32_t C, void* stream);
-/* Encoder stem from the caller's fp32 [B,Ci,T,H,W] (t_rep replicated leading frames); out channels-last
- * [B,T+t_rep,H,W,Co] in the precision's activation type (BF16 / EXACT_TC). */
+/* Encoder stem from the caller's fp32 [B,Ci,T,H,W] (t_rep replicated leading frames, two zero frames in front); out
+ * channels-last [B,T+t_rep,H,W,Co] in the precision's activation type (BF16 / EXACT_TC). */
 int32_t vt_op_conv_stem(int32_t precision, const float* x, const float* w, const float* bias, void* out, int32_t B,
                         int32_t Ci, int32_t T, int32_t H, int32_t W, int32_t Co, int32_t t_rep, void* stream);
+/* The same with pt zero frames in front: 2 (causal, = vt_op_conv_stem) or 1 (the non-causal family: one zero frame at
+ * each end, t_rep 0). */
+int32_t vt_op_conv_stem_ex(int32_t precision, const float* x, const float* w, const float* bias, void* out, int32_t B,
+                           int32_t Ci, int32_t T, int32_t H, int32_t W, int32_t Co, int32_t t_rep, int32_t pt, void* stream);
 /* Decoder head of the BF16 mode (tap-planes GEMM + gather): x bf16 [B,T,H,W,Ci] -> out fp32 [B,Co,T-to_off,H,W]. */
 int32_t vt_op_head_planes(const void* x, const float* w, const float* bias, float* out, int32_t B, int32_t T, int32_t H,
                           int32_t W, int32_t Ci, int32_t Co, int32_t to_off, void* stream);
 /* "nearest 2x upsample then conv" through the phase-collapsed weights (kind 0: Upsample, w [Co,Ci,3,3];
- * kind 1: v1.0 TimeUpsampleResCausal2x, w [C,C,3,3,3], alpha = sigmoid(mix_factor)); gamma/beta/out2 optional: the
- * following LayerNorm(+SiLU) fused into the phase convolutions. */
+ * kind 1: v1.0 TimeUpsampleResCausal2x, w [C,C,3,3,3], alpha = sigmoid(mix_factor); kind 2: the non-causal
+ * TimeUpsampleRes2x, the same with the 3x3x3 conv zero-padded by one frame on both sides, model_3dnoncausal.py:105-115);
+ * gamma/beta/out2 optional: the following LayerNorm(+SiLU) fused into the phase convolutions. */
 int32_t vt_op_upsample_conv(int32_t precision, int32_t kind, const void* x, const float* w, const float* bias, float alpha,
                             const float* gamma, const float* beta, int32_t ln_silu, void* out, void* out2, int32_t B,
                             int32_t T, int32_t H, int32_t W, int32_t Ci, int32_t Co, void* stream);

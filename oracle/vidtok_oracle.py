@@ -501,14 +501,15 @@ def kl_regularize(h: Tensor, noise: Optional[Tensor], sample: bool = True):
     return z, {"kl_loss": torch.sum(kl) / kl.shape[0]}
 
 
-def fsq_constants(levels, dtype=torch.float32):
-    """regularizers.py:111-115,153-158: levels, basis=cumprod([1]+levels[:-1]), half_l, offset, shift."""
+def fsq_constants(levels, dtype=torch.float32, device="cpu"):
+    """regularizers.py:111-115,153-158: levels, basis=cumprod([1]+levels[:-1]), half_l, offset, shift (computed on the
+    CPU, then placed on `device`)."""
     lv = torch.tensor(levels, dtype=torch.int32)
     basis = torch.cumprod(torch.tensor([1] + list(levels[:-1])), dim=0, dtype=torch.int32)
     half_l = (lv - 1) * (1 + 1e-3) / 2
     offset = torch.where(lv % 2 == 0, 0.5, 0.0)
     shift = (offset / half_l).atanh()
-    return lv, basis, half_l.to(dtype), offset.to(dtype), shift.to(dtype)
+    return tuple(t.to(device) for t in (lv, basis, half_l.to(dtype), offset.to(dtype), shift.to(dtype)))
 
 
 def fsq_regularize(h: Tensor, levels):
@@ -517,7 +518,7 @@ def fsq_regularize(h: Tensor, levels):
     :225-227, cast back to the input dtype :249) and int32 indices [B,T,H,W].
     aux_loss (the 32768-way entropy branch, :232-245) is NOT restated: no inference consumer reads it
     (SURVEY.md section 0.7); reported as 0."""
-    lv, basis, half_l, offset, shift = fsq_constants(levels)
+    lv, basis, half_l, offset, shift = fsq_constants(levels, device=h.device)
     z = h.permute(0, 2, 3, 4, 1).float()  # b t h w d
     bounded = torch.tanh(z + shift) * half_l - offset  # bound(): :153-158
     q = bounded.round()  # round_ste: :35-38 (half-to-even)
@@ -525,13 +526,13 @@ def fsq_regularize(h: Tensor, levels):
     codes = q / half_w  # quantize(): :160-164
     idx = ((codes * half_w + half_w) * basis).sum(dim=-1).to(torch.int32)  # :166-178
     codes = codes.to(h.dtype).permute(0, 4, 1, 2, 3)
-    return codes, {"indices": idx, "aux_loss": torch.zeros((), dtype=h.dtype), "pre_round": bounded}
+    return codes, {"indices": idx, "aux_loss": torch.zeros((), dtype=h.dtype, device=h.device), "pre_round": bounded}
 
 
 def fsq_indices_to_codes(idx: Tensor, levels, dtype=torch.float32) -> Tensor:
     """indices_to_codes + AutoencodingEngine.indices_to_latent: regularizers.py:180-198,
     autoencoder.py:205-213.  idx [B,T,H,W] int -> codes [B,d,T,H,W]."""
-    lv, basis, *_ = fsq_constants(levels)
+    lv, basis, *_ = fsq_constants(levels, device=idx.device)
     d = (idx.unsqueeze(-1) // basis) % lv
     half_w = lv // 2
     codes = (d - half_w) / half_w

@@ -20,7 +20,7 @@ def test_library_exports_every_declared_symbol():
     for name in sorted(declared):
         assert hasattr(lib, name), f"{name} declared in include/vidtok_b200.h but not exported"
     assert declared == set(N.EXPORTS), declared ^ set(N.EXPORTS)
-    assert N.lib().vt_abi_version() == 2
+    assert N.lib().vt_abi_version() == 3
 
 
 @pytest.mark.parametrize("case", golden_cases())

@@ -490,10 +490,11 @@ def test_fused_temporal_resblock_many_frames_per_cta():
 # regularizers as the epilogue of the bottleneck convolution (encoder conv_out)
 # ---------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("precision", PRECS, ids=PIDS)
-@pytest.mark.parametrize("zc", [4, 16])
+@pytest.mark.parametrize("zc", [4, 8, 16])
 def test_conv_out_kl_epilogue(precision, zc):
     """conv_out 512 -> 2z (k333) + DiagonalGaussianRegularizer in one launch: z = mean + exp(.5*clamp(logvar))*noise and
-    kl_loss = .5 * sum(mean^2 + var - 1 - logvar) / B (distributions.py:8-28, regularizers.py:82-92)."""
+    kl_loss = .5 * sum(mean^2 + var - 1 - logvar) / B (distributions.py:8-28, regularizers.py:82-92).  Every shipped z:
+    4 and 16 channels, and 8 (the 8chn configurations), which the epilogue compiles as a separate instantiation."""
     from gpu_util import _p, cl, conv_desc, stream, to_act
     from oracle.vidtok_oracle import kl_regularize
     B, Ci, T, H, W = 2, 512, 3, 16, 16
@@ -523,25 +524,28 @@ def test_conv_out_kl_epilogue(precision, zc):
 
 
 @pytest.mark.parametrize("precision", PRECS, ids=PIDS)
-def test_conv_out_fsq_epilogue(precision):
-    """conv_out 512 -> 5 + FSQ bound / round / index (regularizers.py:153-178) in one launch"""
+@pytest.mark.parametrize("levels", [(8,) * 4, (8,) * 5, (8,) * 6], ids=["4096", "32768", "262144"])
+def test_conv_out_fsq_epilogue(precision, levels):
+    """conv_out 512 -> len(levels) + FSQ bound / round / index (regularizers.py:153-178) in one launch, for every shipped
+    codebook: 4, 5 and 6 levels of 8 (4096, 32768 and 262144 codes)"""
     from gpu_util import _p, cl, conv_desc, stream, to_act
     from oracle.vidtok_oracle import fsq_regularize
     B, Ci, T, H, W = 2, 512, 3, 16, 16
-    levels = (8, 8, 8, 8, 8)
+    d_ = len(levels)
     x = prep(rnd(B, Ci, T, H, W, seed=1), precision)
-    w = prep(rnd(5, Ci, 3, 3, 3, seed=2, scale=1.5 / math.sqrt(27 * Ci)), precision)
-    b = rnd(5, seed=3)
+    w = prep(rnd(d_, Ci, 3, 3, 3, seed=2, scale=1.5 / math.sqrt(27 * Ci)), precision)
+    b = rnd(d_, seed=3)
     d, _ = conv_desc(x.shape, w.shape)
     xd, wd, bd = to_act(cl(x), precision), w.cuda(), b.cuda()
-    h = torch.empty((B, 5, T, H, W), device="cuda")
-    z = torch.empty((B, 5, T, H, W), device="cuda")
+    h = torch.empty((B, d_, T, H, W), device="cuda")
+    z = torch.empty((B, d_, T, H, W), device="cuda")
     idx = torch.empty((B, T, H, W), dtype=torch.int32, device="cuda")
-    lv = (C.c_int32 * 5)(*levels)
-    N.check(N.lib().vt_op_conv_regularize(precision, C.byref(d), _p(xd), _p(wd), _p(bd), 2, 5, lv, None, _p(h), _p(z), _p(idx), None, stream()))
+    lv = (C.c_int32 * d_)(*levels)
+    N.check(N.lib().vt_op_conv_regularize(precision, C.byref(d), _p(xd), _p(wd), _p(bd), 2, d_, lv, None, _p(h), _p(z), _p(idx), None, stream()))
     torch.cuda.synchronize()
     codes_ref, log = fsq_regularize(h.cpu(), levels)      # bit-exact given the kernel's own h
     assert torch.equal(idx.cpu(), log["indices"]) and torch.equal(z.cpu(), codes_ref)
+    assert int(idx.max()) >= 8 ** (d_ - 1)                # the last level's digit is in play
     if precision == N.PREC_EXACT_TC:                       # and against the fp64 conv: codes equal outside the tie band
         _, log64 = fsq_regularize(conv3d_ref(x, w, b).float(), levels)
         bad = idx.cpu() != log64["indices"]

@@ -15,6 +15,9 @@ of kl488, fsq488, v11long (tiled, chunk 16) and kl41616 launch at B = 1, and tes
     exact: 4e-5 (1 + |ref|)), and over the whole tensor against fp32 torch with TF32 off, with 2e-5 (1 + |ref|) more for
     the fp32 reference's own rounding.
 
+The same cases run the plans of the rest of the shipped configurations (test_gpu_zoo.py): keys of the non-causal family
+carry their time padding (" pad<front>.<back>", " pool<off>"), and the regularizer heads take every shipped z / codebook.
+
 test_bench_forward_keys_are_in_table re-derives the keys from the model forwards and lists any that the table misses.
 """
 import ctypes as C
@@ -151,8 +154,10 @@ def ln_params(rng, C_):
 # ---------------------------------------------------------------------------------------------------------------
 KEY_RE = re.compile(r"(?P<kern>conv_tc3?) k(?P<kt>\d)(?P<kh>\d)(?P<kw>\d) s(?P<st>\d)(?P<sh>\d) (?P<ci>\d+)->(?P<co>\d+) "
                     r"@(?P<T>\d+)x(?P<H>\d+)x(?P<W>\d+) tile\S+ bn\d+( halo)? ln(?P<ln>\d) r(?P<r>\d)(?P<m>m?) p\d+ "
-                    r"t(?P<t>\d) st\d+$")
-STEM_RE = re.compile(r"(?P<kern>conv_stem3?) k333 (?P<ci>\d+)->(?P<co>\d+) @(?P<T>\d+)x(?P<H>\d+)x(?P<W>\d+)$")
+                    r"t(?P<t>\d) st\d+( pad(?P<pf>\d+)\.(?P<pb>\d+))?( pool(?P<pool>\d+))?$")
+STEM_RE = re.compile(r"(?P<kern>conv_stem3?) k333 (?P<ci>\d+)->(?P<co>\d+) @(?P<T>\d+)x(?P<H>\d+)x(?P<W>\d+)"
+                     r"( pad(?P<pf>\d+)\.(?P<pb>\d+))?$")
+REG_CO = (4, 5, 6, 8, 16, 32)       # encoder conv_out: FSQ with 4 / 5 / 6 levels, KL with z = 4 / 8 / 16 (Co = 2 z)
 TBLOCK_RE = re.compile(r"tblock_tc strip \S+ T(?P<T>\d+) ln_out(?P<ln>\d)$")
 
 
@@ -172,14 +177,15 @@ def entry_of(p):
         return "tblock"
     if p["kind"].startswith("conv_stem"):
         return "stem"
-    if (p["ci"], p["co"]) in ((512, 1024), (1024, 512)) and p["kt"] * p["kh"] * p["kw"] == 1 and p["T"] == 1:
-        return "attention"                     # S = Q K^T (C -> tokens) and O = P V (tokens -> C) of a 32 x 32 frame
+    tokens = p["H"] * p["W"]
+    if (p["ci"], p["co"]) in ((512, tokens), (tokens, 512)) and p["kt"] * p["kh"] * p["kw"] == 1 and p["T"] == 1:
+        return "attention"                     # S = Q K^T (C -> tokens) and O = P V (tokens -> C) of a 32 x 32 / 16 x 16 frame
     if (p["kt"], p["kh"], p["kw"]) == (1, 2, 2):
         return "upsample"                      # one of the four phase convolutions of Upsample
     if (p["kt"], p["kh"], p["kw"]) == (2, 3, 3):
         return "time_upsample"                 # one of the two phase convolutions of TimeUpsampleResCausal2x (v1.0)
-    if p["co"] in (5, 8, 32):
-        return "regularize"                    # encoder conv_out + FSQ (5) / KL (2 z = 8, 32) in the epilogue
+    if p["co"] in REG_CO:
+        return "regularize"                    # encoder conv_out + FSQ (4, 5, 6) / KL (2 z = 8, 16, 32) in the epilogue
     if p["co"] == 3:
         return "head"                          # decoder conv_out, fp32 [B,C,T,H,W] output
     if p["kind"] == "conv_tc" and (p["kt"], p["ci"], p["co"]) == (1, 128, 128) and p["kh"] == 1:
@@ -202,12 +208,21 @@ def _stream():
     return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
-def _desc(B, Ci, Co, k, stride, Ti, Hi, Wi, pads, res_mode=0, alpha=0.0):
+def time_pads(p):
+    """(front, back) zero frames of the key's conv: the causal (kt-1)+(1-st) in front unless the key names its padding"""
+    if p.get("pf") is not None:
+        return p["pf"], p["pb"]
+    if p["kind"].startswith("conv_stem"):
+        return 2, 0
+    return (p["kt"] - 1) + (1 - p["st"]), 0
+
+
+def _desc(B, Ci, Co, k, stride, Ti, Hi, Wi, pads, res_mode=0, alpha=0.0, pt=None):
     d = N.ConvDesc()
     d.B, d.Ti, d.Hi, d.Wi, d.Ci, d.Co = B, Ti, Hi, Wi, Ci, Co
     d.kt, d.kh, d.kw = k
     d.st, d.sh, d.sw = stride
-    d.pt = (k[0] - 1) + (1 - stride[0])
+    d.pt = (k[0] - 1) + (1 - stride[0]) if pt is None else pt
     d.ph0, d.ph1, d.pw0, d.pw1 = pads
     d.ut = d.uh = d.uw = 1
     d.res_mode, d.alpha = res_mode, alpha
@@ -226,20 +241,24 @@ def _front(x, t_mode, pt, rng, prec):
 
 def case_conv(p, prec, B, rng, weight_scale=1.0):
     """vt_op_conv_ex: plain / residual (r1m: + x through the MMA; r1: alpha-mix of v1.1 TimeUpsample) / time-downsample
-    avg-pool mix (r3), fused LayerNorm+SiLU (ln1 / ln2), v1.1 replicate / cache time padding, stride-2 Downsample"""
+    avg-pool mix (r3, window shifted by one frame with pool1), fused LayerNorm+SiLU (ln1 / ln2), v1.1 replicate / cache
+    time padding, the non-causal family's zero padding behind the end (pad<front>.<back>), stride-2 Downsample"""
     kt, kh, kw, st, sh = p["kt"], p["kh"], p["kw"], p["st"], p["sh"]
     Ci, Co, To, Ho, Wo = p["ci"], p["co"], p["T"], p["H"], p["W"]
     head = entry_of(p) == "head"
-    to_off = 3 if head and p["t"] == 0 else 0                    # v1.0 decoder conv_out drops its first tdf-1 = 3 frames
-    Ti, Hi, Wi = To * st + to_off, Ho * sh, Wo * sh
+    # v1.0 causal decoder conv_out drops its first tdf-1 = 3 frames (the non-causal family drops none)
+    to_off = 3 if head and p["t"] == 0 and p.get("pf") is None else 0
+    pt, pt_back = time_pads(p)
+    pool_off = p.get("pool") or 0
+    Ti, Hi, Wi = (To - 1 + to_off) * st + kt - pt - pt_back, Ho * sh, Wo * sh
     pads = (0, 1, 0, 1) if sh == 2 else ((kh - 1) // 2, kh // 2, (kw - 1) // 2, kw // 2)
-    pt = (kt - 1) + (1 - st)
     K = Ci * kt * kh * kw
     x = prep(rng(B, Ci, Ti, Hi, Wi), prec)
     w = prep(rng(Co, Ci, kt, kh, kw, scale=weight_scale / math.sqrt(K)), prec)
     b = rng(Co)
     front, cache = _front(x, p["t"], pt, rng, prec)
-    xp = F.pad(torch.cat([front, x], dim=2), (pads[2], pads[3], pads[0], pads[1], 0, 0))
+    back = x.new_zeros(B, Ci, pt_back, Hi, Wi)
+    xp = F.pad(torch.cat([front, x, back], dim=2), (pads[2], pads[3], pads[0], pads[1], 0, 0))
     res, mix, res_mode, res_t_mode = None, False, p["r"], 0
     if res_mode == 1:
         res = prep(rng(B, Co, To, Ho, Wo), prec)
@@ -261,14 +280,18 @@ def case_conv(p, prec, B, rng, weight_scale=1.0):
             r = res.to(dtype) if frames is None else res[:, :, frames].to(dtype)
             y = ALPHA * r + (1 - ALPHA) * y if mix else r + y
         elif res_mode == 3:
-            pool_in = torch.cat([front if p["t"] else torch.zeros_like(x[:, :, :1]), x], dim=2).to(dtype)
+            if pool_off:                      # frames 2t .. 2t+2, one zero frame behind the end
+                pool_in = torch.cat([x, torch.zeros_like(x[:, :, :1])], dim=2).to(dtype)
+            else:
+                pool_in = torch.cat([front if p["t"] else torch.zeros_like(x[:, :, :1]), x], dim=2).to(dtype)
             pool = F.avg_pool3d(pool_in, (3, 1, 1), stride=(2, 1, 1))
             y = ALPHA * (pool if frames is None else pool[:, :, frames]) + (1 - ALPHA) * y
         return y
 
     e = N.ConvEx()
-    e.d = _desc(B, Ci, Co, (kt, kh, kw), (st, sh, sh), Ti, Hi, Wi, pads, res_mode, ALPHA if (mix or res_mode == 3) else 0.0)
+    e.d = _desc(B, Ci, Co, (kt, kh, kw), (st, sh, sh), Ti, Hi, Wi, pads, res_mode, ALPHA if (mix or res_mode == 3) else 0.0, pt)
     e.force_simt, e.t_mode, e.ln_mode, e.ln_silu, e.to_off = 0, p["t"], p["ln"], 1, to_off
+    e.pt_back, e.res_pool_off = pt_back, pool_off
     e.out_f32_ncdhw, e.res_mix, e.res_t_mode = int(head), int(mix), res_t_mode
     e.cacheT = 0 if cache is None else cache.shape[2]
     xd, cd = act(x, prec), (act(cache, prec) if cache is not None else None)
@@ -289,33 +312,37 @@ def case_conv(p, prec, B, rng, weight_scale=1.0):
 
 
 def case_regularize(p, prec, B, rng):
-    """vt_op_conv_regularize_ex: encoder conv_out with KL (Co = 2 z) or FSQ (Co = 5) in the epilogue; the head h against the
-    conv reference, z / indices / kl_loss against the oracle's regularizer on the kernel's own h"""
+    """vt_op_conv_regularize_ex: encoder conv_out with KL (Co = 2 z, z = 4, 8, 16) or FSQ (Co = 4, 5, 6 levels of 8) in the
+    epilogue; the head h against the conv reference, z / indices / kl_loss against the oracle's regularizer on the
+    kernel's own h"""
     from oracle.vidtok_oracle import fsq_regularize, kl_regularize
     Ci, Co, To, H, W = p["ci"], p["co"], p["T"], p["H"], p["W"]
-    x = prep(rng(B, Ci, To, H, W), prec)
+    pt, pt_back = time_pads(p)
+    Ti = To + 2 - pt - pt_back
+    x = prep(rng(B, Ci, Ti, H, W), prec)
     w = prep(rng(Co, Ci, 3, 3, 3, scale=1.5 / math.sqrt(27 * Ci)), prec)
     b = rng(Co)
-    front, cache = _front(x, p["t"], 2, rng, prec)
-    xp = F.pad(torch.cat([front, x], dim=2), (1, 1, 1, 1, 0, 0))
-    fsq = Co == 5
+    front, cache = _front(x, p["t"], pt, rng, prec)
+    xp = F.pad(torch.cat([front, x, x.new_zeros(B, Ci, pt_back, H, W)], dim=2), (1, 1, 1, 1, 0, 0))
+    fsq = Co in (4, 5, 6)
     zc = Co if fsq else Co // 2
+    levels = (8,) * Co if fsq else None
     e = N.ConvEx()
-    e.d = _desc(B, Ci, Co, (3, 3, 3), (1, 1, 1), To, H, W, (1, 1, 1, 1))
-    e.t_mode, e.cacheT = p["t"], 0 if cache is None else 2
+    e.d = _desc(B, Ci, Co, (3, 3, 3), (1, 1, 1), Ti, H, W, (1, 1, 1, 1), pt=pt)
+    e.t_mode, e.cacheT, e.pt_back = p["t"], 0 if cache is None else pt, pt_back
     h = torch.empty((B, Co, To, H, W), device="cuda")
     z = torch.empty((B, zc, To, H, W), device="cuda")
     idx = torch.empty((B, To, H, W), dtype=torch.int32, device="cuda") if fsq else None
     kl = torch.zeros((), device="cuda")
     noise = None if fsq else rng(B, zc, To, H, W)
-    levels = (C.c_int32 * 5)(8, 8, 8, 8, 8) if fsq else None
+    lv = (C.c_int32 * Co)(*levels) if fsq else None
     xd, cd = act(x, prec), (act(cache, prec) if cache is not None else None)
     from gpu_util import plan_keys
     _, keys = plan_keys(lambda: N.check(N.lib().vt_op_conv_regularize_ex(prec, C.byref(e), _p(xd), _p(cd), _p(w), _p(b), 2 if fsq else 1, zc,
-                                                                       levels, _p(noise), _p(h), _p(z), _p(idx), _p(None if fsq else kl),
+                                                                       lv, _p(noise), _p(h), _p(z), _p(idx), _p(None if fsq else kl),
                                                                        _stream())))
     if fsq:
-        codes, log = fsq_regularize(h.cpu(), (8, 8, 8, 8, 8))
+        codes, log = fsq_regularize(h.cpu(), levels)
         assert torch.equal(idx.cpu(), log["indices"]) and torch.equal(z.cpu(), codes)
     else:
         z_ref, log = kl_regularize(h.cpu(), noise.cpu(), True)
@@ -344,27 +371,34 @@ def case_head_planes(p, prec, B, rng):
 
 
 def case_stem(p, prec, B, rng):
-    """vt_op_conv_stem: encoder conv_in 3 -> 128 from the caller's fp32 [B,3,T,H,W]; t_rep replicated leading frames
-    (the v1.0 clip of 17 frames and the first v1.1 chunk of 1 frame get 3)"""
+    """vt_op_conv_stem (vt_op_conv_stem_ex for pad1.1): encoder conv_in 3 -> 128 from the caller's fp32 [B,3,T,H,W]; t_rep replicated leading frames
+    (the v1.0 clip of 17 frames and the first v1.1 chunk of 1 frame get 3), or one zero frame at each end (pad1.1: the
+    non-causal family)"""
     To, H, W, Ci, Co = p["T"], p["H"], p["W"], p["ci"], p["co"]
-    t_rep = 3 if To in (20, 4) else 0
+    pt, pt_back = time_pads(p)
+    t_rep = 3 if To in (20, 4) and pt == 2 else 0
     T = To - t_rep
     x = prep(rng(B, Ci, T, H, W), prec)
     w = prep(rng(Co, Ci, 3, 3, 3, scale=1 / math.sqrt(27 * Ci)), prec)
     b = rng(Co)
     xr = torch.cat([x[:, :, :1].repeat(1, 1, t_rep, 1, 1), x], dim=2)
-    xp = F.pad(xr, (1, 1, 1, 1, 2, 0))
+    xp = F.pad(xr, (1, 1, 1, 1, pt, pt_back))
     out = empty((B, To, H, W, Co), prec)
     from gpu_util import plan_keys
-    _, keys = plan_keys(lambda: N.check(N.lib().vt_op_conv_stem(prec, _p(x), _p(w), _p(b), _p(out), B, Ci, T, H, W, Co, t_rep, _stream())))
+    if pt == 2:
+        run = lambda: N.lib().vt_op_conv_stem(prec, _p(x), _p(w), _p(b), _p(out), B, Ci, T, H, W, Co, t_rep, _stream())  # noqa: E731
+    else:
+        run = lambda: N.lib().vt_op_conv_stem_ex(prec, _p(x), _p(w), _p(b), _p(out), B, Ci, T, H, W, Co, t_rep, pt, _stream())  # noqa: E731
+    _, keys = plan_keys(lambda: N.check(run()))
     return keys, [("stem", unact(out, prec), lambda dt, fr: conv_frames(xp, w, b, (1, 1, 1), fr, dt), 1.0)], To, 3
 
 
 def case_upsample(p, prec, B, rng):
     """vt_op_upsample_conv: kind 0 = Upsample (nearest 2x in H, W, then 3x3: four 1x2x2 phase convs on the low-resolution
-    input), kind 1 = TimeUpsampleResCausal2x v1.0 (nearest 2x in T, alpha-mix with a causal 3x3x3: two 2x3x3 phase convs).
-    Collapsed bf16 weights are sums of up to 4 taps rounded once: slack 2 (2.5 after the LayerNorm)"""
-    kind = 0 if p["kt"] == 1 else 1
+    input), kind 1 = TimeUpsampleResCausal2x v1.0 (nearest 2x in T, alpha-mix with a causal 3x3x3: two 2x3x3 phase convs),
+    kind 2 = the non-causal TimeUpsampleRes2x (the 3x3x3 zero-padded by one frame at each end; its odd phase is the key
+    with pad0.1).  Collapsed bf16 weights are sums of up to 4 taps rounded once: slack 2 (2.5 after the LayerNorm)"""
+    kind = 0 if p["kt"] == 1 else (2 if p.get("pf") is not None else 1)
     C_, T, H, W = p["ci"], p["T"], p["H"], p["W"]
     x = prep(rng(B, C_, T, H, W), prec)
     b = rng(C_)
@@ -383,7 +417,7 @@ def case_upsample(p, prec, B, rng):
         w = rng(C_, C_, 3, 3, 3, scale=1 / math.sqrt(27 * C_))
         To, Ho, Wo = 2 * T, H, W
         xu = x.repeat_interleave(2, dim=2)
-        xp = F.pad(xu, (1, 1, 1, 1, 2, 0))
+        xp = F.pad(xu, (1, 1, 1, 1, 2, 0) if kind == 1 else (1, 1, 1, 1, 1, 1))
 
         def v_ref(dt, fr):
             u = xu.to(dt) if fr is None else xu[:, :, fr].to(dt)
@@ -402,9 +436,10 @@ def case_upsample(p, prec, B, rng):
     return keys, outs, To, 3 if kind else 1
 
 
-def case_attention(p, prec, frames, rng, H=32, W=32, C_=512):
+def case_attention(p, prec, frames, rng, C_=512):
     """vt_op_attention_hw on frames of H x W tokens: S = Q K^T / sqrt(C) and O = P V on wgmma (per-frame K / V^T as the B
     operand), softmax in between; BF16 rounds P to bf16 (2^-8 relative on probabilities that sum to 1)"""
+    H, W = p["H"], p["W"]
     tokens = H * W
     q, k, v = (prep(rng(frames, C_, 1, H, W), prec) for _ in range(3))
     qd, kd, vd = (act(t, prec) for t in (q, k, v))

@@ -36,7 +36,8 @@ class ConvDesc(C.Structure):
 
 class ConvEx(C.Structure):
     _fields_ = [("d", ConvDesc)] + [(n, C.c_int32) for n in (
-        "force_simt", "t_mode", "cacheT", "ln_mode", "ln_silu", "to_off", "out_f32_ncdhw", "res_mix", "res_t_mode")]
+        "force_simt", "t_mode", "cacheT", "ln_mode", "ln_silu", "to_off", "out_f32_ncdhw", "res_mix", "res_t_mode", "pt_back",
+        "res_pool_off")]
 
 
 _P, _I32, _I64 = C.c_void_p, C.c_int32, C.c_int64
@@ -105,6 +106,7 @@ _SIGS = {
     "vt_op_conv_regularize": (_I32, [_I32, C.POINTER(ConvDesc), _P, _P, _P, _I32, _I32, C.POINTER(_I32), _P, _P, _P, _P, _P, _P]),
     "vt_op_conv_regularize_ex": (_I32, [_I32, C.POINTER(ConvEx), _P, _P, _P, _P, _I32, _I32, C.POINTER(_I32), _P, _P, _P, _P, _P, _P]),
     "vt_op_conv_stem": (_I32, [_I32, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P]),
+    "vt_op_conv_stem_ex": (_I32, [_I32, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P]),
     "vt_op_head_planes": (_I32, [_P, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P]),
     "vt_op_upsample_conv": (_I32, [_I32, _I32, _P, _P, _P, C.c_float, _P, _P, _I32, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P]),
     "vt_op_tblock": (_I32, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I32, _P, _P, _I32, _I32, _I32, _I32, _I32, _P]),

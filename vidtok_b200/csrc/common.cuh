@@ -190,4 +190,12 @@ struct ConvP {
   int relu;
 };
 
+// Zero frames behind the end of the time axis that the output extent To implies: the last output frame reads virtual
+// frame (To - 1 + to_off) * st + kt - 1 - pt, and any part of that past the input (t_rep + ut * Ti frames) is padding.
+// 0 for causal convolutions; 1 for the non-causal family's symmetric k3 padding and stride-2 time downsample.
+inline int time_pad_back(const ConvP& p) {
+  const int back = (p.To - 1 + p.to_off) * p.st + p.kt - p.pt - (p.t_rep + p.ut * p.Ti);
+  return back > 0 ? back : 0;
+}
+
 }  // namespace vt

@@ -364,7 +364,9 @@ cudaError_t launch_conv_stem(const ConvP& p, const float* x, const bf16* wpk, bf
   const int num_sms = device_sms(dev);
   const double M = (double)t.num_tiles * 128;
   char det[96] = "";
-  if (prof_enabled()) snprintf(det, sizeof(det), "k333 %d->%d @%dx%dx%d", p.Ci, p.Co, p.To, p.Hi, p.Wi);
+  // plan key: " pad<front>.<back>" only for the symmetric time padding of the non-causal family
+  if (prof_enabled()) snprintf(det, sizeof(det), p.pt != 2 ? "k333 %d->%d @%dx%dx%d pad%d.%d" : "k333 %d->%d @%dx%dx%d", p.Ci, p.Co, p.To,
+                               p.Hi, p.Wi, p.pt, time_pad_back(p));
   ProfScope _ps(p.split ? "conv_stem3" : "conv_stem", 2.0 * M * 27 * p.Ci * p.Co, (double)p.B * p.Ci * p.Ti * p.Hi * p.Wi * 4.0 + M * p.Co * 2.0 * pl, s, det);
   // as many resident CTAs per SM as fit: the phases of a tile (patch loads -> im2col -> MMA -> epilogue) are serialised
   // inside a CTA by block barriers, and a second resident CTA fills the bubbles

@@ -1145,10 +1145,18 @@ cudaError_t launch_conv_tc(const TcPlan& pl, const bf16* x, const bf16* w_nk, vo
   const unsigned grid = (unsigned)(t.num_tiles < num_sms ? t.num_tiles : num_sms);
   const double Mrows = (double)p.B * p.To * p.Ho * p.Wo;
   // plan key of the launch (profiler detail): geometry, tile, N tile, halo windows, fused LayerNorm, residual mode (m: through
-  // the MMA), kparts, time padding (t0 zeros / t1 replicate / t2 cache) and pipeline stages; " relu" only when ReLU is on, so
-  // the keys of every other plan stay as they were
-  char det[160] = "";
-  if (prof_enabled()) snprintf(det, sizeof(det), "k%d%d%d s%d%d %d->%d @%dx%dx%d tile%dx%dx%d bn%d%s ln%d r%d%s p%d t%d st%d%s", p.kt, p.kh, p.kw, p.st, p.sh, p.Ci, p.Co, p.To, p.Ho, p.Wo, t.BT, t.BH, t.BW, t.BN, t.halo ? " halo" : "", t.ln_mode, p.res_mode, t.res_mma ? "m" : "", split ? t.kparts : 1, p.t_mode, t.stages, p.relu ? " relu" : "");
+  // the MMA), kparts, time padding (t0 zeros / t1 replicate / t2 cache) and pipeline stages; " pad<front>.<back>" only when
+  // the time padding is not the causal one (the non-causal family), " pool<off>" only for a shifted avg-pool window of
+  // res_mode 3 and " relu" only when ReLU is on, so the keys of every other plan stay as they were
+  char det[192] = "";
+  if (prof_enabled()) {
+    char pad[48] = "";
+    const int pt_back = time_pad_back(p);
+    int n = 0;
+    if (p.pt != (p.kt - 1) + (1 - p.st) || pt_back != 0) n = snprintf(pad, sizeof(pad), " pad%d.%d", p.pt, pt_back);
+    if (p.res_mode == 3 && p.res_pool_off != 0) snprintf(pad + n, sizeof(pad) - n, " pool%d", p.res_pool_off);
+    snprintf(det, sizeof(det), "k%d%d%d s%d%d %d->%d @%dx%dx%d tile%dx%dx%d bn%d%s ln%d r%d%s p%d t%d st%d%s%s", p.kt, p.kh, p.kw, p.st, p.sh, p.Ci, p.Co, p.To, p.Ho, p.Wo, t.BT, t.BH, t.BW, t.BN, t.halo ? " halo" : "", t.ln_mode, p.res_mode, t.res_mma ? "m" : "", split ? t.kparts : 1, p.t_mode, t.stages, pad, p.relu ? " relu" : "");
+  }
   ProfScope _ps(split ? "conv_tc3" : "conv_tc", 2.0 * Mrows * p.kt * p.kh * p.kw * p.Ci * p.Co,
                 2.0 * cw * ((double)p.B * p.Ti * p.Hi * p.Wi * p.Ci) + Mrows * p.Co * (pl.tout == DT_F32 ? 4.0 : 2.0 * cw), s, det);
   auto launch = [&](auto kern) { kern<<<grid, kThreads, pl.smem, s>>>(maps, t); };

@@ -1415,7 +1415,7 @@ using namespace vt;
 extern "C" {
 
 const char* vt_last_error(void) { return g_err.c_str(); }
-int32_t vt_abi_version(void) { return 2; }
+int32_t vt_abi_version(void) { return 3; }
 int64_t vt_launch_count(int32_t reset) {
   const long long v = g_launches;
   if (reset) g_launches = 0;
@@ -1473,6 +1473,15 @@ int32_t vt_model_num_params(const vt_model* m) { return m ? m->params.size() : 0
 
 int32_t vt_model_param_info(const vt_model* m, int32_t i, char* name, int32_t cap, int64_t* shape5, int32_t* ndim) {
   return m ? m->params.info(i, name, cap, shape5, 5, ndim) : fail(VT_ERR_INVALID, "bad parameter index");
+}
+
+// Time taps of the 3x3x3 conv of the 2x time upsampling that each output parity reads, collapsed onto the 2 input frames of
+// its phase conv (launch_pack_w_collapsed).  Causal: even frames t'=2i read x'[2i-2..2i] = x[i-1],x[i-1],x[i]; odd frames
+// x[i-1],x[i],x[i].  Non-causal (pad 1 on both sides): even frames read x'[2i-1..2i+1] = x[i-1],x[i],x[i]; odd frames
+// x[i],x[i],x[i+1].
+static const int* tup_phase_map(bool noncausal, int parity) {
+  static const int lo[3] = {0, 1, 1}, hi[3] = {0, 0, 1};   // taps {0 | 1,2} / taps {0,1 | 2}
+  return (noncausal ? parity == 0 : parity != 0) ? lo : hi;
 }
 
 static int ensure_device(vt_model* m) {
@@ -1563,9 +1572,7 @@ int32_t vt_model_finalize(vt_model* m, void* stream) {
         ConvW& ph = lv.tup_ph[pt];
         ph.bias = c.bias; ph.w_nk = m->packed_nk + onk; ph.w_nk3 = m->packed_nk3 + 2 * onk; ph.wscale3 = c.wscale3;
         onk += align_up((size_t)ph.Co_pad * ph.Kpad, 512);
-        // even frames t'=2i read x'[2i-2..2i] = x[i-1],x[i-1],x[i]; odd frames read x[i-1],x[i],x[i]
-        // non-causal (pad 1 on both sides): even frames read x'[2i-1..2i+1] = x[i-1],x[i],x[i]; odd frames x[i],x[i],x[i+1]
-        const int* tmap = m->desc.noncausal ? (pt == 0 ? lo : hi) : (pt == 0 ? hi : lo);
+        const int* tmap = tup_phase_map(m->desc.noncausal != 0, pt);
         VT_CUDA(launch_pack_w_collapsed(w, ph.w_nk, c.Co, c.Co, c.Ci, 3, 3, 3, tmap, id3, id3, 2, 3, 3, s));
         VT_CUDA(launch_pack_w_collapsed(w, ph.w_nk3, c.Co, c.Co, c.Ci, 3, 3, 3, tmap, id3, id3, 2, 3, 3, s, c.wscale3));
       }
@@ -2266,7 +2273,8 @@ int vt::op_conv_impl(int precision, int force_simt, const vt_conv_desc* d, const
   p.pt = d->pt; p.ph = d->ph0; p.pw = d->pw0;
   p.to_off = e ? e->to_off : 0;
   p.Co = d->Co;
-  if (!conv_out_size(p, 0, d->ph1, d->pw1)) return fail(VT_ERR_INVALID, "conv: empty output");
+  if (e && (e->pt_back < 0 || e->res_pool_off < 0 || e->res_pool_off > 1)) return fail(VT_ERR_INVALID, "pt_back >= 0, res_pool_off 0 or 1");
+  if (!conv_out_size(p, e ? e->pt_back : 0, d->ph1, d->pw1)) return fail(VT_ERR_INVALID, "conv: empty output");
   const bool out_f32 = e && e->out_f32_ncdhw;
   // out_f32: external fp32 [B,Co,To,Ho,Wo] (the heads)
   set_out(p, out_f32 ? ncdhw_strides(p.Co, p.To, p.Ho, p.Wo) : cl_strides(p.To, p.Ho, p.Wo, p.Co, cw));
@@ -2289,7 +2297,7 @@ int vt::op_conv_impl(int precision, int force_simt, const vt_conv_desc* d, const
     set_res(p, cl_strides(d->Ti, p.Ho, p.Wo, p.Co, cw));
     p.resT = d->Ti;
     p.ra = d->alpha; p.rb = 1.f - d->alpha;
-    if (e) { p.res_t_mode = e->res_t_mode; p.res_cache = e->res_t_mode == 2 ? cache : nullptr; }
+    if (e) { p.res_t_mode = e->res_t_mode; p.res_cache = e->res_t_mode == 2 ? cache : nullptr; p.res_pool_off = e->res_pool_off; }
   } else {
     p.ra = 0.f; p.rb = 1.f;
   }
@@ -2362,6 +2370,7 @@ int32_t vt_op_conv_regularize_ex(int32_t precision, const vt_conv_ex* ex, const 
   e.d = *d;
   e.t_mode = ex->t_mode;
   e.cacheT = ex->cacheT;
+  e.pt_back = ex->pt_back;
   e.out_f32_ncdhw = 1;
   TcRegFusion rf;
   rf.mode = reg_mode; rf.zc = zc; rf.z = z; rf.noise = noise; rf.indices = indices; rf.sample = noise ? 1 : 0;
@@ -2396,14 +2405,16 @@ int32_t vt_op_conv_regularize(int32_t precision, const vt_conv_desc* d, const vo
   return vt_op_conv_regularize_ex(precision, &e, x, nullptr, w, bias, reg_mode, zc, fsq_levels, noise, h_out, z, indices, kl_loss, stream);
 }
 
-// Encoder stem (conv_in from the caller's fp32 [B,Ci,T,H,W] tensor) on the conv_stem kernel.
-int32_t vt_op_conv_stem(int32_t precision, const float* x, const float* w, const float* bias, void* out, int32_t B,
-                        int32_t Ci, int32_t T, int32_t H, int32_t W, int32_t Co, int32_t t_rep, void* stream) {
+// Encoder stem (conv_in from the caller's fp32 [B,Ci,T,H,W] tensor) on the conv_stem kernel; pt zero frames in front
+// (2: causal; 1: the non-causal family's symmetric padding).
+int32_t vt_op_conv_stem_ex(int32_t precision, const float* x, const float* w, const float* bias, void* out, int32_t B,
+                           int32_t Ci, int32_t T, int32_t H, int32_t W, int32_t Co, int32_t t_rep, int32_t pt, void* stream) {
   if (!x || !w || !out) return fail(VT_ERR_INVALID, "null argument");
   if (precision != VT_PREC_BF16 && precision != VT_PREC_EXACT_TC) return fail(VT_ERR_INVALID, "the stem kernel is a wgmma kernel (BF16 / EXACT_TC)");
   cudaStream_t s = (cudaStream_t)stream;
   const bool split = precision == VT_PREC_EXACT_TC;
   ConvP p = stem_p(B, Ci, T, H, W, Co, t_rep, split, bias);
+  p.pt = pt;
   if (!conv_stem_supported(p)) return fail(VT_ERR_INVALID, "stem kernel does not take this geometry");
   bf16* wpk = nullptr;
   float wsc = 0.f;
@@ -2419,6 +2430,10 @@ int32_t vt_op_conv_stem(int32_t precision, const float* x, const float* w, const
   cudaFree(wpk);
   if (er != cudaSuccess || e2 != cudaSuccess) return fail(VT_ERR_CUDA, "conv_stem: %s", cudaGetErrorString(er != cudaSuccess ? er : e2));
   return VT_OK;
+}
+int32_t vt_op_conv_stem(int32_t precision, const float* x, const float* w, const float* bias, void* out, int32_t B,
+                        int32_t Ci, int32_t T, int32_t H, int32_t W, int32_t Co, int32_t t_rep, void* stream) {
+  return vt_op_conv_stem_ex(precision, x, w, bias, out, B, Ci, T, H, W, Co, t_rep, 2, stream);
 }
 
 // Decoder head (conv_out Cin -> Co <= 4, 3x3x3, v1.0 zero padding, first to_off output frames dropped) as the BF16 path
@@ -2453,17 +2468,21 @@ int32_t vt_op_head_planes(const void* x, const float* w, const float* bias, floa
 // LayerNorm(+SiLU) of the result into out2.
 //   kind 0: Upsample (model_3dcausal.py:208-212): x [B,T,H,W,C] -> out [B,T,2H,2W,Co], w [Co,C,3,3]
 //   kind 1: TimeUpsampleResCausal2x, v1.0 (:267-273): out [B,2T,H,W,C] = alpha*x' + (1-alpha)*conv(x'), w [C,C,3,3,3]
+//   kind 2: TimeUpsampleRes2x of the non-causal family (model_3dnoncausal.py:105-115): kind 1 with the conv zero-padded by
+//           one frame on both sides; the executor of a non-causal model (its phase maps and time padding) runs it
 int32_t vt_op_upsample_conv(int32_t precision, int32_t kind, const void* x, const float* w, const float* bias, float alpha,
                             const float* gamma, const float* beta, int32_t ln_silu, void* out, void* out2, int32_t B,
                             int32_t T, int32_t H, int32_t W, int32_t Ci, int32_t Co, void* stream) {
   if (!x || !w || !bias || !out) return fail(VT_ERR_INVALID, "null argument");
   if (precision != VT_PREC_BF16 && precision != VT_PREC_EXACT_TC) return fail(VT_ERR_INVALID, "phase-collapsed convs exist in the tensor-core modes only");
-  if (Ci % 64 != 0 || Co % 32 != 0 || (kind == 1 && Ci != Co)) return fail(VT_ERR_INVALID, "unsupported channel counts");
+  if (kind < 0 || kind > 2) return fail(VT_ERR_INVALID, "kind must be 0, 1 or 2");
+  if (Ci % 64 != 0 || Co % 32 != 0 || (kind != 0 && Ci != Co)) return fail(VT_ERR_INVALID, "unsupported channel counts");
   cudaStream_t s = (cudaStream_t)stream;
   vt_model dummy;
   memset(&dummy.desc, 0, sizeof(dummy.desc));
   dummy.desc.norm_type = VT_NORM_LAYERNORM;
   dummy.desc.version = 0;
+  dummy.desc.noncausal = kind == 2 ? 1 : 0;
   const bool split = precision == VT_PREC_EXACT_TC;
   const int nph = kind == 0 ? 4 : 2, taps2 = kind == 0 ? 4 : 18;
   bf16* wp = nullptr;
@@ -2487,10 +2506,10 @@ int32_t vt_op_upsample_conv(int32_t precision, int32_t kind, const void* x, cons
     bf16* dst = wp + per * i * (split ? 2 : 1);
     if (split) ph.w_nk3 = dst; else ph.w_nk = dst;
     if (kind == 0) VT_CUDA(launch_pack_w_collapsed(w, dst, Co, Co, Ci, 1, 3, 3, id1, (i >> 1) == 0 ? lo : hi, (i & 1) == 0 ? lo : hi, 1, 2, 2, s, wsc));
-    else VT_CUDA(launch_pack_w_collapsed(w, dst, Co, Co, Ci, 3, 3, 3, i == 0 ? hi : lo, id3, id3, 2, 3, 3, s, wsc));
+    else VT_CUDA(launch_pack_w_collapsed(w, dst, Co, Co, Ci, 3, 3, 3, tup_phase_map(dummy.desc.noncausal != 0, i), id3, id3, 2, 3, 3, s, wsc));
   }
   lv.has_resample = kind == 0; lv.has_up_phase = kind == 0;
-  lv.has_tres = kind == 1; lv.has_tup_phase = kind == 1;
+  lv.has_tres = kind != 0; lv.has_tup_phase = kind != 0;
   lv.alpha = alpha;
   lv.tkey = "op";
   NormW nw;
