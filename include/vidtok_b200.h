@@ -179,6 +179,16 @@ int32_t vt_encode_chunk_fsq_aux(vt_chunk_state* s, int32_t is_first, const float
  * all decoded frames of this chunk (the caller trims the look-ahead tail as autoencoder_v1_1.py:327-328). */
 int32_t vt_decode_chunk(vt_chunk_state* s, int32_t is_first, const float* z_chunk, int32_t Cz, int32_t Tzc, float* x_out,
                         void* workspace, int64_t workspace_bytes, void* stream);
+/* Slot transplant: for every cache src holds, copies the readable cache of batch slot src_slots[i] of src into slot
+ * dst_slots[i] of dst (host arrays of n slots), in one launch on `stream`.  The caches are the whole state a chunk carries
+ * to the next (is_first is an argument of each chunk call, the overlap decoder's cache offsets depend on the cache key
+ * alone), so after the copy dst slot dst_slots[i] is the state the src slot would have had: the next non-first chunk
+ * computes in that slot what it would have computed in src's.  Caches dst does not hold yet are allocated for dst's batch
+ * (zeroed) and every cache filled is marked written.  Refused with VT_ERR_INVALID, before anything is enqueued: states of
+ * different models, precisions, H x W, direction or use_overlap, the same state as both ends, slots out of range, a dst
+ * slot listed twice, or a cache whose per-slot size differs between the two.  Calls on one dst state must use one stream. */
+int32_t vt_chunk_state_copy_slots(vt_chunk_state* dst, const vt_chunk_state* src, int32_t n, const int32_t* dst_slots,
+                                  const int32_t* src_slots, void* stream);
 
 /* ---- whole-video tiling below the ABI (tile_encode / tile_decode, autoencoder_v1_1.py:218-228,244-264,302-331): the chunk
  *      schedule, the causal caches and the chunk staging run inside the library -- one call per video, no host

@@ -67,6 +67,7 @@ _SIGS = {
     "vt_chunk_fsq_aux_workspace_bytes": (_I64, [_P, _I32]),
     "vt_encode_chunk_fsq_aux": (_I32, [_P, _I32, _P, _I32, _I32, _P, _P, C.c_float, _P, _P, _P, _I64, _P]),
     "vt_decode_chunk": (_I32, [_P, _I32, _P, _I32, _I32, _P, _P, _I64, _P]),
+    "vt_chunk_state_copy_slots": (_I32, [_P, _P, _I32, C.POINTER(_I32), C.POINTER(_I32), _P]),
     "vt_encode_video_workspace_bytes": (_I64, [_P, _I32, _I32, _I32, _I32, _I32, _I32]),
     "vt_encode_video": (_I32, [_P, _I32, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _I64, _P]),
     "vt_encode_video_fsq_aux_workspace_bytes": (_I64, [_P, _I32, _I32, _I32, _I32, _I32, _I32]),

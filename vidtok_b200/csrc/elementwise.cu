@@ -1179,6 +1179,34 @@ cudaError_t launch_copy_frames(DType t, const void* src, void* dst, int B, long 
   return cudaGetLastError();
 }
 
+// One segment per blockIdx.y (a cache key of one batch slot); the blocks along x stride over it with 16-byte loads and
+// stores when both ends are 16-byte aligned, and copy the remaining bytes (or a misaligned segment) one byte at a time.
+__global__ void __launch_bounds__(256) slot_copy_kernel(const SlotSeg* __restrict__ segs) {
+  const SlotSeg sg = segs[blockIdx.y];
+  const char* src = (const char*)sg.src;
+  char* dst = (char*)sg.dst;
+  const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
+  const unsigned long long t0 = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+  unsigned long long done = 0;
+  if ((((uintptr_t)src | (uintptr_t)dst) & 15) == 0) {
+    const unsigned long long n16 = sg.bytes / 16;
+    for (unsigned long long i = t0; i < n16; i += stride) ((uint4*)dst)[i] = __ldg((const uint4*)src + i);
+    done = n16 * 16;
+  }
+  for (unsigned long long i = done + t0; i < sg.bytes; i += stride) dst[i] = src[i];
+}
+cudaError_t launch_slot_copy(const SlotSeg* segs, int n, unsigned long long max_bytes, unsigned long long total_bytes,
+                             cudaStream_t s) {
+  if (n <= 0 || max_bytes == 0) return cudaSuccess;
+  ProfScope _ps("slot_copy", 0.0, 2.0 * (double)total_bytes, s);
+  // enough blocks along x for the largest segment at 4 vectors per thread, at most 256
+  const unsigned long long vec_blocks = (max_bytes / 16 + 1023) / 1024;
+  const unsigned gx = (unsigned)std::min<unsigned long long>(std::max<unsigned long long>(vec_blocks, 1), 256);
+  slot_copy_kernel<<<dim3(gx, (unsigned)n), 256, 0, s>>>(segs);
+  count_launch();
+  return cudaGetLastError();
+}
+
 cudaError_t launch_u8_frames_to_clip(const uint8_t* src, float* dst, int T, int Hs, int Ws, int C, int h0, int w0, int H, int W,
                                     cudaStream_t s) {
   const long long total = (long long)C * T * H * W;

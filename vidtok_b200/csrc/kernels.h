@@ -97,6 +97,15 @@ cudaError_t launch_ncdhw_to_cl(DType t, const float* x, void* y, int B, int C, i
                                cudaStream_t s);
 cudaError_t launch_copy_frames(DType t, const void* src, void* dst, int B, long long src_bs, long long dst_bs,
                                long long n_per_batch, cudaStream_t s);
+// byte copies of n segments in one launch (vt_chunk_state_copy_slots): segs is a DEVICE table; max_bytes is the largest
+// segment, total_bytes the sum (the profiler's byte count)
+struct SlotSeg {
+  const void* src;
+  void* dst;
+  unsigned long long bytes;
+};
+cudaError_t launch_slot_copy(const SlotSeg* segs, int n, unsigned long long max_bytes, unsigned long long total_bytes,
+                             cudaStream_t s);
 
 // video I/O adjacent steps: decoded uint8 frames [T,Hs,Ws,C] -> cropped normalised clip fp32 [C,T,H,W]; clip -> uint8 frames
 cudaError_t launch_u8_frames_to_clip(const uint8_t* src, float* dst, int T, int Hs, int Ws, int C, int h0, int w0, int H, int W,

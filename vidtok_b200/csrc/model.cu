@@ -318,6 +318,9 @@ struct vt_chunk_state {
   bool persist = true;           // false: one-shot "first chunk" context (untiled v1.1 forward)
   // (v1.0 streams: a persistent state; the first chunk has zero padding in front, later chunks read the caches)
   std::map<std::string, vt::CacheBuf> caches;
+  // device segment table of vt_chunk_state_copy_slots into this state (grown on demand; stream-ordered reuse)
+  void* seg_table = nullptr;
+  size_t seg_table_bytes = 0;
   ~vt_chunk_state() {
     for (auto& kv : caches)
       for (int i = 0; i < 2; ++i)
@@ -325,6 +328,7 @@ struct vt_chunk_state {
           if (m && persist) vt::pool_put(m, kv.second.bytes, kv.second.buf[i]);
           else cudaFree(kv.second.buf[i]);
         }
+    if (seg_table) cudaFree(seg_table);
   }
 };
 
@@ -1844,6 +1848,78 @@ int32_t vt_decode_chunk(vt_chunk_state* cs, int32_t is_first, const float* z_chu
   ex.ck = cs;
   run_decoder(ex, z_chunk, cs->B, Tzc, cs->H, cs->W, x_out);
   return ex.rc;
+}
+
+// Every cache keeps the batch outermost (NDHWC activations, [B,2,H,W,C] temporal-block caches, fp32 [B,C,2,H,W] stem /
+// conv_in caches, [B,n,H,W,C] time-upsampling caches), so slot b of a cache is the contiguous byte range
+// [b * bytes / B, (b + 1) * bytes / B) of its readable buffer.
+int32_t vt_chunk_state_copy_slots(vt_chunk_state* dst, const vt_chunk_state* src, int32_t n, const int32_t* dst_slots,
+                                  const int32_t* src_slots, void* stream) {
+  if (!dst || !src || n < 0 || (n > 0 && (!dst_slots || !src_slots))) return fail(VT_ERR_INVALID, "null argument");
+  if (dst == src) return fail(VT_ERR_INVALID, "copy_slots: source and destination are the same state");
+  if (dst->m != src->m) return fail(VT_ERR_INVALID, "copy_slots: the states belong to different models");
+  if (dst->prec != src->prec) return fail(VT_ERR_INVALID, "copy_slots: precision %d vs %d", dst->prec, src->prec);
+  if (dst->H != src->H || dst->W != src->W)
+    return fail(VT_ERR_INVALID, "copy_slots: geometry %dx%d vs %dx%d", dst->H, dst->W, src->H, src->W);
+  if (dst->is_decoder != src->is_decoder) return fail(VT_ERR_INVALID, "copy_slots: an encoder and a decoder state");
+  if (dst->use_overlap != src->use_overlap) return fail(VT_ERR_INVALID, "copy_slots: use_overlap differs");
+  std::vector<char> taken(dst->B, 0);
+  for (int i = 0; i < n; ++i) {
+    if (src_slots[i] < 0 || src_slots[i] >= src->B) return fail(VT_ERR_INVALID, "copy_slots: source slot %d of %d", src_slots[i], src->B);
+    if (dst_slots[i] < 0 || dst_slots[i] >= dst->B) return fail(VT_ERR_INVALID, "copy_slots: destination slot %d of %d", dst_slots[i], dst->B);
+    if (taken[dst_slots[i]]++) return fail(VT_ERR_INVALID, "copy_slots: destination slot %d listed twice", dst_slots[i]);
+  }
+  for (const auto& kv : src->caches) {
+    const vt::CacheBuf& c = kv.second;
+    auto it = dst->caches.find(kv.first);
+    if (c.bytes % src->B) return fail(VT_ERR_INVALID, "copy_slots: cache %s is not split by batch", kv.first.c_str());
+    if (it != dst->caches.end() && it->second.bytes && it->second.bytes / dst->B != c.bytes / src->B)
+      return fail(VT_ERR_INVALID, "copy_slots: cache %s holds %zu bytes per slot, the source %zu", kv.first.c_str(),
+                  it->second.bytes / dst->B, c.bytes / src->B);
+  }
+  if (n == 0) return VT_OK;
+  size_t nseg = 0;
+  for (const auto& kv : src->caches)
+    if (kv.second.valid && kv.second.buf[kv.second.cur]) nseg += (size_t)n;
+  if (nseg > 65535) return fail(VT_ERR_INVALID, "copy_slots: %zu segments (at most 65535)", nseg);
+  vt_model* m = dst->m;
+  VT_CUDA(cudaSetDevice(m->device));
+  cudaStream_t s = (cudaStream_t)stream;
+  std::vector<SlotSeg> segs;
+  unsigned long long max_bytes = 0, total = 0;
+  for (const auto& kv : src->caches) {
+    const vt::CacheBuf& c = kv.second;
+    if (!c.valid || !c.buf[c.cur]) continue;   // nothing written yet
+    const size_t per = c.bytes / src->B;
+    vt::CacheBuf& d = dst->caches[kv.first];
+    if (!d.buf[0]) {   // the destination does not hold this key yet: allocate it for dst->B slots, zeroed
+      d.bytes = per * dst->B;
+      d.cur = 0;
+      for (int i = 0; i < 2; ++i) {
+        d.buf[i] = vt::pool_take(m, d.bytes);
+        if (!d.buf[i]) VT_CUDA(cudaMalloc(&d.buf[i], d.bytes));
+        VT_CUDA(cudaMemsetAsync(d.buf[i], 0, d.bytes, s));
+      }
+    }
+    for (int i = 0; i < n; ++i) {
+      segs.push_back({(const char*)c.buf[c.cur] + (size_t)src_slots[i] * per, (char*)d.buf[d.cur] + (size_t)dst_slots[i] * per, per});
+      max_bytes = std::max<unsigned long long>(max_bytes, per);
+      total += per;
+    }
+    d.valid = true;
+  }
+  if (segs.empty()) return VT_OK;
+  const size_t tb = segs.size() * sizeof(SlotSeg);
+  if (dst->seg_table_bytes < tb) {
+    if (dst->seg_table) VT_CUDA(cudaFree(dst->seg_table));
+    dst->seg_table = nullptr;
+    dst->seg_table_bytes = 0;
+    VT_CUDA(cudaMalloc(&dst->seg_table, tb));
+    dst->seg_table_bytes = tb;
+  }
+  VT_CUDA(cudaMemcpyAsync(dst->seg_table, segs.data(), tb, cudaMemcpyHostToDevice, s));
+  VT_CUDA(launch_slot_copy((const SlotSeg*)dst->seg_table, (int)segs.size(), max_bytes, total, s));
+  return VT_OK;
 }
 
 // ---- whole-video temporal tiling in the library (autoencoder_v1_1.py:218-228,244-264,302-331) ------------------------------

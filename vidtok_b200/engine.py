@@ -263,6 +263,15 @@ class ChunkState:
         """workspace of vt_encode_chunk_fsq_aux for a chunk of Tc frames"""
         return self.native._workspace(int(self.native.lib.vt_chunk_fsq_aux_workspace_bytes(self.handle, Tc)))
 
+    def copy_slots(self, src: "ChunkState", dst_slots: Sequence[int], src_slots: Sequence[int]):
+        """vt_chunk_state_copy_slots: slot dst_slots[i] of this state becomes the state slot src_slots[i] of src would
+        have had (every cache copied, in one launch on the current stream)."""
+        n = len(dst_slots)
+        if len(src_slots) != n:
+            raise ValueError("dst_slots and src_slots must have the same length")
+        d, s = (C.c_int32 * max(n, 1))(*dst_slots), (C.c_int32 * max(n, 1))(*src_slots)
+        N.check(self.native.lib.vt_chunk_state_copy_slots(self.handle, src.handle, n, d, s, _stream_ptr(self.native.device)))
+
 
 # --------------------------------------------------------------------------------------------------
 # parameter trees with the reference's checkpoint keys

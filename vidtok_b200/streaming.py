@@ -53,6 +53,24 @@ far, with n_steps = global_step // 2 as `encode` uses:
 Streams use world size 1: ranks need not push in lockstep, so avg_prob is not all-reduced across ranks.  KL noise is one
 CPU `torch.randn` per push over the push's latent frames (with `t_chunk`: one per chunk, in chunk order, the draws
 tile_encode makes) unless `noise` is passed.  No push synchronises with the host.
+
+Pools (EncodePool / DecodePool) carry many videos that start and end independently through one chunk state of batch S
+(the capacity), one slot per video.  Every chunk of a video is a chunk of its own recipe stream (PoolSchedule):
+  - its first chunk runs on a side state of batch 1 and is then transplanted into its slot
+    (vt_chunk_state_copy_slots: every cache of the slot, in one launch);
+  - later chunks of exactly t_chunk frames (decoder: t_chunk latent frames, plus the look-ahead frame with use_overlap)
+    run as one batched chunk of all S slots per step();
+  - close() transplants the slot out to the side state and runs the rest there: v1.1's short last chunk, the decoder's
+    last chunk without look-ahead.
+A batched chunk advances the caches of every row, so a started video without a full chunk buffered sits the step out:
+its slot is copied to a parking state before the batched chunk and back after it (two transplants of that slot's caches
+per step it waits; none while every open video keeps up).  Empty slots run on zeros and their outputs are dropped.
+Each slot's outputs are therefore its own tile_encode / tile_decode (v1.1) or whole-clip encode / decode (v1.0): bit for
+bit in "bf16" and "fma"; in "exact" and "mixed" to fp32 rounding, since the split-operand kernels' tiles (and so their
+rounding) may depend on the batch.  Per-slot losses are formed from each video's own slice of the pre-bound latent
+(vt_encode_chunk_pre): kl_loss with vt_op_kl per chunk, FSQ aux_loss from vt_fsq_aux_partials / vt_fsq_aux_finalize per
+chunk, both over everything the video encoded so far, as the streams report them.  Non-causal models are refused; world
+size 1, as the streams.
 """
 from __future__ import annotations
 
@@ -385,3 +403,408 @@ class DecodeStream(_Stream):
             return self._empty(z.device)
         x = outs[0].contiguous() if len(outs) == 1 else torch.cat(outs, dim=2)
         return x.to(self.out_dtype)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Pools: many videos, each starting and ending on its own, through one batched chunk state
+# ---------------------------------------------------------------------------------------------------------------------
+def check_pool_recipe(version: int, tdf: int, t_chunk: Optional[int], use_overlap: bool, is_decoder: bool):
+    """The options a pool accepts (ValueError otherwise): every pool has a chunk length, t_chunk frames (encoder, a
+    multiple of tdf) or latent frames (decoder); v1.1 pools follow the stream recipe's rules."""
+    if t_chunk is None:
+        raise ValueError("a pool needs t_chunk: the batched chunks of all its slots have one length")
+    if version == 1:
+        check_recipe(version, tdf, t_chunk, use_overlap, is_decoder)
+        return
+    if use_overlap:
+        raise ValueError("use_overlap needs a v1.1 model and t_chunk (the look-ahead follows the tile_decode chunks)")
+    if int(t_chunk) < 1 or (not is_decoder and int(t_chunk) % tdf != 0):
+        raise ValueError(f"t_chunk must be a positive multiple of time_downsample_factor ({tdf}), got {t_chunk}"
+                         if not is_decoder else f"t_chunk must be a positive number of latent frames, got {t_chunk}")
+
+
+class PoolSchedule:
+    """The host-side plan of a pool, without device work: which slots hold a video, how many frames (encoder) or latent
+    frames (decoder) each has buffered, and where each chunk runs.  Chunks are (frames in, frames consumed, decoded frames
+    dropped at the tail) as recipe_decode_chunks; an encoder chunk is (n, n, 0).
+
+    A video's chunks are those of the recipe stream run alone: its first chunk (one frame, or one latent plus its look-ahead)
+    "joins" on a side state, later chunks of exactly t_chunk (+ look-ahead) run batched, and close() gives the rest -- the
+    short last chunk, or the decoder's last chunk without look-ahead -- which runs on the side state again.  For v1.1 these
+    are the chunks of build_chunk_start_end; for v1.0 they are valid stream chunks (1 frame, then multiples of tdf), which
+    give the whole clip's result."""
+
+    def __init__(self, capacity: int, version: int, tdf: int, t_chunk: int, is_decoder: bool, use_overlap: bool = False):
+        if int(capacity) < 1:
+            raise ValueError(f"capacity must be positive, got {capacity}")
+        self.S, self.version, self.tdf, self.t_chunk = int(capacity), int(version), int(tdf), int(t_chunk)
+        self.is_decoder, self.use_overlap = bool(is_decoder), bool(use_overlap)
+        self.busy = [False] * self.S     # the slot holds a video
+        self.avail = [0] * self.S        # frames buffered and not yet consumed
+        self.first = [True] * self.S     # the video's first chunk has not run
+
+    def _chunks(self, slot: int, final: bool) -> List[Tuple[int, int, int]]:
+        if self.is_decoder:
+            return recipe_decode_chunks(self.avail[slot], self.first[slot], self.t_chunk, self.use_overlap, self.tdf, final)
+        return [(n, n, 0) for n in recipe_encode_chunks(self.avail[slot], self.first[slot], self.t_chunk, final)]
+
+    def check(self, slot: int):
+        if not (0 <= slot < self.S) or not self.busy[slot]:
+            raise RuntimeError(f"slot {slot} holds no open video")
+
+    def open(self) -> int:
+        for s in range(self.S):
+            if not self.busy[s]:
+                self.busy[s], self.avail[s], self.first[s] = True, 0, True
+                return s
+        raise RuntimeError(f"all {self.S} slots hold a video: close one first")
+
+    def push(self, slot: int, n: int):
+        self.check(slot)
+        self.avail[slot] += int(n)
+
+    def started(self) -> List[int]:
+        """slots whose video has run its first chunk: their caches must survive every batched chunk"""
+        return [s for s in range(self.S) if self.busy[s] and not self.first[s]]
+
+    def plan_step(self) -> Tuple[List[Tuple[int, Tuple[int, int, int]]], List[int], Optional[Tuple[int, int, int]]]:
+        """(joins, ready, chunk): the first chunks to run on the side state, in slot order; the slots of the batched chunk
+        and its (frames in, consumed, dropped), the same for every ready slot (None when no slot is ready)."""
+        joins = []
+        for s in range(self.S):
+            if self.busy[s] and self.first[s]:
+                c = self._chunks(s, final=False)
+                if c:
+                    joins.append((s, c[0]))
+                    self.avail[s] -= c[0][1]
+                    self.first[s] = False
+        ready, chunk = [], None
+        for s in self.started():
+            c = self._chunks(s, final=False)
+            if c:
+                ready.append(s)
+                chunk = c[0]
+        for s in ready:
+            self.avail[s] -= chunk[1]
+        return joins, ready, chunk
+
+    def close(self, slot: int) -> Tuple[bool, List[Tuple[int, int, int]]]:
+        """(started, chunks): the chunks that finish the video (all buffered frames), and whether its first chunk ran
+        before (its caches are then in the slot).  Frees the slot."""
+        self.check(slot)
+        started, chunks = not self.first[slot], self._chunks(slot, final=True)
+        if not self.is_decoder and self.version == 0:
+            for i, (n, _, _) in enumerate(chunks):
+                if (started or i > 0) and n % self.tdf:
+                    raise ValueError(f"{n % self.tdf} frames do not complete a group of {self.tdf}: a v1.0 pool encodes "
+                                     f"videos of 1 + k * {self.tdf} frames")
+        self.busy[slot], self.avail[slot], self.first[slot] = False, 0, True
+        return started, chunks
+
+
+class _Pool:
+    def __init__(self, model, capacity: int, H: int, W: int, is_decoder: bool, t_chunk: Optional[int],
+                 use_overlap: bool = False):
+        if not model.is_causal:
+            raise ValueError("non-causal models cannot stream: their time padding is symmetric, so a frame depends on later frames")
+        self.tdf = int(model.spec.time_downsample_factor)
+        check_pool_recipe(model.spec.version, self.tdf, t_chunk, use_overlap, is_decoder)
+        self.sched = PoolSchedule(capacity, model.spec.version, self.tdf, int(t_chunk), is_decoder, use_overlap)
+        self.S, self.t_chunk, self.use_overlap = self.sched.S, int(t_chunk), bool(use_overlap)
+        rt = model._rt
+        self.model = model
+        self.native = rt.sync()
+        self.spec = model.spec
+        self.precision = rt.precision()
+        self.out_dtype = rt.out_dtype()
+        self.H, self.W = int(H), int(W)
+        self.main = ChunkState(self.native, self.precision, self.S, self.H, self.W, is_decoder, self.use_overlap)
+        self.side = ChunkState(self.native, self.precision, 1, self.H, self.W, is_decoder, self.use_overlap)
+        self.park: Optional[ChunkState] = None   # holds the caches of started slots that sit out a batched chunk
+        self.pending: List[Optional[torch.Tensor]] = [None] * self.S
+        # batched: batched chunks run; slot_chunks: video chunks they carried; side: chunks on the side state;
+        # transplants: slots copied between states
+        self.counts = {"batched": 0, "slot_chunks": 0, "side": 0, "transplants": 0}
+
+    def close_pool(self):
+        for st in (self.main, self.side, self.park):
+            if st is not None:
+                st.close()
+
+    def _copy(self, dst: ChunkState, src: ChunkState, dst_slots: List[int], src_slots: List[int]):
+        dst.copy_slots(src, dst_slots, src_slots)
+        self.counts["transplants"] += len(dst_slots)
+
+    def _open(self) -> int:
+        slot = self.sched.open()
+        self.pending[slot] = None
+        return slot
+
+    def _buffer(self, slot: int, t: torch.Tensor):
+        self.sched.push(slot, t.shape[2])
+        self.pending[slot] = t if self.pending[slot] is None else torch.cat([self.pending[slot], t], dim=2)
+
+    def _take(self, slot: int, chunk: Tuple[int, int, int]) -> torch.Tensor:
+        n, step, _ = chunk
+        p = self.pending[slot]
+        out = p[:, :, :n].contiguous()
+        self.pending[slot] = p[:, :, step:] if step < p.shape[2] else None
+        return out
+
+    def _batched(self, ready: List[int], chunk: Tuple[int, int, int], run):
+        """run(x_rows) over the main state, every other started slot parked (copied out before and back after, so its
+        caches are exactly as they were) and every other row fed zeros; x_rows: {slot: its chunk}"""
+        rows = {s: self._take(s, chunk) for s in ready}
+        waiting = [s for s in self.sched.started() if s not in rows]
+        if waiting:
+            if self.park is None:
+                self.park = ChunkState(self.native, self.precision, self.S, self.H, self.W, self.sched.is_decoder,
+                                       self.use_overlap)
+            self._copy(self.park, self.main, waiting, waiting)
+        out = run(rows)
+        if waiting:
+            self._copy(self.main, self.park, waiting, waiting)
+        self.counts["batched"] += 1
+        self.counts["slot_chunks"] += len(ready)
+        return out
+
+    @staticmethod
+    def _stack(rows: Dict[int, torch.Tensor], S: int) -> torch.Tensor:
+        any_row = next(iter(rows.values()))
+        x = torch.zeros((S,) + tuple(any_row.shape[1:]), dtype=any_row.dtype, device=any_row.device)
+        for s, r in rows.items():
+            x[s] = r[0]
+        return x
+
+
+class _SlotLosses:
+    """One video's running losses, as tile_encode (v1.1: mean over its chunks) or the whole clip (v1.0) forms them."""
+
+    def __init__(self, dev, aux: bool, J: int):
+        self.n_chunks = 0
+        self.kl_sum = torch.zeros((), dtype=torch.float32, device=dev)
+        self.aux_sum = torch.zeros((), dtype=torch.float32, device=dev)
+        self.aux_loss = torch.zeros((), dtype=torch.float32, device=dev)
+        if aux:
+            self.tok_stats = torch.zeros((2,), dtype=torch.float64, device=dev)
+            self.tok_avg = torch.zeros((J,), dtype=torch.float64, device=dev)
+            self.tokens = 0
+
+
+class EncodePool(_Pool):
+    """S slots of one encoder, one (H, W).  Each slot holds one video at a time; videos open, push frames and close
+    independently, and each video's outputs equal its own tile_encode (v1.1, t_chunk = t_chunk_enc) or its whole-clip
+    encode (v1.0) -- see the module docstring of the pools.
+
+        pool = EncodePool(model, capacity=S, H=H, W=W, t_chunk=16)
+        a = pool.open(); pool.push(a, frames)          # frames [1, C, t, H, W], any t
+        for slot, (z, reg_log) in pool.step().items(): ...
+        z, reg_log = pool.close(a)                      # the rest of the video, its short last chunk included
+
+    generator (open): the CPU generator of the video's KL noise (one torch.randn per chunk, in chunk order, as
+    tile_encode draws them); None draws from torch's default generator in the order the pool runs the chunks."""
+
+    def __init__(self, model, capacity: int, H: int, W: int, t_chunk: Optional[int] = None):
+        super().__init__(model, capacity, H, W, is_decoder=False, t_chunk=t_chunk)
+        self.Hz, self.Wz = self.native.latent_shape(1, H, W)[1:]
+        self.reg = model.regularization
+        self.aux = self.spec.regularizer == "fsq" and self.reg.aux_enabled()
+        self.losses: List[Optional[_SlotLosses]] = [None] * self.S
+        self.gens: List[Optional[torch.Generator]] = [None] * self.S
+
+    def open(self, generator: Optional[torch.Generator] = None) -> int:
+        slot = self._open()
+        J = self.reg.codebook_size if self.aux else 0
+        self.losses[slot] = _SlotLosses(self.native.device, self.aux, J)
+        self.gens[slot] = generator
+        return slot
+
+    def push(self, slot: int, frames: torch.Tensor):
+        """frames: [1, C, t, H, W] CUDA tensor, any t (buffered until they complete a chunk)."""
+        self.sched.check(slot)
+        if not frames.is_cuda:
+            raise RuntimeError("vidtok_b200: inputs must be CUDA tensors; there is no CPU path")
+        if frames.dim() != 5 or tuple(frames.shape[:2]) != (1, self.spec.in_channels) or tuple(frames.shape[3:]) != (self.H, self.W):
+            raise ValueError(f"expected [1,{self.spec.in_channels},t,{self.H},{self.W}] frames, got {tuple(frames.shape)}")
+        self._buffer(slot, frames.detach().to(torch.float32))
+
+    def step(self) -> Dict[int, Tuple[torch.Tensor, Dict[str, torch.Tensor]]]:
+        """Runs every first chunk that is buffered (side state, then transplanted into its slot) and one batched chunk of
+        every slot with t_chunk frames buffered.  Returns {slot: (z, reg_log)} for the slots that produced latents."""
+        joins, ready, chunk = self.sched.plan_step()
+        parts: Dict[int, List] = {}
+        for s, c in joins:
+            got = self._run(self.side, {0: self._take(s, c)}, {0: s}, first=True)
+            self.counts["side"] += 1
+            self._copy(self.main, self.side, [s], [0])
+            parts.setdefault(s, []).append(got[0])
+        if ready:
+            got = self._batched(ready, chunk, lambda rows: self._run(self.main, rows, {s: s for s in rows}, first=False))
+            for s in ready:
+                parts.setdefault(s, []).append(got[s])
+        return {s: self._result(s, p) for s, p in parts.items()}
+
+    def close(self, slot: int) -> Tuple[torch.Tensor, Dict[str, torch.Tensor]]:
+        """End of the slot's video: encodes the frames still buffered (v1.1: the last, shorter chunk) on the side state
+        and frees the slot.  Returns the latents of those chunks and the video's reg_log (its final losses)."""
+        started, chunks = self.sched.close(slot)
+        if started and chunks:
+            self._copy(self.side, self.main, [0], [slot])
+        parts = []
+        for i, c in enumerate(chunks):
+            parts.append(self._run(self.side, {0: self._take(slot, c)}, {0: slot}, first=not started and i == 0)[0])
+            self.counts["side"] += 1
+        self.pending[slot] = None
+        out = self._result(slot, parts)
+        self.losses[slot], self.gens[slot] = None, None
+        return out
+
+    def _result(self, slot: int, parts: List) -> Tuple[torch.Tensor, Dict[str, torch.Tensor]]:
+        s, dev = self.spec, self.native.device
+        if parts:
+            z = torch.cat([p[0] for p in parts], dim=2) if len(parts) > 1 else parts[0][0]
+        else:
+            z = torch.empty((1, s.z_channels, 0, self.Hz, self.Wz), dtype=torch.float32, device=dev)
+        L = self.losses[slot]
+        if s.regularizer == "fsq":
+            if parts:
+                idx = torch.cat([p[1] for p in parts], dim=1) if len(parts) > 1 else parts[0][1]
+            else:
+                idx = torch.empty((1, 0, self.Hz, self.Wz), dtype=torch.int32, device=dev)
+            log = {"indices": idx, "aux_loss": L.aux_loss}
+        elif s.version == 1:
+            log = {"kl_loss": EncodeStream._mean(L.kl_sum, L.n_chunks) if L.n_chunks else torch.zeros((), device=dev)}
+        else:
+            log = {"kl_loss": L.kl_sum}
+        return z.to(self.out_dtype), log
+
+    def _run(self, state: ChunkState, rows: Dict[int, torch.Tensor], slot_of: Dict[int, int], first: bool) -> Dict[int, Tuple]:
+        """One chunk of `state` over rows {batch row: frames [1,C,n,H,W]} (other rows zeros); per row (z, indices) and
+        the row's video's losses updated from its own slice of the pre-bound latent."""
+        s, lib, dev = self.spec, self.native.lib, self.native.device
+        B = self.S if state is self.main else 1
+        n = next(iter(rows.values())).shape[2]
+        tz = self.native.latent_shape(n, self.H, self.W)[0]
+        x = self._stack(rows, B)
+        noise = None
+        if s.regularizer == "kl" and s.kl_sample:
+            noise = torch.zeros((B, s.z_channels, tz, self.Hz, self.Wz), dtype=torch.float32)
+            for r in rows:   # CPU draws, one per video chunk (distributions.py:17), as tile_encode makes them
+                noise[r] = torch.randn((1, s.z_channels, tz, self.Hz, self.Wz), generator=self.gens[slot_of[r]])[0]
+            noise = noise.to(dev)
+        hC = (2 if s.double_z else 1) * s.z_channels
+        z = torch.empty((B, s.z_channels, tz, self.Hz, self.Wz), dtype=torch.float32, device=dev)
+        idx = torch.empty((B, tz, self.Hz, self.Wz), dtype=torch.int32, device=dev) if s.regularizer == "fsq" else None
+        kl_batch = torch.empty((1,), dtype=torch.float32, device=dev) if s.regularizer == "kl" else None
+        h = torch.empty((B, hC, tz, self.Hz, self.Wz), dtype=torch.float32, device=dev)
+        ws = state.workspace(n)
+        N.check(lib.vt_encode_chunk_pre(state.handle, int(first), _ptr(x), s.in_channels, n, _ptr(noise), _ptr(z), _ptr(idx),
+                                        _ptr(kl_batch), _ptr(h), _ptr(ws), ws.numel(), _stream_ptr(dev)))
+        out = {}
+        for r in rows:
+            self._add_losses(self.losses[slot_of[r]], h[r:r + 1], tz)
+            out[r] = (z[r:r + 1], idx[r:r + 1] if idx is not None else None)
+        return out
+
+    def _add_losses(self, L: _SlotLosses, h: torch.Tensor, tz: int):
+        """one chunk of one video: KL from its pre-bound slice (vt_op_kl), FSQ aux partials (vt_fsq_aux_partials)"""
+        s, dev = self.spec, self.native.device
+        L.n_chunks += 1
+        if s.regularizer == "kl":
+            P = tz * self.Hz * self.Wz
+            zs = torch.empty((1, s.z_channels, tz, self.Hz, self.Wz), dtype=torch.float32, device=dev)
+            kl = torch.empty((), dtype=torch.float32, device=dev)
+            N.check(self.native.lib.vt_op_kl(_ptr(h), None, s.z_channels, P, 1, 0, _ptr(zs), _ptr(kl), _stream_ptr(dev)))
+            L.kl_sum = L.kl_sum + kl   # in chunk order, as tile_encode's mean sums them
+        elif self.aux:
+            stats, avg = self.reg.aux_partials(h)
+            if s.version == 0:   # all of the video's tokens as one segment, as the whole-clip encode
+                tokens = tz * self.Hz * self.Wz
+                L.tok_stats += tokens * stats[0].double()
+                L.tok_avg += tokens * avg[0].double()
+                L.tokens += tokens
+                L.aux_loss = self.reg.aux_finalize((L.tok_stats / L.tokens).float().view(1, 2),
+                                                   (L.tok_avg / L.tokens).float().view(1, -1),
+                                                   n_steps=self.model.global_step // 2, world_size=1)
+            else:                # tile_encode: the mean over the chunks of each chunk's aux
+                aux = self.reg.aux_finalize(stats, avg, n_steps=self.model.global_step // 2, world_size=1)
+                L.aux_sum = L.aux_sum + aux
+                L.aux_loss = EncodeStream._mean(L.aux_sum, L.n_chunks)
+
+
+class DecodePool(_Pool):
+    """S slots of one decoder, one latent (Hz, Wz): the decoding counterpart of EncodePool.  Each video's decoded frames
+    equal its own tile_decode (v1.1, t_chunk = t_chunk_dec, the same use_overlap) or its whole-clip decode (v1.0).
+
+        pool = DecodePool(model, capacity=S, Hz=Hz, Wz=Wz, t_chunk=4, use_overlap=True)
+        a = pool.open(); pool.push(a, z)                # z [1, z_channels, tz, Hz, Wz], or FSQ indices [1, tz, Hz, Wz]
+        for slot, frames in pool.step().items(): ...
+        frames = pool.close(a)                          # the last chunk, without look-ahead"""
+
+    def __init__(self, model, capacity: int, Hz: int, Wz: int, t_chunk: Optional[int] = None, use_overlap: bool = False):
+        super().__init__(model, capacity, Hz, Wz, is_decoder=True, t_chunk=t_chunk, use_overlap=use_overlap)
+        self.f = self.native.spatial_factor()
+
+    def open(self) -> int:
+        return self._open()
+
+    def push(self, slot: int, z: torch.Tensor):
+        self.sched.check(slot)
+        if not z.is_cuda:
+            raise RuntimeError("vidtok_b200: inputs must be CUDA tensors; there is no CPU path")
+        s = self.spec
+        if z.dim() == 4 and not z.is_floating_point():
+            if s.regularizer != "fsq":
+                raise ValueError("token indices need an FSQ model")
+            z = self.model.indices_to_latent(z)
+        if z.dim() != 5 or tuple(z.shape[:2]) != (1, s.z_channels) or tuple(z.shape[3:]) != (self.H, self.W):
+            raise ValueError(f"expected a [1,{s.z_channels},tz,{self.H},{self.W}] latent, got {tuple(z.shape)}")
+        self._buffer(slot, z.detach().to(torch.float32))
+
+    def step(self) -> Dict[int, torch.Tensor]:
+        """Runs every first chunk that is buffered (side state, then transplanted into its slot) and one batched chunk of
+        every slot with a full chunk (and its look-ahead) buffered.  Returns {slot: decoded frames} of the slots that
+        produced frames."""
+        joins, ready, chunk = self.sched.plan_step()
+        parts: Dict[int, List[torch.Tensor]] = {}
+        for s, c in joins:
+            parts.setdefault(s, []).append(self._run(self.side, {0: self._take(s, c)}, c, first=True)[0])
+            self.counts["side"] += 1
+            self._copy(self.main, self.side, [s], [0])
+        if ready:
+            got = self._batched(ready, chunk, lambda rows: self._run(self.main, rows, chunk, first=False))
+            for s in ready:
+                parts.setdefault(s, []).append(got[s])
+        return {s: self._cat(p) for s, p in parts.items()}
+
+    def close(self, slot: int) -> torch.Tensor:
+        """End of the slot's video: decodes the latents still buffered on the side state (the last chunk without
+        look-ahead) and frees the slot."""
+        started, chunks = self.sched.close(slot)
+        if started and chunks:
+            self._copy(self.side, self.main, [0], [slot])
+        parts = []
+        for i, c in enumerate(chunks):
+            parts.append(self._run(self.side, {0: self._take(slot, c)}, c, first=not started and i == 0)[0])
+            self.counts["side"] += 1
+        self.pending[slot] = None
+        return self._cat(parts)
+
+    def _cat(self, parts: List[torch.Tensor]) -> torch.Tensor:
+        if not parts:
+            return torch.empty((1, self.spec.out_ch, 0, self.H * self.f, self.W * self.f), dtype=self.out_dtype,
+                               device=self.native.device)
+        x = parts[0].contiguous() if len(parts) == 1 else torch.cat(parts, dim=2)
+        return x.to(self.out_dtype)
+
+    def _run(self, state: ChunkState, rows: Dict[int, torch.Tensor], chunk: Tuple[int, int, int], first: bool) -> Dict[int, torch.Tensor]:
+        s, dev = self.spec, self.native.device
+        B = self.S if state is self.main else 1
+        n, _, trim = chunk
+        To = self.native.decoded_frames(n) if (first or s.version == 1) else n * self.tdf
+        z = self._stack(rows, B)
+        out = torch.empty((B, s.out_ch, To, self.H * self.f, self.W * self.f), dtype=torch.float32, device=dev)
+        ws = state.workspace(n)
+        N.check(self.native.lib.vt_decode_chunk(state.handle, int(first), _ptr(z), s.z_channels, n, _ptr(out), _ptr(ws), ws.numel(),
+                                                _stream_ptr(dev)))
+        return {r: out[r:r + 1, :, :To - trim] if trim else out[r:r + 1] for r in rows}
