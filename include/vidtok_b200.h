@@ -35,7 +35,9 @@ typedef enum {
   VT_ERR_CUDA = -2,       /* CUDA runtime or driver error */
   VT_ERR_NOT_READY = -3,  /* parameters missing or vt_model_finalize not called */
   VT_ERR_WORKSPACE = -4,  /* workspace too small */
-  VT_ERR_NO_DEVICE = -5   /* no sm_90a (H100) device: there is deliberately no CPU fallback */
+  VT_ERR_NO_DEVICE = -5,  /* no sm_90a (H100) device: there is deliberately no CPU fallback */
+  VT_ERR_CAPTURE = -6     /* the caller's stream is capturing a CUDA graph and the call would allocate, synchronise or
+                             copy from host memory (see "CUDA graph capture" below); nothing was enqueued */
 } vt_status;
 
 /* Precision modes.
@@ -97,7 +99,7 @@ int64_t vt_launch_count(int32_t reset);
 
 /* Optional per-kernel profile of everything this thread launches between start and stop: CUDA events on the launch
  * stream around every kernel (adds launch gaps: use it to attribute time, not to measure throughput).
- * vt_profile_stop synchronises the device and writes a JSON object
+ * vt_profile_stop waits for the profiled kernels (their events, not the device) and writes a JSON object
  * {"kernel": {"launches": n, "ms": total, "flops": algorithmic, "bytes": algorithmic}, ...}; returns its length. */
 void vt_profile_start(void);
 void vt_profile_start_detailed(void); /* keys additionally carry the layer geometry */
@@ -189,6 +191,30 @@ int32_t vt_decode_chunk(vt_chunk_state* s, int32_t is_first, const float* z_chun
  * slot listed twice, or a cache whose per-slot size differs between the two.  Calls on one dst state must use one stream. */
 int32_t vt_chunk_state_copy_slots(vt_chunk_state* dst, const vt_chunk_state* src, int32_t n, const int32_t* dst_slots,
                                   const int32_t* src_slots, void* stream);
+
+/* ---- CUDA graph capture.  vt_encode, vt_decode, vt_encode_chunk, vt_encode_chunk_pre, vt_encode_chunk_fsq_aux and
+ *      vt_decode_chunk may be captured into a CUDA graph on the caller's stream: they launch kernels and stream-ordered
+ *      memsets only, with every tensor map and launch parameter fixed at capture.  State a call may create must exist before
+ *      capture: the residual identity tiles (made by vt_model_finalize) and, for a chunk state, both buffers of every cache a
+ *      chunk of that length uses (vt_chunk_state_reserve).  Each entry point asks cudaStreamIsCapturing of `stream`; when
+ *      it is capturing and the call would allocate, synchronise or copy from host memory, it returns VT_ERR_CAPTURE before
+ *      anything is enqueued and vt_last_error() names what was missing.  Refused under capture: vt_encode_video,
+ *      vt_decode_video and vt_encode_video_fsq_aux (library copy stream, host staging), vt_chunk_state_copy_slots (uploads
+ *      a host table), any call while the profiler is on, and a chunk whose caches were not reserved.
+ *      A captured chunk is only valid for the cache parity it was captured at: it reads buffer `parity` and writes the other
+ *      one of every cache.  Capturing updates the state as running the chunk would (its caches flip); a replay of that graph
+ *      must be followed by vt_chunk_state_advance, with no other chunk call on the state in between. ---- */
+/* Allocates (or takes from the model's pool) and zeroes both buffers of every cache a chunk of T_chunk frames (encoder) or
+ * latent frames (decoder) uses, found by the dry run of vt_chunk_workspace_bytes; caches already held at that size are left
+ * as they are.  The zeroing is enqueued on `stream`, which must not be capturing (VT_ERR_CAPTURE).  After it, chunks of that
+ * length run under capture. */
+int32_t vt_chunk_state_reserve(vt_chunk_state* s, int32_t T_chunk, void* stream);
+/* The cur bit of the state's double-buffered caches (every cache commits on every chunk, so they agree): 0 or 1, 0 for a
+ * state that holds no cache yet, -1 (and a message) for a null state or caches that disagree. */
+int32_t vt_chunk_state_parity(const vt_chunk_state* s);
+/* Marks one chunk as run outside the library, by the replay of a graph captured at the current parity: every cache flips
+ * its parity and counts as written, as the chunk call itself would have left them.  Enqueues nothing. */
+int32_t vt_chunk_state_advance(vt_chunk_state* s);
 
 /* ---- whole-video tiling below the ABI (tile_encode / tile_decode, autoencoder_v1_1.py:218-228,244-264,302-331): the chunk
  *      schedule, the causal caches and the chunk staging run inside the library -- one call per video, no host

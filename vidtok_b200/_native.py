@@ -10,6 +10,7 @@ VT_MAX_LEVELS = 8
 PREC_FMA32, PREC_BF16, PREC_EXACT_TC, PREC_MIXED = 0, 1, 2, 3
 PREC_EXACT = PREC_EXACT_TC  # the parity mode
 DTYPE_F32, DTYPE_BF16, DTYPE_F16 = 0, 1, 2   # VT_DTYPE_*
+ERR_CAPTURE = -6   # VT_ERR_CAPTURE: refused while the stream captures a CUDA graph
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libvidtok_b200.so")
 
@@ -68,6 +69,9 @@ _SIGS = {
     "vt_encode_chunk_fsq_aux": (_I32, [_P, _I32, _P, _I32, _I32, _P, _P, C.c_float, _P, _P, _P, _I64, _P]),
     "vt_decode_chunk": (_I32, [_P, _I32, _P, _I32, _I32, _P, _P, _I64, _P]),
     "vt_chunk_state_copy_slots": (_I32, [_P, _P, _I32, C.POINTER(_I32), C.POINTER(_I32), _P]),
+    "vt_chunk_state_reserve": (_I32, [_P, _I32, _P]),
+    "vt_chunk_state_parity": (_I32, [_P]),
+    "vt_chunk_state_advance": (_I32, [_P]),
     "vt_encode_video_workspace_bytes": (_I64, [_P, _I32, _I32, _I32, _I32, _I32, _I32]),
     "vt_encode_video": (_I32, [_P, _I32, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _I64, _P]),
     "vt_encode_video_fsq_aux_workspace_bytes": (_I64, [_P, _I32, _I32, _I32, _I32, _I32, _I32]),

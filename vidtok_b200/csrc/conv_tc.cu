@@ -895,9 +895,45 @@ int choose_bn(int Co) {
   return 0;
 }
 
+// The residual-through-MMA identity of device dev: 256 x 256 bf16 I, or the 16 fp16 matrices 2^s * I of the split mode.
+// Made once per device and precision, and filled (s synchronised) before any launch can read it.  Making it allocates and
+// synchronises, which a capturing stream must not do: there it is an error (vt_model_finalize makes both in advance).
+cudaError_t identity_tiles(int dev, bool split, cudaStream_t s, const bf16** out) {
+  static bf16* ident_dev[2][kMaxDevices] = {{nullptr}};
+  static std::mutex ident_mu;
+  const int ik = split ? 1 : 0;
+  std::lock_guard<std::mutex> lock(ident_mu);
+  if (!ident_dev[ik][dev]) {
+    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+    if (cudaStreamIsCapturing(s, &cap) != cudaSuccess || cap != cudaStreamCaptureStatusNone) {
+      cudaGetLastError();
+      g_tc_err = "the residual identity tiles do not exist yet and the stream is capturing";
+      return cudaErrorStreamCaptureUnsupported;
+    }
+    const int nmat = split ? 16 : 1;
+    bf16* e = nullptr;
+    cudaError_t err = cudaMalloc(&e, (size_t)nmat * 256 * 256 * sizeof(bf16));
+    if (err != cudaSuccess) { g_tc_err = "cudaMalloc(identity)"; return err; }
+    for (int i = 0; i < nmat; ++i) fill_identity_kernel<<<256, 256, 0, s>>>(e + (size_t)i * 256 * 256, ik, ldexpf(1.0f, i));
+    if ((err = cudaStreamSynchronize(s)) != cudaSuccess) { cudaFree(e); g_tc_err = "identity fill"; return err; }
+    ident_dev[ik][dev] = e;
+  }
+  *out = ident_dev[ik][dev];
+  return cudaSuccess;
+}
+
 }  // namespace
 
 const char* conv_tc_last_error() { return g_tc_err.c_str(); }
+
+cudaError_t conv_tc_prepare_identity(cudaStream_t s) {
+  int dev = 0;
+  if (cudaError_t e = current_device(dev)) return e;
+  const bf16* unused;
+  for (int split = 0; split < 2; ++split)
+    if (cudaError_t e = identity_tiles(dev, split != 0, s, &unused)) return e;
+  return cudaSuccess;
+}
 
 bool conv_tc_plan(const ConvP& p, DType tout, const TcLnFusion* ln, const TcRegFusion* reg, int w_batches, TcPlan* out) {
   g_tc_err.clear();
@@ -1099,24 +1135,9 @@ cudaError_t launch_conv_tc(const TcPlan& pl, const bf16* x, const bf16* w_nk, vo
   };
   maps.r = maps.a[0]; maps.e = maps.b;
   if (t.res_mma) {
-    // 256 x 256 identity: bf16 I, or the 16 fp16 matrices 2^s * I of the split mode; built once per device, and filled
-    // before any launch can read it
-    static bf16* ident_dev[2][kMaxDevices] = {{nullptr}};
-    static std::mutex ident_mu;
-    const int ik = split ? 1 : 0;
-    {
-      std::lock_guard<std::mutex> lock(ident_mu);
-      if (!ident_dev[ik][dev]) {
-        const int nmat = split ? 16 : 1;
-        bf16* e = nullptr;
-        cudaError_t err = cudaMalloc(&e, (size_t)nmat * 256 * 256 * sizeof(bf16));
-        if (err != cudaSuccess) { g_tc_err = "cudaMalloc(identity)"; return err; }
-        for (int i = 0; i < nmat; ++i) fill_identity_kernel<<<256, 256, 0, s>>>(e + (size_t)i * 256 * 256, ik, ldexpf(1.0f, i));
-        if ((err = cudaStreamSynchronize(s)) != cudaSuccess) { cudaFree(e); g_tc_err = "identity fill"; return err; }
-        ident_dev[ik][dev] = e;
-      }
-    }
-    const bf16* ident = ident_dev[ik][dev] + (size_t)pl.ident_s * 256 * 256;
+    const bf16* ident = nullptr;
+    if (cudaError_t err = identity_tiles(dev, split, s, &ident)) return err;
+    ident += (size_t)pl.ident_s * 256 * 256;
     if (!encode_out(&maps.r, p.res, p.resT, p.rsW, p.rsH, p.rsT, p.rsB, t.halo ? t.hP : t.BW, t.halo ? 16 + p.kh - 1 : t.BH, t.BT)) return cudaErrorInvalidValue;
     cuuint64_t dims[3] = {256, 256, 1};
     cuuint64_t strides[2] = {512, 256 * 512};

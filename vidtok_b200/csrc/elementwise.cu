@@ -47,7 +47,9 @@ void prof_start() {
 // aggregates per kernel name into a JSON object; returns the number of bytes written (0 if it does not fit)
 int prof_stop(char* buf, int cap) {
   g_prof_on = false;
-  cudaDeviceSynchronize();
+  // wait for the profiled kernels' own events rather than the device: a device-wide synchronise would break a CUDA graph
+  // that another stream is capturing (the tokenizer refuses to launch under capture while the profiler is on)
+  for (auto& r : g_prof) cudaEventSynchronize(r.e1);
   struct Agg { std::string name; long long n; double ms, flops, bytes; };
   std::vector<Agg> aggs;
   for (auto& r : g_prof) {

@@ -172,6 +172,9 @@ bool conv_tc_plan(const ConvP& p, DType tout, const TcLnFusion* ln, const TcRegF
 // w_nk: [Co_pad][K = taps * Cin] bf16 weights, w_batch_stride apart when batched; out may be null when a regularizer
 // epilogue consumes the result.  A driver without cuTensorMapEncodeTiled is a launch error.
 cudaError_t launch_conv_tc(const TcPlan& pl, const bf16* x, const bf16* w_nk, void* out, cudaStream_t s, long long w_batch_stride = 0);
+// Makes the current device's residual identity tiles (bf16 and split) that res_mma launches read, if they do not exist yet;
+// synchronises s when it makes them.  A launch that needs them while its stream is capturing fails instead of making them.
+cudaError_t conv_tc_prepare_identity(cudaStream_t s);
 cudaError_t launch_kl_clear(double* scratch, cudaStream_t s);
 cudaError_t launch_kl_finish(const double* scratch, int B, float* kl_loss, cudaStream_t s);
 // decoder head through per-tap partial outputs (see elementwise.cu)

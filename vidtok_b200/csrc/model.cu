@@ -321,6 +321,8 @@ struct vt_chunk_state {
   // device segment table of vt_chunk_state_copy_slots into this state (grown on demand; stream-ordered reuse)
   void* seg_table = nullptr;
   size_t seg_table_bytes = 0;
+  // vt_chunk_state_reserve: chunk length -> the caches (key, bytes) such a chunk uses, checked before a captured chunk
+  std::map<int, std::map<std::string, size_t>> reserved;
   ~vt_chunk_state() {
     for (auto& kv : caches)
       for (int i = 0; i < 2; ++i)
@@ -1601,6 +1603,8 @@ int32_t vt_model_finalize(vt_model* m, void* stream) {
     n->gamma = m->pool + m->params[n->pg].offset;
     n->beta = m->pool + m->params[n->pb].offset;
   }
+  // made here rather than on first use, so that a first call inside a CUDA graph capture finds them
+  VT_CUDA(conv_tc_prepare_identity(s));
   VT_CUDA(cudaStreamSynchronize(s));
   auto set_alpha = [&](LevelW& lv) -> int {
     if (!lv.has_tres) return VT_OK;
@@ -1661,6 +1665,42 @@ static int check_stream_chunk(const vt_model* m, bool first, int Tc) {
 
 static int check_precision(int precision) {
   if (precision < 0 || precision > VT_PREC_MIXED) return fail(VT_ERR_INVALID, "unknown precision mode %d", precision);
+  return VT_OK;
+}
+
+// ---- CUDA graph capture (include/vidtok_b200.h) ----------------------------------------------------------------------------
+// Whether s is capturing a graph.  The legacy stream while another stream captures counts as capturing: the call then refuses
+// rather than join the caller's capture implicitly.
+static bool capturing(cudaStream_t s) {
+  cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+  const cudaError_t e = cudaStreamIsCapturing(s, &st);
+  if (e != cudaSuccess) { cudaGetLastError(); return e == cudaErrorStreamCaptureImplicit; }
+  return st != cudaStreamCaptureStatusNone;
+}
+// The calls that allocate, synchronise or copy from host memory: VT_ERR_CAPTURE under capture
+static int refuse_capture(cudaStream_t s, const char* what) {
+  if (capturing(s)) return fail(VT_ERR_CAPTURE, "%s cannot run while the stream is capturing a CUDA graph", what);
+  return VT_OK;
+}
+// The capturable calls: the profiler's events cannot be read back from a graph
+static int check_capture(cudaStream_t s) {
+  if (prof_enabled() && capturing(s)) return fail(VT_ERR_CAPTURE, "the profiler is on: stop it before capturing a CUDA graph");
+  return VT_OK;
+}
+// A chunk call under capture: every cache the chunk uses must be held at its size (vt_chunk_state_reserve), and a later chunk
+// needs them written, so that Exec::cache neither allocates nor fails half way through the capture
+static int check_chunk_capture(const vt_chunk_state* cs, int Tc, cudaStream_t s) {
+  if (!capturing(s)) return VT_OK;
+  if (prof_enabled()) return fail(VT_ERR_CAPTURE, "the profiler is on: stop it before capturing a CUDA graph");
+  auto r = cs->reserved.find(Tc);
+  if (r == cs->reserved.end())
+    return fail(VT_ERR_CAPTURE, "chunks of %d frames were not reserved (vt_chunk_state_reserve) before the capture", Tc);
+  for (const auto& kv : r->second) {
+    auto c = cs->caches.find(kv.first);
+    if (c == cs->caches.end() || c->second.bytes != kv.second || !c->second.buf[0] || !c->second.buf[1])
+      return fail(VT_ERR_CAPTURE, "cache %s is not held at %zu bytes: reserve the chunk length again before the capture", kv.first.c_str(), kv.second);
+    if (!cs->first && !c->second.valid) return fail(VT_ERR_NOT_READY, "cache %s empty on a non-first chunk", kv.first.c_str());
+  }
   return VT_OK;
 }
 
@@ -1727,6 +1767,8 @@ int32_t vt_encode(vt_model* m, int32_t precision, const float* x, int32_t B, int
   rc = check_hw(m, H, W);
   if (rc) return rc;
   VT_CUDA(cudaSetDevice(m->device));
+  rc = check_capture((cudaStream_t)stream);
+  if (rc) return rc;
   Exec ex(m, stack_prec(precision, false), (cudaStream_t)stream, workspace, (size_t)workspace_bytes, false);
   vt_chunk_state one; one.m = m; one.persist = false; one.first = true;
   if (m->desc.version == 1) ex.ck = &one;
@@ -1741,6 +1783,7 @@ int32_t vt_decode(vt_model* m, int32_t precision, const void* z, int32_t from_in
   if (check_precision(precision)) return VT_ERR_INVALID;
   VT_CUDA(cudaSetDevice(m->device));
   cudaStream_t s = (cudaStream_t)stream;
+  if (int rc = check_capture(s)) return rc;
   Exec ex(m, stack_prec(precision, true), s, workspace, (size_t)workspace_bytes, false);
   vt_chunk_state one; one.m = m; one.persist = false; one.first = true; one.is_decoder = true;
   if (m->desc.version == 1) ex.ck = &one;
@@ -1804,6 +1847,65 @@ int64_t vt_chunk_workspace_bytes(const vt_chunk_state* cs, int32_t Tc) {
   return (int64_t)(peak + 4096);
 }
 
+int32_t vt_chunk_state_reserve(vt_chunk_state* cs, int32_t Tc, void* stream) {
+  if (!cs) return fail(VT_ERR_INVALID, "null state");
+  if (Tc <= 0) return fail(VT_ERR_INVALID, "bad shape");
+  vt_model* m = cs->m;
+  VT_CUDA(cudaSetDevice(m->device));
+  cudaStream_t s = (cudaStream_t)stream;
+  if (int rc = refuse_capture(s, "vt_chunk_state_reserve (it allocates)")) return rc;
+  // the caches a first and a later chunk of Tc frames use, from the dry run vt_chunk_workspace_bytes makes
+  vt_chunk_state tmp;
+  tmp.m = m; tmp.prec = cs->prec; tmp.B = cs->B; tmp.H = cs->H; tmp.W = cs->W;
+  tmp.is_decoder = cs->is_decoder; tmp.use_overlap = cs->use_overlap; tmp.persist = true;
+  for (int first = 0; first < 2; ++first) {
+    tmp.first = first != 0;
+    Exec ex(m, stack_prec(cs->prec, cs->is_decoder), 0, nullptr, 0, true);
+    ex.ck = &tmp;
+    if (cs->is_decoder) {
+      run_decoder(ex, (const float*)(uintptr_t)0x1000, cs->B, Tc, cs->H, cs->W, (float*)(uintptr_t)0x1000);
+    } else {
+      run_encoder(ex, (const float*)(uintptr_t)0x1000, cs->B, Tc, cs->H, cs->W, (float*)(uintptr_t)0x1000);
+    }
+    if (!ex.ok()) return ex.rc;
+  }
+  const int parity = vt_chunk_state_parity(cs);
+  std::map<std::string, size_t>& need = cs->reserved[Tc];
+  need.clear();
+  for (const auto& kv : tmp.caches) {
+    const size_t bytes = kv.second.bytes;
+    need[kv.first] = bytes;
+    vt::CacheBuf& c = cs->caches[kv.first];
+    if (c.bytes == bytes && c.buf[0] && c.buf[1]) continue;
+    for (int i = 0; i < 2; ++i) {
+      if (c.buf[i]) vt::pool_put(m, c.bytes, c.buf[i]);
+      c.buf[i] = vt::pool_take(m, bytes);
+      if (!c.buf[i]) VT_CUDA(cudaMalloc(&c.buf[i], bytes));
+      VT_CUDA(cudaMemsetAsync(c.buf[i], 0, bytes, s));
+    }
+    c.bytes = bytes; c.valid = false; c.cur = parity > 0 ? parity : 0;   // in step with the caches already held
+  }
+  return VT_OK;
+}
+
+int32_t vt_chunk_state_parity(const vt_chunk_state* cs) {
+  if (!cs) { fail(VT_ERR_INVALID, "null state"); return -1; }
+  int parity = -1;
+  for (const auto& kv : cs->caches) {
+    if (!kv.second.buf[0]) continue;
+    if (parity >= 0 && kv.second.cur != parity) { fail(VT_ERR_INVALID, "the caches of the state are not in step (%s)", kv.first.c_str()); return -1; }
+    parity = kv.second.cur;
+  }
+  return parity < 0 ? 0 : parity;
+}
+
+int32_t vt_chunk_state_advance(vt_chunk_state* cs) {
+  if (!cs) return fail(VT_ERR_INVALID, "null state");
+  for (auto& kv : cs->caches)
+    if (kv.second.buf[0]) kv.second.commit();
+  return VT_OK;
+}
+
 // h_out (optional): the chunk's encoder output before the regularizer, fp32 [B,Cz,Tz,Hz,Wz] (the FSQ aux loss reads it)
 static int encode_chunk(vt_chunk_state* cs, int32_t is_first, const float* x_chunk, int32_t C, int32_t Tc, const float* noise,
                         float* z, int32_t* indices, float* kl_loss, float* h_out, void* workspace, int64_t workspace_bytes,
@@ -1818,6 +1920,8 @@ static int encode_chunk(vt_chunk_state* cs, int32_t is_first, const float* x_chu
   rc = check_stream_chunk(m, is_first != 0, Tc);
   if (rc) return rc;
   cs->first = is_first != 0;
+  rc = check_chunk_capture(cs, Tc, (cudaStream_t)stream);
+  if (rc) return rc;
   Exec ex(m, stack_prec(cs->prec, false), (cudaStream_t)stream, workspace, (size_t)workspace_bytes, false);
   ex.ck = cs;
   return encode(ex, x_chunk, cs->B, Tc, cs->H, cs->W, noise, z, indices, kl_loss, h_out);
@@ -1844,6 +1948,7 @@ int32_t vt_decode_chunk(vt_chunk_state* cs, int32_t is_first, const float* z_chu
   if (Tzc <= 0) return fail(VT_ERR_INVALID, "bad shape");
   VT_CUDA(cudaSetDevice(m->device));
   cs->first = is_first != 0;
+  if (int rc = check_chunk_capture(cs, Tzc, (cudaStream_t)stream)) return rc;
   Exec ex(m, stack_prec(cs->prec, true), (cudaStream_t)stream, workspace, (size_t)workspace_bytes, false);
   ex.ck = cs;
   run_decoder(ex, z_chunk, cs->B, Tzc, cs->H, cs->W, x_out);
@@ -1885,6 +1990,7 @@ int32_t vt_chunk_state_copy_slots(vt_chunk_state* dst, const vt_chunk_state* src
   vt_model* m = dst->m;
   VT_CUDA(cudaSetDevice(m->device));
   cudaStream_t s = (cudaStream_t)stream;
+  if (int rc = refuse_capture(s, "vt_chunk_state_copy_slots (it uploads a host table)")) return rc;
   std::vector<SlotSeg> segs;
   unsigned long long max_bytes = 0, total = 0;
   for (const auto& kv : src->caches) {
@@ -2104,6 +2210,8 @@ static int encode_video(vt_model* m, int32_t precision, const float* x, int32_t 
   rc = check_hw(m, H, W);
   if (rc) return rc;
   VT_CUDA(cudaSetDevice(m->device));
+  rc = refuse_capture((cudaStream_t)stream, "whole-video tiling (tile_encode / tile_decode: the library's copy stream and staging)");
+  if (rc) return rc;
   rc = ensure_copy_stream(m);
   if (rc) return rc;
   const vt_model_desc& d = m->desc;
@@ -2276,6 +2384,8 @@ int32_t vt_decode_video(vt_model* m, int32_t precision, const float* z, int32_t 
   const int tdf = d.time_downsample_factor;
   if (use_overlap && tdf != 2 && tdf != 4 && tdf != 8) return fail(VT_ERR_INVALID, "use_overlap supports 2x, 4x or 8x temporal downsampling only");
   VT_CUDA(cudaSetDevice(m->device));
+  rc = refuse_capture((cudaStream_t)stream, "whole-video tiling (tile_encode / tile_decode: the library's copy stream and staging)");
+  if (rc) return rc;
   rc = ensure_copy_stream(m);
   if (rc) return rc;
   cudaStream_t s = (cudaStream_t)stream, cs = m->copy_stream;

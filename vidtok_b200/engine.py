@@ -110,12 +110,25 @@ class TokenizerSpec:
         return d
 
 
+def _capturing() -> bool:
+    """The current stream is capturing a CUDA graph (torch.cuda.graph, or torch.compile's CUDA graphs)."""
+    return torch.cuda.is_available() and torch.cuda.is_current_stream_capturing()
+
+
 def _stream_ptr(device: torch.device) -> C.c_void_p:
     return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
 
 def _ptr(t: Optional[torch.Tensor]) -> C.c_void_p:
     return C.c_void_p(0 if t is None else t.data_ptr())
+
+
+def _refuse_capture(what: str):
+    """Calls that stage through the library's copy stream, draw CPU noise or move slots with host tables cannot be captured
+    in a CUDA graph: refused before anything is enqueued, so the caller's capture stays intact."""
+    if _capturing():
+        raise RuntimeError(f"vidtok_b200: {what} cannot be captured in a CUDA graph (VT_ERR_CAPTURE): run it eagerly; untiled "
+                           "encode / decode / forward and the steady chunks of the streams are the capturable calls")
 
 
 # --------------------------------------------------------------------------------------------------
@@ -132,6 +145,10 @@ class NativeModel:
         N.check(self.lib.vt_model_create(C.byref(desc), device_index, C.byref(self.handle)))
         self.device_index = device_index
         self._ws: Optional[torch.Tensor] = None
+        # workspaces that a captured CUDA graph reads: kept for the model's lifetime once the workspace grows past them, so
+        # that the graph never replays into memory torch has handed to someone else
+        self._ws_captured = False
+        self._ws_kept: List[torch.Tensor] = []
         # handles of the open chunk states: a state returns its caches to the model when destroyed, so any still open go
         # first (the garbage collector finalises a cycle holding both in no particular order)
         self._chunk_handles: Dict[int, C.c_void_p] = {}
@@ -187,9 +204,19 @@ class NativeModel:
     def _workspace(self, nbytes: int) -> torch.Tensor:
         if nbytes < 0:
             raise RuntimeError(f"vidtok_b200: {self.lib.vt_last_error().decode()}")
+        capturing = _capturing()
         if self._ws is None or self._ws.numel() < nbytes:
+            if capturing:
+                raise RuntimeError(f"vidtok_b200: the workspace ({0 if self._ws is None else self._ws.numel()} bytes) is smaller than the "
+                                   f"{nbytes} bytes this call needs, and it cannot grow while a CUDA graph is being captured: run "
+                                   "the call once eagerly with the same geometry and precision before capturing it")
+            if self._ws is not None and self._ws_captured:
+                self._ws_kept.append(self._ws)
             self._ws = None
+            self._ws_captured = False
             self._ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        if capturing:
+            self._ws_captured = True
         return self._ws
 
     def workspace_for(self, precision: int, B: int, T: int, H: int, W: int) -> torch.Tensor:
@@ -572,6 +599,10 @@ class FSQRegularizer(nn.Module):
         components (optional, fp32 [n,4] on the device) receives each segment's (per_sample_entropy, codebook_entropy,
         commit_loss, aux)."""
         if world_size is None:
+            import torch.distributed as dist
+            if _capturing() and dist.is_available() and dist.is_initialized():
+                raise RuntimeError("vidtok_b200: the FSQ aux_loss all-reduces avg_prob over the process group, which is not "
+                                   "captured in a CUDA graph: capture without return_reg_log, or pass world_size")
             world_size = _world_size()
             if world_size > 1:
                 import torch.distributed as dist
@@ -658,6 +689,11 @@ class _Runtime:
         if dev.type != "cuda":
             raise RuntimeError("vidtok_b200: the model must live on a CUDA device (model.to('cuda')); there is no CPU path")
         sig = (dev.index, tuple((p.data_ptr(), p._version) for _, p in plist))
+        if _capturing():   # loading and finalizing copy and synchronise: a capture needs the weights the last call used
+            if self.native is None or sig != self._sig:
+                raise RuntimeError("vidtok_b200: the weights changed (or were never loaded) since the last call, and they cannot be "
+                                   "repacked while a CUDA graph is being captured: run one eager call after changing them")
+            return self.native
         if self.native is None or self.native.device_index != (dev.index or 0):
             self.native = NativeModel(self.spec, dev.index or 0)
             self._sig = None
@@ -692,6 +728,18 @@ class _Runtime:
         if x.device.index != nat.device_index:
             raise RuntimeError("input and model are on different devices")
         B, _, T, H, W = x.shape
+        sampled = self.spec.regularizer == "kl" and self.spec.kl_sample
+        if need_reg and noise is not None:
+            if not sampled:
+                raise ValueError("noise= is the KL regularizer's sample: this model does not sample")
+            shape = (B, self.spec.z_channels) + nat.latent_shape(T, H, W)
+            if tuple(noise.shape) != shape or not noise.is_cuda or noise.device.index != nat.device_index:
+                raise ValueError(f"noise must be a CUDA tensor of shape {shape} on the model's device, got {tuple(noise.shape)}")
+            noise = noise.detach().to(torch.float32).contiguous()
+        elif need_reg and sampled and _capturing():
+            raise RuntimeError("vidtok_b200: the KL sample draws its noise on the CPU generator, which a CUDA graph cannot "
+                               "capture: pass noise= (a static device tensor you refill before each replay), or build the "
+                               "regularizer with sample=False")
         if need_reg and noise is None:
             Tz, Hz, Wz = nat.latent_shape(T, H, W)
             noise = self.draw_noise((B, self.spec.z_channels, Tz, Hz, Wz), x.device)
@@ -816,8 +864,10 @@ class AutoencodingEngine(_EngineBase):
 
     _version = 0
 
-    def encode(self, x: Any, return_reg_log: bool = False) -> Any:
-        z, idx, kl, h = self._rt.encode_raw(x, want_h=self._wants_aux(return_reg_log))
+    def encode(self, x: Any, return_reg_log: bool = False, *, noise: Optional[torch.Tensor] = None) -> Any:
+        """noise (extension, KL with sampling): the sample's standard normal draws [B,z,Tz,Hz,Wz] on the device instead of
+        the CPU generator's; required inside a CUDA graph capture."""
+        z, idx, kl, h = self._rt.encode_raw(x, want_h=self._wants_aux(return_reg_log), noise=noise)
         z = z.to(self._rt.out_dtype())
         if return_reg_log:
             return z, self._reg_log(idx, kl, h)
@@ -826,8 +876,8 @@ class AutoencodingEngine(_EngineBase):
     def decode(self, z: Any, decode_from_indices: bool = False) -> torch.Tensor:
         return self._rt.decode_raw(z, decode_from_indices).to(self._rt.out_dtype())
 
-    def forward(self, x: Any):
-        z, reg_log = self.encode(x, return_reg_log=True)
+    def forward(self, x: Any, *, noise: Optional[torch.Tensor] = None):
+        z, reg_log = self.encode(x, return_reg_log=True, noise=noise)
         dec = self.decode(z)
         return z, dec, reg_log
 
@@ -855,11 +905,14 @@ class AutoencodingEngineV11(_EngineBase):
             start = end
         return start_end
 
-    def encode(self, x: Any, return_reg_log: bool = False) -> Any:
+    def encode(self, x: Any, return_reg_log: bool = False, *, noise: Optional[torch.Tensor] = None) -> Any:
+        """noise: as AutoencodingEngine.encode (untiled calls only)."""
         if self.use_tiling:
+            if noise is not None:
+                raise ValueError("noise= applies to untiled calls: tile_encode draws one sample per chunk")
             z, reg_log = self.tile_encode(x)
         else:
-            z, idx, kl, h = self._rt.encode_raw(x, want_h=self._wants_aux(return_reg_log))
+            z, idx, kl, h = self._rt.encode_raw(x, want_h=self._wants_aux(return_reg_log), noise=noise)
             reg_log = self._reg_log(idx, kl, h)
         z = z.to(self._rt.out_dtype())
         if return_reg_log:
@@ -870,7 +923,9 @@ class AutoencodingEngineV11(_EngineBase):
         """autoencoder_v1_1.py:244-264: first frame alone, then chunks of t_chunk_enc, causal caches carried over.  One
         native call per video (vt_encode_video): the chunk loop, the caches and the double-buffered chunk staging live in
         the library.  `x` may be a CUDA tensor or a (pinned) host tensor -- then the chunks are staged host -> device on the
-        library's copy stream while the previous chunk computes."""
+        library's copy stream while the previous chunk computes.  Not capturable in a CUDA graph (the copy stream and the
+        host staging): refused under capture."""
+        _refuse_capture("tile_encode")
         rt = self._rt
         nat = rt.sync()
         if x.dim() != 5:
@@ -928,7 +983,9 @@ class AutoencodingEngineV11(_EngineBase):
     def tile_decode(self, z: Any, out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """autoencoder_v1_1.py:302-331: one look-ahead latent frame per chunk when use_overlap, tail frames dropped.  One
         native call per video (vt_decode_video).  `out` (optional): a pre-allocated fp32 [B,C,T',H,W] tensor, CUDA or pinned
-        host memory -- decoded chunks are then copied out on the library's copy stream while the next chunk computes."""
+        host memory -- decoded chunks are then copied out on the library's copy stream while the next chunk computes.  Not
+        capturable in a CUDA graph, as tile_encode."""
+        _refuse_capture("tile_decode")
         rt = self._rt
         nat = rt.sync()
         if not z.is_cuda:
@@ -957,8 +1014,8 @@ class AutoencodingEngineV11(_EngineBase):
             torch.cuda.current_stream(z.device).synchronize()
         return out
 
-    def forward(self, x: Any):
-        z, reg_log = self.encode(x, return_reg_log=True)
+    def forward(self, x: Any, *, noise: Optional[torch.Tensor] = None):
+        z, reg_log = self.encode(x, return_reg_log=True, noise=noise)
         dec = self.decode(z)
         if dec.shape[2] != x.shape[2]:  # autoencoder_v1_1.py:340-341
             dec = dec[:, :, -x.shape[2]:, ...]

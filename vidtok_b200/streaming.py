@@ -52,7 +52,8 @@ far, with n_steps = global_step // 2 as `encode` uses:
   - v1.1: tile_encode's, the mean over the stream's chunks of each chunk's aux.
 Streams use world size 1: ranks need not push in lockstep, so avg_prob is not all-reduced across ranks.  KL noise is one
 CPU `torch.randn` per push over the push's latent frames (with `t_chunk`: one per chunk, in chunk order, the draws
-tile_encode makes) unless `noise` is passed.  No push synchronises with the host.
+tile_encode makes) unless `noise` is passed.  No push synchronises with the host.  A stream replays its steady chunks
+from CUDA graphs (ChunkGraphs): the same native calls on static buffers, so the outputs are those of the eager chunks.
 
 Pools (EncodePool / DecodePool) carry many videos that start and end independently through one chunk state of batch S
 (the capacity), one slot per video.  Every chunk of a video is a chunk of its own recipe stream (PoolSchedule):
@@ -79,7 +80,7 @@ from typing import Dict, List, Optional, Tuple
 import torch
 
 from . import _native as N
-from .engine import ChunkState, _ptr, _stream_ptr
+from .engine import ChunkState, _ptr, _refuse_capture, _stream_ptr
 
 
 def encode_chunks(avail: int, first: bool, tdf: int, version: int) -> List[int]:
@@ -138,6 +139,60 @@ def recipe_decode_chunks(avail: int, first: bool, t_chunk: int, use_overlap: boo
     return out
 
 
+def chunk_graph_key(n: int, first: bool, final: bool, entry: str, parity: int) -> Optional[Tuple[int, str, int]]:
+    """The CUDA graph a stream chunk replays: None (eager) for a video's first chunk and for the chunk flush() runs, else
+    (frames or latent frames in, entry point, cache parity).  A graph reads one buffer of every double-buffered cache and
+    writes the other, so it is only valid at the parity it was captured at."""
+    if first or final:
+        return None
+    return (int(n), entry, int(parity))
+
+
+class ChunkGraphs:
+    """The CUDA graphs of one stream's steady chunks.  A key that occurs for the first time runs eagerly (lengths seen once
+    never pay for a capture); its second occurrence is captured, after vt_chunk_state_reserve, and runs as the graph's
+    first replay; every later occurrence replays.  Each graph owns static input / output buffers: a push copies its chunk in
+    and its results out, so the tensors it returns are fresh."""
+
+    def __init__(self):
+        self.seen: Dict[Tuple, int] = {}
+        self.graphs: Dict[Tuple, Dict] = {}
+        self.runs: Dict[Tuple, int] = {}   # per key: chunks run by replaying its graph (the capture's own run included)
+        self.replays = 0                    # over all keys
+        self.captures = 0
+
+    def action(self, key: Optional[Tuple]) -> str:
+        """"eager", "capture" or "replay" for the next chunk of this key (counts the occurrence)."""
+        if key is None:
+            return "eager"
+        if key in self.graphs:
+            return "replay"
+        self.seen[key] = self.seen.get(key, 0) + 1
+        return "eager" if self.seen[key] < 2 else "capture"
+
+    def run(self, key: Tuple, action: str, state: ChunkState, launch, bufs: Dict) -> Dict:
+        """Captures (action "capture", launch() being the chunk's native call on the static buffers `bufs`) or looks up the
+        graph of key, replays it and advances the state's caches as the chunk call would have.  Returns the static buffers."""
+        lib = state.native.lib
+        if action == "capture":
+            N.check(lib.vt_chunk_state_reserve(state.handle, key[0], _stream_ptr(state.native.device)))
+            bufs["ws"] = bufs["ws_fn"]()      # sized eagerly, and held here: the graph keeps reading it if the model's grows
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                launch(bufs)                   # capturing flips the caches' parity, as running the chunk does
+            bufs["graph"] = g
+            self.graphs[key] = bufs
+            self.captures += 1
+            g.replay()
+        else:
+            bufs = self.graphs[key]
+            bufs["graph"].replay()
+            N.check(lib.vt_chunk_state_advance(state.handle))
+        self.runs[key] = self.runs.get(key, 0) + 1
+        self.replays += 1
+        return bufs
+
+
 def check_recipe(version: int, tdf: int, t_chunk: Optional[int], use_overlap: bool, is_decoder: bool):
     """The stream options build_chunk_start_end and the overlap rule accept (ValueError otherwise)."""
     if t_chunk is not None:
@@ -172,6 +227,7 @@ class _Stream:
         self.state = ChunkState(self.native, self.precision, self.B, self.H, self.W, is_decoder, self.use_overlap)
         self.first = True
         self.finished = False
+        self.graphs = ChunkGraphs()
 
     def reset(self):
         """Start a new video: the next push is its first chunk (the caches are rewritten, not read)."""
@@ -179,7 +235,12 @@ class _Stream:
         self.finished = False
 
     def close(self):
+        self.graphs = ChunkGraphs()
         self.state.close()
+
+    def _graph_action(self, n: int, final: bool, entry: str) -> Tuple[Optional[Tuple], str]:
+        key = chunk_graph_key(n, self.first, final, entry, self.native.lib.vt_chunk_state_parity(self.state.handle))
+        return key, self.graphs.action(key)
 
     def _workspace(self, n: int) -> torch.Tensor:
         return self.state.workspace(n)
@@ -237,7 +298,7 @@ class EncodeStream(_Stream):
             chunks = encode_chunks(frames.shape[2], self.first, self.tdf, self.spec.version)
         else:
             chunks = recipe_encode_chunks(frames.shape[2], self.first, self.t_chunk, final=False)
-        return self._encode(frames, chunks, noise)
+        return self._encode(frames, chunks, noise, final=False)
 
     def flush(self, noise: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, Dict[str, torch.Tensor]]:
         """End of the video: encodes the frames still held back as the last, shorter chunk (v1.1; a v1.0 stream has
@@ -249,9 +310,9 @@ class EncodeStream(_Stream):
             raise ValueError(f"{n} frames do not complete a group of {self.tdf}: a v1.0 stream encodes videos of 1 + k * {self.tdf} frames")
         frames = self.pending if n else torch.empty((self.B, self.spec.in_channels, 0, self.H, self.W), device=self.native.device)
         self.finished = True
-        return self._encode(frames, [n] if n else [], noise)
+        return self._encode(frames, [n] if n else [], noise, final=True)
 
-    def _encode(self, frames: torch.Tensor, chunks: List[int], noise: Optional[torch.Tensor]):
+    def _encode(self, frames: torch.Tensor, chunks: List[int], noise: Optional[torch.Tensor], final: bool):
         tzs = [self.native.latent_shape(n, self.H, self.W)[0] for n in chunks]
         Tz = sum(tzs)
         dev, s = frames.device, self.spec
@@ -270,30 +331,25 @@ class EncodeStream(_Stream):
         kls = torch.zeros((max(len(chunks), 1),), dtype=torch.float32, device=dev)
         hC = (2 if s.double_z else 1) * s.z_channels
         h = torch.empty((self.B, hC, Tz, self.Hz, self.Wz), dtype=torch.float32, device=dev) if self.keep_pre else None
-        lib, stream = self.native.lib, _stream_ptr(dev)
         t0 = tz0 = 0
+        entry = "pre" if self.keep_pre else ("fsq_aux" if self.aux else "plain")
         for i, (n, tz) in enumerate(zip(chunks, tzs)):
-            xc = frames[:, :, t0:t0 + n].contiguous()
-            zc = torch.empty((self.B, s.z_channels, tz, self.Hz, self.Wz), dtype=torch.float32, device=dev)
-            ic = torch.empty((self.B, tz, self.Hz, self.Wz), dtype=torch.int32, device=dev) if idx is not None else None
-            nc = noise[:, :, tz0:tz0 + tz].contiguous() if kl_noise else None
-            if self.keep_pre:
-                ws = self._workspace(n)
-                hc = torch.empty((self.B, hC, tz, self.Hz, self.Wz), dtype=torch.float32, device=dev)
-                N.check(lib.vt_encode_chunk_pre(self.state.handle, int(self.first), _ptr(xc), s.in_channels, n, _ptr(nc), _ptr(zc),
-                                                _ptr(ic), _ptr(kls[i:i + 1]) if s.regularizer == "kl" else None, _ptr(hc), _ptr(ws),
-                                                ws.numel(), stream))
-                h[:, :, tz0:tz0 + tz] = hc
-            elif self.aux:
-                ws = self.state.aux_workspace(n)
-                N.check(lib.vt_encode_chunk_fsq_aux(self.state.handle, int(self.first), _ptr(xc), s.in_channels, n, _ptr(zc), _ptr(ic),
-                                                    100.0, _ptr(self.aux_stats), _ptr(self.aux_avg), _ptr(ws), ws.numel(), stream))
-                self._add_aux_chunk(self.B * tz * self.Hz * self.Wz)
+            key, action = self._graph_action(n, final, entry)
+            if action != "eager":
+                g = self._graph_chunk(key, action, n, tz, hC)
+                g["x"].copy_(frames[:, :, t0:t0 + n])
+                if kl_noise:
+                    g["noise"].copy_(noise[:, :, tz0:tz0 + tz])
+                g = self.graphs.run(key, action, self.state, self._launch_encode, g)
+                zc, ic = g["z"], g["idx"]
+                if s.regularizer == "kl":
+                    kls[i:i + 1].copy_(g["kl"])
+                if self.keep_pre:
+                    h[:, :, tz0:tz0 + tz] = g["h"]
+                if self.aux:
+                    self._add_aux_chunk(self.B * tz * self.Hz * self.Wz)
             else:
-                ws = self._workspace(n)
-                N.check(lib.vt_encode_chunk(self.state.handle, int(self.first), _ptr(xc), s.in_channels, n, _ptr(nc), _ptr(zc),
-                                            _ptr(ic), _ptr(kls[i:i + 1]) if s.regularizer == "kl" else None, _ptr(ws), ws.numel(),
-                                            stream))
+                zc, ic = self._eager_chunk(frames, noise, kls, h, i, n, tz, t0, tz0, hC, kl_noise, idx is not None)
             z[:, :, tz0:tz0 + tz] = zc
             if idx is not None:
                 idx[:, tz0:tz0 + tz] = ic
@@ -303,6 +359,68 @@ class EncodeStream(_Stream):
             self.n_chunks += 1
             t0 += n
             tz0 += tz
+        return self._finish_push(frames, chunks, idx, kls, h, z, t0, dev)
+
+    def _graph_chunk(self, key: Tuple, action: str, n: int, tz: int, hC: int) -> Dict:
+        """The static buffers of key's graph (new ones for a capture)."""
+        if action == "replay":
+            return self.graphs.graphs[key]
+        s, dev = self.spec, self.native.device
+        lat = (self.B, s.z_channels, tz, self.Hz, self.Wz)
+        kl_noise = s.regularizer == "kl" and s.kl_sample
+        return {
+            "n": n,
+            "x": torch.empty((self.B, s.in_channels, n, self.H, self.W), dtype=torch.float32, device=dev),
+            "noise": torch.empty(lat, dtype=torch.float32, device=dev) if kl_noise else None,
+            "z": torch.empty(lat, dtype=torch.float32, device=dev),
+            "idx": torch.empty((self.B, tz, self.Hz, self.Wz), dtype=torch.int32, device=dev) if s.regularizer == "fsq" else None,
+            "kl": torch.zeros((1,), dtype=torch.float32, device=dev) if s.regularizer == "kl" else None,
+            "h": torch.empty((self.B, hC, tz, self.Hz, self.Wz), dtype=torch.float32, device=dev) if self.keep_pre else None,
+            "ws_fn": (lambda: self.state.aux_workspace(n)) if self.aux else (lambda: self._workspace(n)),
+        }
+
+    def _launch_encode(self, g: Dict):
+        """The chunk's native call on a graph's static buffers (a later chunk: is_first 0)."""
+        s, lib, ws, n = self.spec, self.native.lib, g["ws"], g["n"]
+        stream = _stream_ptr(self.native.device)
+        if self.keep_pre:
+            N.check(lib.vt_encode_chunk_pre(self.state.handle, 0, _ptr(g["x"]), s.in_channels, n, _ptr(g["noise"]), _ptr(g["z"]),
+                                            _ptr(g["idx"]), _ptr(g["kl"]), _ptr(g["h"]), _ptr(ws), ws.numel(), stream))
+        elif self.aux:
+            N.check(lib.vt_encode_chunk_fsq_aux(self.state.handle, 0, _ptr(g["x"]), s.in_channels, n, _ptr(g["z"]), _ptr(g["idx"]),
+                                                100.0, _ptr(self.aux_stats), _ptr(self.aux_avg), _ptr(ws), ws.numel(), stream))
+        else:
+            N.check(lib.vt_encode_chunk(self.state.handle, 0, _ptr(g["x"]), s.in_channels, n, _ptr(g["noise"]), _ptr(g["z"]),
+                                        _ptr(g["idx"]), _ptr(g["kl"]), _ptr(ws), ws.numel(), stream))
+
+    def _eager_chunk(self, frames, noise, kls, h, i, n, tz, t0, tz0, hC, kl_noise, want_idx):
+        s, dev = self.spec, frames.device
+        lib, stream = self.native.lib, _stream_ptr(dev)
+        xc = frames[:, :, t0:t0 + n].contiguous()
+        zc = torch.empty((self.B, s.z_channels, tz, self.Hz, self.Wz), dtype=torch.float32, device=dev)
+        ic = torch.empty((self.B, tz, self.Hz, self.Wz), dtype=torch.int32, device=dev) if want_idx else None
+        nc = noise[:, :, tz0:tz0 + tz].contiguous() if kl_noise else None
+        if self.keep_pre:
+            ws = self._workspace(n)
+            hc = torch.empty((self.B, hC, tz, self.Hz, self.Wz), dtype=torch.float32, device=dev)
+            N.check(lib.vt_encode_chunk_pre(self.state.handle, int(self.first), _ptr(xc), s.in_channels, n, _ptr(nc), _ptr(zc),
+                                            _ptr(ic), _ptr(kls[i:i + 1]) if s.regularizer == "kl" else None, _ptr(hc), _ptr(ws),
+                                            ws.numel(), stream))
+            h[:, :, tz0:tz0 + tz] = hc
+        elif self.aux:
+            ws = self.state.aux_workspace(n)
+            N.check(lib.vt_encode_chunk_fsq_aux(self.state.handle, int(self.first), _ptr(xc), s.in_channels, n, _ptr(zc), _ptr(ic),
+                                                100.0, _ptr(self.aux_stats), _ptr(self.aux_avg), _ptr(ws), ws.numel(), stream))
+            self._add_aux_chunk(self.B * tz * self.Hz * self.Wz)
+        else:
+            ws = self._workspace(n)
+            N.check(lib.vt_encode_chunk(self.state.handle, int(self.first), _ptr(xc), s.in_channels, n, _ptr(nc), _ptr(zc),
+                                        _ptr(ic), _ptr(kls[i:i + 1]) if s.regularizer == "kl" else None, _ptr(ws), ws.numel(),
+                                        stream))
+        return zc, ic
+
+    def _finish_push(self, frames, chunks, idx, kls, h, z, t0, dev):
+        s = self.spec
         self.pending = frames[:, :, t0:].clone() if t0 < frames.shape[2] else None
         if s.regularizer == "fsq":
             if self.aux and chunks and s.version == 0:
@@ -367,13 +485,14 @@ class DecodeStream(_Stream):
         z = z.detach().to(torch.float32).contiguous()
         if self.t_chunk is not None:
             z = z if self.pending is None else torch.cat([self.pending, z], dim=2)
-            return self._decode(z, recipe_decode_chunks(z.shape[2], self.first, self.t_chunk, self.use_overlap, self.tdf, False))
+            return self._decode(z, recipe_decode_chunks(z.shape[2], self.first, self.t_chunk, self.use_overlap, self.tdf, False),
+                                final=False)
         tz = z.shape[2]
         if tz == 0:
             return self._empty(z.device)
         # v1.1: the first latent frame is a chunk of its own (build_chunk_start_end)
         chunks = [1, tz - 1] if self.first and s.version == 1 and tz > 1 else [tz]
-        return self._decode(z, [(n, n, 0) for n in chunks])
+        return self._decode(z, [(n, n, 0) for n in chunks], final=False)
 
     def flush(self) -> torch.Tensor:
         """End of the video: decodes the latent frames still held back (with t_chunk) as the last chunk, without
@@ -383,18 +502,27 @@ class DecodeStream(_Stream):
         if self.pending is None:
             return self._empty(self.native.device)
         return self._decode(self.pending, recipe_decode_chunks(self.pending.shape[2], self.first, self.t_chunk, self.use_overlap,
-                                                               self.tdf, True))
+                                                               self.tdf, True), final=True)
 
-    def _decode(self, z: torch.Tensor, plan: List[Tuple[int, int, int]]) -> torch.Tensor:
+    def _decode(self, z: torch.Tensor, plan: List[Tuple[int, int, int]], final: bool) -> torch.Tensor:
         s = self.spec
         outs = []
         t0 = 0
         for n, step, trim in plan:
             To = self.native.decoded_frames(n) if (self.first or s.version == 1) else n * self.tdf
-            out = torch.empty((self.B, s.out_ch, To, self.H * self.f, self.W * self.f), dtype=torch.float32, device=z.device)
-            ws = self._workspace(n)
-            N.check(self.native.lib.vt_decode_chunk(self.state.handle, int(self.first), _ptr(z[:, :, t0:t0 + n].contiguous()), s.z_channels,
-                                                    n, _ptr(out), _ptr(ws), ws.numel(), _stream_ptr(z.device)))
+            key, action = self._graph_action(n, final, "plain")
+            if action != "eager":
+                g = self.graphs.graphs[key] if action == "replay" else {
+                    "n": n, "ws_fn": lambda n=n: self._workspace(n),
+                    "z": torch.empty((self.B, s.z_channels, n, self.H, self.W), dtype=torch.float32, device=z.device),
+                    "out": torch.empty((self.B, s.out_ch, To, self.H * self.f, self.W * self.f), dtype=torch.float32, device=z.device)}
+                g["z"].copy_(z[:, :, t0:t0 + n])
+                out = self.graphs.run(key, action, self.state, self._launch_decode, g)["out"].clone()
+            else:
+                out = torch.empty((self.B, s.out_ch, To, self.H * self.f, self.W * self.f), dtype=torch.float32, device=z.device)
+                ws = self._workspace(n)
+                N.check(self.native.lib.vt_decode_chunk(self.state.handle, int(self.first), _ptr(z[:, :, t0:t0 + n].contiguous()),
+                                                        s.z_channels, n, _ptr(out), _ptr(ws), ws.numel(), _stream_ptr(z.device)))
             outs.append(out[:, :, :To - trim] if trim else out)
             self.first = False
             t0 += step
@@ -403,6 +531,11 @@ class DecodeStream(_Stream):
             return self._empty(z.device)
         x = outs[0].contiguous() if len(outs) == 1 else torch.cat(outs, dim=2)
         return x.to(self.out_dtype)
+
+    def _launch_decode(self, g: Dict):
+        ws = g["ws"]
+        N.check(self.native.lib.vt_decode_chunk(self.state.handle, 0, _ptr(g["z"]), self.spec.z_channels, g["n"], _ptr(g["out"]),
+                                                _ptr(ws), ws.numel(), _stream_ptr(self.native.device)))
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -631,6 +764,7 @@ class EncodePool(_Pool):
     def step(self) -> Dict[int, Tuple[torch.Tensor, Dict[str, torch.Tensor]]]:
         """Runs every first chunk that is buffered (side state, then transplanted into its slot) and one batched chunk of
         every slot with t_chunk frames buffered.  Returns {slot: (z, reg_log)} for the slots that produced latents."""
+        _refuse_capture("EncodePool.step (slot transplants upload host tables; KL noise comes from the CPU generator)")
         joins, ready, chunk = self.sched.plan_step()
         parts: Dict[int, List] = {}
         for s, c in joins:
@@ -765,6 +899,7 @@ class DecodePool(_Pool):
         """Runs every first chunk that is buffered (side state, then transplanted into its slot) and one batched chunk of
         every slot with a full chunk (and its look-ahead) buffered.  Returns {slot: decoded frames} of the slots that
         produced frames."""
+        _refuse_capture("DecodePool.step (slot transplants upload host tables)")
         joins, ready, chunk = self.sched.plan_step()
         parts: Dict[int, List[torch.Tensor]] = {}
         for s, c in joins:
