@@ -131,6 +131,24 @@ def _refuse_capture(what: str):
                            "encode / decode / forward and the steady chunks of the streams are the capturable calls")
 
 
+def chunk_start_end(t: int, step: int) -> List[Tuple[int, int]]:
+    """build_chunk_start_end (autoencoder_v1_1.py:218-228): [0,1], then chunks of `step`."""
+    out, start, end = [(0, 1)], 1, 1
+    while start < t:
+        end = min(t, end + step)
+        out.append((start, end))
+        start = end
+    return out
+
+
+def chunk_noise(B: int, channels: int, tzs: Sequence[int], Hz: int, Wz: int,
+                generator: Optional[torch.Generator] = None) -> torch.Tensor:
+    """KL noise of consecutive chunks of tzs latent frames: one CPU torch.randn per chunk, in chunk order, concatenated
+    along time -- the draws tile_encode makes, as the reference samples each chunk (distributions.py:17)."""
+    draws = [torch.randn((B, channels, tz, Hz, Wz), generator=generator) for tz in tzs]
+    return draws[0] if len(draws) == 1 else torch.cat(draws, dim=2)
+
+
 # --------------------------------------------------------------------------------------------------
 # native handle
 # --------------------------------------------------------------------------------------------------
@@ -270,6 +288,7 @@ class ChunkState:
         N.check(native.lib.vt_chunk_state_create(native.handle, precision, B, H, W, int(is_decoder), int(use_overlap),
                                                  C.byref(self.handle)))
         native._chunk_handles[id(self)] = self.handle
+        self.B, self.H, self.W = B, H, W
 
     def close(self):
         self.native._chunk_handles.pop(id(self), None)
@@ -283,12 +302,68 @@ class ChunkState:
         except Exception:
             pass
 
-    def workspace(self, Tc: int) -> torch.Tensor:
-        return self.native._workspace(int(self.native.lib.vt_chunk_workspace_bytes(self.handle, Tc)))
+    def workspace(self, Tc: int, fsq_aux: bool = False) -> torch.Tensor:
+        """workspace of a chunk of Tc frames (fsq_aux: of vt_encode_chunk_fsq_aux)"""
+        lib = self.native.lib
+        query = lib.vt_chunk_fsq_aux_workspace_bytes if fsq_aux else lib.vt_chunk_workspace_bytes
+        return self.native._workspace(int(query(self.handle, Tc)))
 
-    def aux_workspace(self, Tc: int) -> torch.Tensor:
-        """workspace of vt_encode_chunk_fsq_aux for a chunk of Tc frames"""
-        return self.native._workspace(int(self.native.lib.vt_chunk_fsq_aux_workspace_bytes(self.handle, Tc)))
+    def encode_buffers(self, n: int, want_h: bool = False, fsq_aux: bool = False,
+                       given: Optional[Dict[str, Optional[torch.Tensor]]] = None) -> Dict[str, Optional[torch.Tensor]]:
+        """The outputs and workspace of one encoder chunk of n frames, those in `given` kept: z, idx (FSQ), kl (KL),
+        h (want_h: the pre-bound latent) and ws, the workspace of the entry point encode() calls."""
+        s, dev = self.native.spec, self.native.device
+        tz, Hz, Wz = self.native.latent_shape(n, self.H, self.W)
+        make = {
+            "z": lambda: torch.empty((self.B, s.z_channels, tz, Hz, Wz), dtype=torch.float32, device=dev),
+            "idx": lambda: torch.empty((self.B, tz, Hz, Wz), dtype=torch.int32, device=dev) if s.regularizer == "fsq" else None,
+            "kl": lambda: torch.empty((1,), dtype=torch.float32, device=dev) if s.regularizer == "kl" else None,
+            "h": lambda: (torch.empty((self.B, (2 if s.double_z else 1) * s.z_channels, tz, Hz, Wz), dtype=torch.float32,
+                                      device=dev) if want_h else None),
+            "ws": lambda: self.workspace(n, fsq_aux),
+        }
+        given = given or {}
+        return {k: given[k] if k in given else f() for k, f in make.items()}
+
+    def encode(self, x: torch.Tensor, first: bool, noise: Optional[torch.Tensor] = None, want_h: bool = False,
+               aux: Optional[Tuple[torch.Tensor, torch.Tensor]] = None,
+               out: Optional[Dict[str, Optional[torch.Tensor]]] = None) -> Dict[str, Optional[torch.Tensor]]:
+        """One encoder chunk of x [B,C,n,H,W] (dense fp32): vt_encode_chunk_pre with want_h, vt_encode_chunk_fsq_aux with
+        aux (the caller's stats [1,2] / avg [1,J] buffers of the chunk's FSQ aux partials), else vt_encode_chunk.  out: the
+        caller's buffers, as encode_buffers names them (the graph path passes all of its static ones); the others are
+        new.  Returns the buffers."""
+        n, lib, s = x.shape[2], self.native.lib, self.native.spec
+        b = self.encode_buffers(n, want_h, aux is not None, out)
+        ws, stream = b["ws"], _stream_ptr(self.native.device)
+        if want_h:
+            N.check(lib.vt_encode_chunk_pre(self.handle, int(first), _ptr(x), s.in_channels, n, _ptr(noise), _ptr(b["z"]),
+                                            _ptr(b["idx"]), _ptr(b["kl"]), _ptr(b["h"]), _ptr(ws), ws.numel(), stream))
+        elif aux is not None:
+            N.check(lib.vt_encode_chunk_fsq_aux(self.handle, int(first), _ptr(x), s.in_channels, n, _ptr(b["z"]), _ptr(b["idx"]),
+                                                100.0, _ptr(aux[0]), _ptr(aux[1]), _ptr(ws), ws.numel(), stream))
+        else:
+            N.check(lib.vt_encode_chunk(self.handle, int(first), _ptr(x), s.in_channels, n, _ptr(noise), _ptr(b["z"]),
+                                        _ptr(b["idx"]), _ptr(b["kl"]), _ptr(ws), ws.numel(), stream))
+        return b
+
+    def decode_buffers(self, n: int, first: bool) -> Dict[str, torch.Tensor]:
+        """The output (every frame the chunk decodes) and workspace of one decoder chunk of n latent frames.  v1.0 drops
+        tdf-1 frames of a video's first chunk only; v1.1 decodes every chunk as a video of its own."""
+        s, nat = self.native.spec, self.native
+        To = nat.decoded_frames(n) if (first or s.version == 1) else n * s.time_downsample_factor
+        f = nat.spatial_factor()
+        return {"out": torch.empty((self.B, s.out_ch, To, self.H * f, self.W * f), dtype=torch.float32, device=nat.device),
+                "ws": self.workspace(n)}
+
+    def decode(self, z: torch.Tensor, first: bool, out: Optional[Dict[str, torch.Tensor]] = None) -> torch.Tensor:
+        """One decoder chunk of z [B,Cz,n,Hz,Wz] (dense fp32, the look-ahead frame included): vt_decode_chunk into
+        out["out"] with workspace out["ws"] (the graph path's static buffers), or new ones.  Returns the decoded frames."""
+        n, nat = z.shape[2], self.native
+        b = self.decode_buffers(n, first) if out is None else out
+        ws = b["ws"]
+        N.check(nat.lib.vt_decode_chunk(self.handle, int(first), _ptr(z), nat.spec.z_channels, n, _ptr(b["out"]), _ptr(ws),
+                                        ws.numel(), _stream_ptr(nat.device)))
+        return b["out"]
 
     def copy_slots(self, src: "ChunkState", dst_slots: Sequence[int], src_slots: Sequence[int]):
         """vt_chunk_state_copy_slots: slot dst_slots[i] of this state becomes the state slot src_slots[i] of src would
@@ -895,15 +970,8 @@ class AutoencodingEngineV11(_EngineBase):
         self.use_overlap = False
 
     def build_chunk_start_end(self, t, decoder_mode=False):
-        """autoencoder_v1_1.py:218-228"""
-        start_end = [[0, 1]]
-        start = end = 1
-        step = self.t_chunk_dec if decoder_mode else self.t_chunk_enc
-        while start < t:
-            end = min(t, end + step)
-            start_end.append([start, end])
-            start = end
-        return start_end
+        """autoencoder_v1_1.py:218-228: a list of [start, end] lists"""
+        return [list(c) for c in chunk_start_end(t, self.t_chunk_dec if decoder_mode else self.t_chunk_enc)]
 
     def encode(self, x: Any, return_reg_log: bool = False, *, noise: Optional[torch.Tensor] = None) -> Any:
         """noise: as AutoencodingEngine.encode (untiled calls only)."""
@@ -944,8 +1012,7 @@ class AutoencodingEngineV11(_EngineBase):
         Tz = sum(sh[0] for sh in shapes)
         noise = None
         if self.spec.regularizer == "kl" and self.spec.kl_sample:
-            # one torch.randn per chunk, in chunk order, exactly the draws the reference makes (distributions.py:17)
-            noise = torch.cat([torch.randn((B, self.spec.z_channels, sh[0], Hz, Wz)) for sh in shapes], dim=2).to(dev)
+            noise = chunk_noise(B, self.spec.z_channels, [sh[0] for sh in shapes], Hz, Wz).to(dev)
         z = torch.empty((B, self.spec.z_channels, Tz, Hz, Wz), dtype=torch.float32, device=dev)
         idx = torch.empty((B, Tz, Hz, Wz), dtype=torch.int32, device=dev) if self.spec.regularizer == "fsq" else None
         kl = torch.empty((), dtype=torch.float32, device=dev) if self.spec.regularizer == "kl" else None

@@ -42,7 +42,8 @@ from typing import List, Optional, Tuple
 import torch
 
 from . import _native as N
-from .streaming import DecodeStream, EncodeStream
+from .engine import chunk_noise, chunk_start_end
+from .streaming import DecodeStream, EncodeStream, _loss_terms, _mean
 
 
 def temporal_reach(native, is_decoder: bool, use_overlap: bool = False) -> int:
@@ -50,16 +51,6 @@ def temporal_reach(native, is_decoder: bool, use_overlap: bool = False) -> int:
     r = C.c_int32()
     N.check(native.lib.vt_temporal_reach(native.handle, int(is_decoder), int(use_overlap), C.byref(r)))
     return r.value
-
-
-def chunk_start_end(t: int, step: int) -> List[Tuple[int, int]]:
-    """build_chunk_start_end (autoencoder_v1_1.py:218-228): [0,1], then chunks of `step`."""
-    out, start, end = [(0, 1)], 1, 1
-    while start < t:
-        end = min(t, end + step)
-        out.append((start, end))
-        start = end
-    return out
 
 
 @dataclass
@@ -191,8 +182,7 @@ def encode_sharded(model, x: torch.Tensor, shards: int):
     Tz = lat0[-1]
     kl_noise = s.regularizer == "kl" and s.kl_sample
     if kl_noise:
-        # one torch.randn per global chunk, in chunk order, as tile_encode draws them
-        draws = torch.cat([torch.randn((1, s.z_channels, t, Hz, Wz)) for t in tz], dim=2)
+        draws = chunk_noise(1, s.z_channels, tz, Hz, Wz)   # every global chunk's, as tile_encode draws them
     row = [(a, e, nat.latent_shape(e - a, H, W)[0]) for a, e in chunk_start_end(plan.window, c)]   # a window's chunks
     zlen = sum(t for _, _, t in row)
     row0 = [p // tdf for p in starts]                          # global latent frame of each window's first latent
@@ -229,7 +219,6 @@ def encode_sharded(model, x: torch.Tensor, shards: int):
     kls = torch.zeros((G,), dtype=torch.float32, device=dev)
     stats = torch.zeros((G, 2), dtype=torch.float32, device=dev) if aux else None
     avg = torch.zeros((G, reg.codebook_size), dtype=torch.float32, device=dev) if aux else None
-    lib, sp = nat.lib, torch.cuda.current_stream(dev).cuda_stream
     for i, (a, b) in enumerate(owned):
         r0, r1 = lat0[a] - row0[i], lat0[b] - row0[i]
         out[0, :, lat0[a]:lat0[b]] = zr[i, :, r0:r1]
@@ -238,11 +227,9 @@ def encode_sharded(model, x: torch.Tensor, shards: int):
         for g in range(a, b):   # each owned chunk's loss terms, from its own pre-bound latent
             h = hr[i:i + 1, :, lat0[g] - row0[i]:lat0[g + 1] - row0[i]].contiguous()
             if s.regularizer == "kl":
-                zscr = torch.empty((1, s.z_channels, tz[g], Hz, Wz), dtype=torch.float32, device=dev)
-                N.check(lib.vt_op_kl(C.c_void_p(h.data_ptr()), None, s.z_channels, tz[g] * Hz * Wz, 1, 0,
-                                     C.c_void_p(zscr.data_ptr()), C.c_void_p(kls[g:g + 1].data_ptr()), C.c_void_p(sp)))
+                _loss_terms(nat, reg, h, kls[g:g + 1])
             elif aux:
-                st, av = reg.aux_partials(h)
+                st, av = _loss_terms(nat, reg, h)
                 stats[g], avg[g] = st[0], av[0]
     if world > 1:
         import torch.distributed as dist
@@ -253,7 +240,7 @@ def encode_sharded(model, x: torch.Tensor, shards: int):
         total = torch.zeros((), dtype=torch.float32, device=dev)
         for g in range(G):
             total = total + kls[g]   # in chunk order, as tile_encode's mean sums them
-        return out, {"kl_loss": total / torch.full((), float(G), dtype=torch.float32, device=dev)}
+        return out, {"kl_loss": _mean(total, G)}
     aux_loss = (reg.aux_finalize(stats, avg, n_steps=model.global_step // 2, world_size=1) if aux
                 else torch.zeros((), device=dev))
     return out, {"aux_loss": aux_loss, "indices": idx}

@@ -80,7 +80,7 @@ from typing import Dict, List, Optional, Tuple
 import torch
 
 from . import _native as N
-from .engine import ChunkState, _ptr, _refuse_capture, _stream_ptr
+from .engine import ChunkState, _ptr, _refuse_capture, _stream_ptr, chunk_noise
 
 
 def encode_chunks(avail: int, first: bool, tdf: int, version: int) -> List[int]:
@@ -152,7 +152,8 @@ class ChunkGraphs:
     """The CUDA graphs of one stream's steady chunks.  A key that occurs for the first time runs eagerly (lengths seen once
     never pay for a capture); its second occurrence is captured, after vt_chunk_state_reserve, and runs as the graph's
     first replay; every later occurrence replays.  Each graph owns static input / output buffers: a push copies its chunk in
-    and its results out, so the tensors it returns are fresh."""
+    and its results out, so the tensors it returns are fresh.  The workspace is one of them, sized eagerly before the
+    capture and held there: the graph keeps reading it if the model's workspace grows."""
 
     def __init__(self):
         self.seen: Dict[Tuple, int] = {}
@@ -176,7 +177,6 @@ class ChunkGraphs:
         lib = state.native.lib
         if action == "capture":
             N.check(lib.vt_chunk_state_reserve(state.handle, key[0], _stream_ptr(state.native.device)))
-            bufs["ws"] = bufs["ws_fn"]()      # sized eagerly, and held here: the graph keeps reading it if the model's grows
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
                 launch(bufs)                   # capturing flips the caches' parity, as running the chunk does
@@ -193,14 +193,18 @@ class ChunkGraphs:
         return bufs
 
 
+def _check_t_chunk(tdf: int, t_chunk: int, is_decoder: bool):
+    if int(t_chunk) < 1 or (not is_decoder and int(t_chunk) % tdf != 0):
+        raise ValueError(f"t_chunk must be a positive multiple of time_downsample_factor ({tdf}), got {t_chunk}"
+                         if not is_decoder else f"t_chunk must be a positive number of latent frames, got {t_chunk}")
+
+
 def check_recipe(version: int, tdf: int, t_chunk: Optional[int], use_overlap: bool, is_decoder: bool):
     """The stream options build_chunk_start_end and the overlap rule accept (ValueError otherwise)."""
     if t_chunk is not None:
         if version != 1:
             raise ValueError("t_chunk needs a v1.1 model: v1.0 streams equal the whole clip for any chunking")
-        if int(t_chunk) < 1 or (not is_decoder and int(t_chunk) % tdf != 0):
-            raise ValueError(f"t_chunk must be a positive multiple of time_downsample_factor ({tdf}), got {t_chunk}"
-                             if not is_decoder else f"t_chunk must be a positive number of latent frames, got {t_chunk}")
+        _check_t_chunk(tdf, t_chunk, is_decoder)
     if use_overlap:
         if t_chunk is None or version != 1:
             raise ValueError("use_overlap needs a v1.1 model and t_chunk (the look-ahead follows the tile_decode chunks)")
@@ -208,13 +212,25 @@ def check_recipe(version: int, tdf: int, t_chunk: Optional[int], use_overlap: bo
             raise ValueError("use_overlap supports 2x, 4x or 8x temporal downsampling only")
 
 
-class _Stream:
-    def __init__(self, model, batch: int, H: int, W: int, is_decoder: bool, t_chunk: Optional[int] = None,
-                 use_overlap: bool = False):
+def check_pool_recipe(version: int, tdf: int, t_chunk: Optional[int], use_overlap: bool, is_decoder: bool):
+    """The options a pool accepts (ValueError otherwise): every pool has a chunk length, t_chunk frames (encoder, a
+    multiple of tdf) or latent frames (decoder); v1.1 pools follow the stream recipe's rules."""
+    if t_chunk is None:
+        raise ValueError("a pool needs t_chunk: the batched chunks of all its slots have one length")
+    # a v1.0 pool's chunks are valid v1.0 stream chunks, which need no t_chunk
+    check_recipe(version, tdf, t_chunk if version == 1 else None, use_overlap, is_decoder)
+    _check_t_chunk(tdf, t_chunk, is_decoder)
+
+
+class _Chunked:
+    """The set-up and input checks of streams and pools: the options are checked before the model is loaded, and the
+    precision is fixed at creation, as encode reads it."""
+
+    def __init__(self, model, H: int, W: int, is_decoder: bool, t_chunk: Optional[int], use_overlap: bool, check):
         if not model.is_causal:
             raise ValueError("non-causal models cannot stream: their time padding is symmetric, so a frame depends on later frames")
         self.tdf = int(model.spec.time_downsample_factor)
-        check_recipe(model.spec.version, self.tdf, t_chunk, use_overlap, is_decoder)
+        check(model.spec.version, self.tdf, t_chunk, use_overlap, is_decoder)
         self.t_chunk = None if t_chunk is None else int(t_chunk)
         self.use_overlap = bool(use_overlap)
         rt = model._rt
@@ -223,7 +239,109 @@ class _Stream:
         self.spec = model.spec
         self.precision = rt.precision()
         self.out_dtype = rt.out_dtype()
-        self.B, self.H, self.W = int(batch), int(H), int(W)
+        self.H, self.W = int(H), int(W)
+
+    def _frames(self, x: torch.Tensor, B: int) -> torch.Tensor:
+        """x checked as frames [B,C,t,H,W], in fp32"""
+        if not x.is_cuda:
+            raise RuntimeError("vidtok_b200: inputs must be CUDA tensors; there is no CPU path")
+        if x.dim() != 5 or tuple(x.shape[:2]) != (B, self.spec.in_channels) or tuple(x.shape[3:]) != (self.H, self.W):
+            raise ValueError(f"expected [{B},{self.spec.in_channels},t,{self.H},{self.W}] frames, got {tuple(x.shape)}")
+        return x.detach().to(torch.float32)
+
+    def _latents(self, z: torch.Tensor, B: int) -> torch.Tensor:
+        """z checked as latents [B,z_channels,tz,Hz,Wz] or FSQ token indices [B,tz,Hz,Wz], as an fp32 latent"""
+        if not z.is_cuda:
+            raise RuntimeError("vidtok_b200: inputs must be CUDA tensors; there is no CPU path")
+        s = self.spec
+        if z.dim() == 4 and not z.is_floating_point():
+            if s.regularizer != "fsq":
+                raise ValueError("token indices need an FSQ model")
+            z = self.model.indices_to_latent(z)
+        if z.dim() != 5 or tuple(z.shape[:2]) != (B, s.z_channels) or tuple(z.shape[3:]) != (self.H, self.W):
+            raise ValueError(f"expected a [{B},{s.z_channels},tz,{self.H},{self.W}] latent, got {tuple(z.shape)}")
+        return z.detach().to(torch.float32)
+
+
+def _mean(total: torch.Tensor, n: int) -> torch.Tensor:
+    """total / n rounded once, as the library's per-chunk means divide (a Python divisor would be applied as a
+    multiplication by its reciprocal)"""
+    return total / torch.full((), float(n), dtype=torch.float32, device=total.device)
+
+
+class _Losses:
+    """One video's running losses over its chunks, as tile_encode (v1.1) or the whole clip (v1.0) forms them.  KL: the
+    chunks' values summed in chunk order, reported as their mean (v1.1) or their sum (v1.0).  FSQ aux: v1.1 the mean over
+    the chunks of each chunk's aux; v1.0 all of the video's tokens as one segment, from token-weighted fp64 sums of the
+    chunks' partials, finalized when reported."""
+
+    def __init__(self, model, device: torch.device, aux: bool):
+        self.model = model
+        self.n_chunks = 0
+        self.kl_sum = torch.zeros((), dtype=torch.float32, device=device)
+        self._aux = torch.zeros((), dtype=torch.float32, device=device)
+        self._unreported = False   # v1.0: partials folded since _aux was finalized
+        if aux:
+            self.aux_sum = torch.zeros((), dtype=torch.float32, device=device)
+            self.tok_stats = torch.zeros((2,), dtype=torch.float64, device=device)
+            self.tok_avg = torch.zeros((model.regularization.codebook_size,), dtype=torch.float64, device=device)
+            self.tokens = 0
+
+    def add(self, kl: Optional[torch.Tensor] = None, partials: Optional[Tuple[torch.Tensor, torch.Tensor]] = None,
+            tokens: int = 0):
+        """One chunk: its KL value, or its FSQ aux partials (stats [1,2], avg [1,J]) over `tokens` tokens."""
+        self.n_chunks += 1
+        if kl is not None:
+            self.kl_sum = self.kl_sum + kl
+        if partials is None:
+            return
+        stats, avg = partials
+        if self.model.spec.version == 0:
+            self.tok_stats += tokens * stats[0].double()
+            self.tok_avg += tokens * avg[0].double()
+            self.tokens += tokens
+            self._unreported = True
+        else:
+            self.aux_sum = self.aux_sum + self._finalize(stats, avg)
+            self._aux = _mean(self.aux_sum, self.n_chunks)
+
+    def kl_loss(self) -> torch.Tensor:
+        if self.model.spec.version == 0:
+            return self.kl_sum
+        if not self.n_chunks:
+            return torch.zeros((), dtype=torch.float32, device=self.kl_sum.device)
+        return _mean(self.kl_sum, self.n_chunks)
+
+    def aux_loss(self) -> torch.Tensor:
+        if self._unreported:
+            self._aux = self._finalize((self.tok_stats / self.tokens).float().view(1, 2),
+                                       (self.tok_avg / self.tokens).float().view(1, -1))
+            self._unreported = False
+        return self._aux
+
+    def _finalize(self, stats: torch.Tensor, avg: torch.Tensor) -> torch.Tensor:
+        return self.model.regularization.aux_finalize(stats, avg, n_steps=self.model.global_step // 2, world_size=1)
+
+
+def _loss_terms(native, reg, h: torch.Tensor, kl: Optional[torch.Tensor] = None):
+    """One chunk's loss terms from its own pre-bound latent h [1,2z|z,tz,Hz,Wz] (dense), apart from the batch it ran in: a
+    KL model's KL value (vt_op_kl into a scratch z; written to `kl`, else to a new scalar), an FSQ model's aux partials
+    (stats, avg)."""
+    s, dev = native.spec, native.device
+    if s.regularizer != "kl":
+        return reg.aux_partials(h)
+    zs = torch.empty((1, s.z_channels) + tuple(h.shape[2:]), dtype=torch.float32, device=dev)
+    kl = torch.empty((), dtype=torch.float32, device=dev) if kl is None else kl
+    N.check(native.lib.vt_op_kl(_ptr(h), None, s.z_channels, h.shape[2] * h.shape[3] * h.shape[4], 1, 0, _ptr(zs), _ptr(kl),
+                                _stream_ptr(dev)))
+    return kl
+
+
+class _Stream(_Chunked):
+    def __init__(self, model, batch: int, H: int, W: int, is_decoder: bool, t_chunk: Optional[int] = None,
+                 use_overlap: bool = False):
+        super().__init__(model, H, W, is_decoder, t_chunk, use_overlap, check_recipe)
+        self.B = int(batch)
         self.state = ChunkState(self.native, self.precision, self.B, self.H, self.W, is_decoder, self.use_overlap)
         self.first = True
         self.finished = False
@@ -241,9 +359,6 @@ class _Stream:
     def _graph_action(self, n: int, final: bool, entry: str) -> Tuple[Optional[Tuple], str]:
         key = chunk_graph_key(n, self.first, final, entry, self.native.lib.vt_chunk_state_parity(self.state.handle))
         return key, self.graphs.action(key)
-
-    def _workspace(self, n: int) -> torch.Tensor:
-        return self.state.workspace(n)
 
     def _check_open(self):
         if self.finished:
@@ -263,36 +378,22 @@ class EncodeStream(_Stream):
         self.reg = model.regularization
         self.aux = self.spec.regularizer == "fsq" and self.reg.aux_enabled() and not self.keep_pre
         if self.aux:
+            # one chunk's partials, at fixed addresses: a captured graph writes them there
             dev, J = self.native.device, self.reg.codebook_size
-            self.aux_stats = torch.empty((1, 2), dtype=torch.float32, device=dev)   # one chunk's partials
+            self.aux_stats = torch.empty((1, 2), dtype=torch.float32, device=dev)
             self.aux_avg = torch.empty((1, J), dtype=torch.float32, device=dev)
-        self._reset_losses()
-
-    def _reset_losses(self):
-        dev = self.native.device
-        self.n_chunks = 0
-        self.kl_sum = torch.zeros((), dtype=torch.float32, device=dev)
-        self.aux_loss = torch.zeros((), dtype=torch.float32, device=dev)
-        if self.aux:
-            self.aux_sum = torch.zeros((), dtype=torch.float32, device=dev)        # v1.1: running sum of per-chunk aux
-            self.tok_stats = torch.zeros((2,), dtype=torch.float64, device=dev)    # v1.0: token-weighted partials
-            self.tok_avg = torch.zeros((self.reg.codebook_size,), dtype=torch.float64, device=dev)
-            self.tokens = 0
+        self.losses = _Losses(model, self.native.device, self.aux)
 
     def reset(self):
         super().reset()
         self.pending = None
-        self._reset_losses()
+        self.losses = _Losses(self.model, self.native.device, self.aux)
 
     def push(self, x: torch.Tensor, noise: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, Dict[str, torch.Tensor]]:
         """x: frames [B,C,t,H,W], any t.  Returns the latent frames of the chunks this push completed (possibly none) and
         reg_log; noise (KL with sampling, optional): [B,z_channels,tz,Hz,Wz] for those latent frames."""
         self._check_open()
-        if not x.is_cuda:
-            raise RuntimeError("vidtok_b200: inputs must be CUDA tensors; there is no CPU path")
-        if x.dim() != 5 or tuple(x.shape[:2]) != (self.B, self.spec.in_channels) or tuple(x.shape[3:]) != (self.H, self.W):
-            raise ValueError(f"expected [{self.B},{self.spec.in_channels},t,{self.H},{self.W}] frames, got {tuple(x.shape)}")
-        x = x.detach().to(torch.float32)
+        x = self._frames(x, self.B)
         frames = x if self.pending is None else torch.cat([self.pending, x], dim=2)
         if self.t_chunk is None:
             chunks = encode_chunks(frames.shape[2], self.first, self.tdf, self.spec.version)
@@ -320,9 +421,8 @@ class EncodeStream(_Stream):
         if kl_noise:
             shape = (self.B, s.z_channels, Tz, self.Hz, self.Wz)
             if noise is None:
-                # CPU generator, as distributions.py:17: one draw per push, or per chunk in chunk order as tile_encode
-                noise = (torch.randn(shape) if self.t_chunk is None or not tzs else
-                         torch.cat([torch.randn((self.B, s.z_channels, tz, self.Hz, self.Wz)) for tz in tzs], dim=2))
+                # one draw per push, or per chunk as tile_encode draws them
+                noise = chunk_noise(self.B, s.z_channels, tzs if self.t_chunk is not None and tzs else [Tz], self.Hz, self.Wz)
             elif tuple(noise.shape) != shape:
                 raise ValueError(f"noise must have shape {shape} (this push's latent frames), got {tuple(noise.shape)}")
             noise = noise.to(device=dev, dtype=torch.float32).contiguous()
@@ -331,129 +431,55 @@ class EncodeStream(_Stream):
         kls = torch.zeros((max(len(chunks), 1),), dtype=torch.float32, device=dev)
         hC = (2 if s.double_z else 1) * s.z_channels
         h = torch.empty((self.B, hC, Tz, self.Hz, self.Wz), dtype=torch.float32, device=dev) if self.keep_pre else None
-        t0 = tz0 = 0
+        aux = (self.aux_stats, self.aux_avg) if self.aux else None
         entry = "pre" if self.keep_pre else ("fsq_aux" if self.aux else "plain")
+        t0 = tz0 = 0
         for i, (n, tz) in enumerate(zip(chunks, tzs)):
+            xc, nc = frames[:, :, t0:t0 + n], noise[:, :, tz0:tz0 + tz] if kl_noise else None
+            kl = kls[i:i + 1] if s.regularizer == "kl" else None
             key, action = self._graph_action(n, final, entry)
-            if action != "eager":
-                g = self._graph_chunk(key, action, n, tz, hC)
-                g["x"].copy_(frames[:, :, t0:t0 + n])
-                if kl_noise:
-                    g["noise"].copy_(noise[:, :, tz0:tz0 + tz])
-                g = self.graphs.run(key, action, self.state, self._launch_encode, g)
-                zc, ic = g["z"], g["idx"]
-                if s.regularizer == "kl":
-                    kls[i:i + 1].copy_(g["kl"])
-                if self.keep_pre:
-                    h[:, :, tz0:tz0 + tz] = g["h"]
-                if self.aux:
-                    self._add_aux_chunk(self.B * tz * self.Hz * self.Wz)
+            if action == "eager":
+                b = self.state.encode(xc.contiguous(), self.first, None if nc is None else nc.contiguous(), self.keep_pre, aux,
+                                      out={"kl": kl})
             else:
-                zc, ic = self._eager_chunk(frames, noise, kls, h, i, n, tz, t0, tz0, hC, kl_noise, idx is not None)
-            z[:, :, tz0:tz0 + tz] = zc
+                g = self.graphs.graphs[key] if action == "replay" else self._graph_buffers(n, tz, kl_noise)
+                g["x"].copy_(xc)
+                if kl_noise:
+                    g["noise"].copy_(nc)
+                b = self.graphs.run(key, action, self.state, self._launch_encode, g)
+                if kl is not None:
+                    kl.copy_(b["kl"])
+            z[:, :, tz0:tz0 + tz] = b["z"]
             if idx is not None:
-                idx[:, tz0:tz0 + tz] = ic
-            if self.t_chunk is not None and s.regularizer == "kl":
-                self.kl_sum = self.kl_sum + kls[i]   # in chunk order, as tile_encode's mean sums them
+                idx[:, tz0:tz0 + tz] = b["idx"]
+            if self.keep_pre:
+                h[:, :, tz0:tz0 + tz] = b["h"]
+            # KL in chunk order for tile_encode's mean; without t_chunk a push reports its own share
+            self.losses.add(kl=kls[i] if self.t_chunk is not None and kl is not None else None, partials=aux,
+                            tokens=self.B * tz * self.Hz * self.Wz)
             self.first = False
-            self.n_chunks += 1
             t0 += n
             tz0 += tz
-        return self._finish_push(frames, chunks, idx, kls, h, z, t0, dev)
-
-    def _graph_chunk(self, key: Tuple, action: str, n: int, tz: int, hC: int) -> Dict:
-        """The static buffers of key's graph (new ones for a capture)."""
-        if action == "replay":
-            return self.graphs.graphs[key]
-        s, dev = self.spec, self.native.device
-        lat = (self.B, s.z_channels, tz, self.Hz, self.Wz)
-        kl_noise = s.regularizer == "kl" and s.kl_sample
-        return {
-            "n": n,
-            "x": torch.empty((self.B, s.in_channels, n, self.H, self.W), dtype=torch.float32, device=dev),
-            "noise": torch.empty(lat, dtype=torch.float32, device=dev) if kl_noise else None,
-            "z": torch.empty(lat, dtype=torch.float32, device=dev),
-            "idx": torch.empty((self.B, tz, self.Hz, self.Wz), dtype=torch.int32, device=dev) if s.regularizer == "fsq" else None,
-            "kl": torch.zeros((1,), dtype=torch.float32, device=dev) if s.regularizer == "kl" else None,
-            "h": torch.empty((self.B, hC, tz, self.Hz, self.Wz), dtype=torch.float32, device=dev) if self.keep_pre else None,
-            "ws_fn": (lambda: self.state.aux_workspace(n)) if self.aux else (lambda: self._workspace(n)),
-        }
-
-    def _launch_encode(self, g: Dict):
-        """The chunk's native call on a graph's static buffers (a later chunk: is_first 0)."""
-        s, lib, ws, n = self.spec, self.native.lib, g["ws"], g["n"]
-        stream = _stream_ptr(self.native.device)
-        if self.keep_pre:
-            N.check(lib.vt_encode_chunk_pre(self.state.handle, 0, _ptr(g["x"]), s.in_channels, n, _ptr(g["noise"]), _ptr(g["z"]),
-                                            _ptr(g["idx"]), _ptr(g["kl"]), _ptr(g["h"]), _ptr(ws), ws.numel(), stream))
-        elif self.aux:
-            N.check(lib.vt_encode_chunk_fsq_aux(self.state.handle, 0, _ptr(g["x"]), s.in_channels, n, _ptr(g["z"]), _ptr(g["idx"]),
-                                                100.0, _ptr(self.aux_stats), _ptr(self.aux_avg), _ptr(ws), ws.numel(), stream))
-        else:
-            N.check(lib.vt_encode_chunk(self.state.handle, 0, _ptr(g["x"]), s.in_channels, n, _ptr(g["noise"]), _ptr(g["z"]),
-                                        _ptr(g["idx"]), _ptr(g["kl"]), _ptr(ws), ws.numel(), stream))
-
-    def _eager_chunk(self, frames, noise, kls, h, i, n, tz, t0, tz0, hC, kl_noise, want_idx):
-        s, dev = self.spec, frames.device
-        lib, stream = self.native.lib, _stream_ptr(dev)
-        xc = frames[:, :, t0:t0 + n].contiguous()
-        zc = torch.empty((self.B, s.z_channels, tz, self.Hz, self.Wz), dtype=torch.float32, device=dev)
-        ic = torch.empty((self.B, tz, self.Hz, self.Wz), dtype=torch.int32, device=dev) if want_idx else None
-        nc = noise[:, :, tz0:tz0 + tz].contiguous() if kl_noise else None
-        if self.keep_pre:
-            ws = self._workspace(n)
-            hc = torch.empty((self.B, hC, tz, self.Hz, self.Wz), dtype=torch.float32, device=dev)
-            N.check(lib.vt_encode_chunk_pre(self.state.handle, int(self.first), _ptr(xc), s.in_channels, n, _ptr(nc), _ptr(zc),
-                                            _ptr(ic), _ptr(kls[i:i + 1]) if s.regularizer == "kl" else None, _ptr(hc), _ptr(ws),
-                                            ws.numel(), stream))
-            h[:, :, tz0:tz0 + tz] = hc
-        elif self.aux:
-            ws = self.state.aux_workspace(n)
-            N.check(lib.vt_encode_chunk_fsq_aux(self.state.handle, int(self.first), _ptr(xc), s.in_channels, n, _ptr(zc), _ptr(ic),
-                                                100.0, _ptr(self.aux_stats), _ptr(self.aux_avg), _ptr(ws), ws.numel(), stream))
-            self._add_aux_chunk(self.B * tz * self.Hz * self.Wz)
-        else:
-            ws = self._workspace(n)
-            N.check(lib.vt_encode_chunk(self.state.handle, int(self.first), _ptr(xc), s.in_channels, n, _ptr(nc), _ptr(zc),
-                                        _ptr(ic), _ptr(kls[i:i + 1]) if s.regularizer == "kl" else None, _ptr(ws), ws.numel(),
-                                        stream))
-        return zc, ic
-
-    def _finish_push(self, frames, chunks, idx, kls, h, z, t0, dev):
-        s = self.spec
         self.pending = frames[:, :, t0:].clone() if t0 < frames.shape[2] else None
         if s.regularizer == "fsq":
-            if self.aux and chunks and s.version == 0:
-                self.aux_loss = self.reg.aux_finalize((self.tok_stats / self.tokens).float().view(1, 2),
-                                                      (self.tok_avg / self.tokens).float().view(1, -1),
-                                                      n_steps=self.model.global_step // 2, world_size=1)
-            log = {"indices": idx, "aux_loss": self.aux_loss}
+            log = {"indices": idx, "aux_loss": self.losses.aux_loss()}
         else:
-            if self.t_chunk is None:
-                kl = kls.sum()
-            else:
-                kl = self._mean(self.kl_sum, self.n_chunks) if self.n_chunks else torch.zeros((), dtype=torch.float32, device=dev)
-            log = {"kl_loss": kl}
+            log = {"kl_loss": kls.sum() if self.t_chunk is None else self.losses.kl_loss()}
         if self.keep_pre:
             log["h_pre"] = h
         return z.to(self.out_dtype), log
 
-    @staticmethod
-    def _mean(total: torch.Tensor, n: int) -> torch.Tensor:
-        """total / n rounded once, as the library's per-chunk means divide (a Python divisor would be applied as a
-        multiplication by its reciprocal)"""
-        return total / torch.full((), float(n), dtype=torch.float32, device=total.device)
+    def _graph_buffers(self, n: int, tz: int, kl_noise: bool) -> Dict:
+        """New static buffers of a chunk graph: the chunk's frames and noise, and encode_buffers."""
+        s, dev = self.spec, self.native.device
+        g = self.state.encode_buffers(n, self.keep_pre, self.aux)
+        g["x"] = torch.empty((self.B, s.in_channels, n, self.H, self.W), dtype=torch.float32, device=dev)
+        g["noise"] = torch.empty((self.B, s.z_channels, tz, self.Hz, self.Wz), dtype=torch.float32, device=dev) if kl_noise else None
+        return g
 
-    def _add_aux_chunk(self, tokens: int):
-        """Fold the partials one chunk just wrote into the stream's running aux state."""
-        if self.spec.version == 0:
-            self.tok_stats += tokens * self.aux_stats[0].double()
-            self.tok_avg += tokens * self.aux_avg[0].double()
-            self.tokens += tokens
-        else:
-            aux = self.reg.aux_finalize(self.aux_stats, self.aux_avg, n_steps=self.model.global_step // 2, world_size=1)
-            self.aux_sum = self.aux_sum + aux
-            self.aux_loss = self._mean(self.aux_sum, self.n_chunks + 1)
+    def _launch_encode(self, g: Dict):
+        """The chunk's native call on a graph's static buffers (a later chunk: is_first 0)."""
+        self.state.encode(g["x"], False, g["noise"], self.keep_pre, (self.aux_stats, self.aux_avg) if self.aux else None, out=g)
 
 
 class DecodeStream(_Stream):
@@ -473,16 +499,7 @@ class DecodeStream(_Stream):
         """z: latents [B,z_channels,tz,Hz,Wz], or FSQ token indices [B,tz,Hz,Wz] (integer tensor).  Returns the decoded
         frames that are final (with t_chunk possibly none)."""
         self._check_open()
-        if not z.is_cuda:
-            raise RuntimeError("vidtok_b200: inputs must be CUDA tensors; there is no CPU path")
-        s = self.spec
-        if z.dim() == 4 and not z.is_floating_point():
-            if s.regularizer != "fsq":
-                raise ValueError("token indices need an FSQ model")
-            z = self.model.indices_to_latent(z)
-        if z.dim() != 5 or tuple(z.shape[:2]) != (self.B, s.z_channels) or tuple(z.shape[3:]) != (self.H, self.W):
-            raise ValueError(f"expected a [{self.B},{s.z_channels},tz,{self.H},{self.W}] latent, got {tuple(z.shape)}")
-        z = z.detach().to(torch.float32).contiguous()
+        z = self._latents(z, self.B).contiguous()
         if self.t_chunk is not None:
             z = z if self.pending is None else torch.cat([self.pending, z], dim=2)
             return self._decode(z, recipe_decode_chunks(z.shape[2], self.first, self.t_chunk, self.use_overlap, self.tdf, False),
@@ -491,7 +508,7 @@ class DecodeStream(_Stream):
         if tz == 0:
             return self._empty(z.device)
         # v1.1: the first latent frame is a chunk of its own (build_chunk_start_end)
-        chunks = [1, tz - 1] if self.first and s.version == 1 and tz > 1 else [tz]
+        chunks = [1, tz - 1] if self.first and self.spec.version == 1 and tz > 1 else [tz]
         return self._decode(z, [(n, n, 0) for n in chunks], final=False)
 
     def flush(self) -> torch.Tensor:
@@ -505,25 +522,20 @@ class DecodeStream(_Stream):
                                                                self.tdf, True), final=True)
 
     def _decode(self, z: torch.Tensor, plan: List[Tuple[int, int, int]], final: bool) -> torch.Tensor:
-        s = self.spec
         outs = []
         t0 = 0
         for n, step, trim in plan:
-            To = self.native.decoded_frames(n) if (self.first or s.version == 1) else n * self.tdf
+            zc = z[:, :, t0:t0 + n]
             key, action = self._graph_action(n, final, "plain")
-            if action != "eager":
-                g = self.graphs.graphs[key] if action == "replay" else {
-                    "n": n, "ws_fn": lambda n=n: self._workspace(n),
-                    "z": torch.empty((self.B, s.z_channels, n, self.H, self.W), dtype=torch.float32, device=z.device),
-                    "out": torch.empty((self.B, s.out_ch, To, self.H * self.f, self.W * self.f), dtype=torch.float32, device=z.device)}
-                g["z"].copy_(z[:, :, t0:t0 + n])
-                out = self.graphs.run(key, action, self.state, self._launch_decode, g)["out"].clone()
+            if action == "eager":
+                out = self.state.decode(zc.contiguous(), self.first)
             else:
-                out = torch.empty((self.B, s.out_ch, To, self.H * self.f, self.W * self.f), dtype=torch.float32, device=z.device)
-                ws = self._workspace(n)
-                N.check(self.native.lib.vt_decode_chunk(self.state.handle, int(self.first), _ptr(z[:, :, t0:t0 + n].contiguous()),
-                                                        s.z_channels, n, _ptr(out), _ptr(ws), ws.numel(), _stream_ptr(z.device)))
-            outs.append(out[:, :, :To - trim] if trim else out)
+                g = self.graphs.graphs[key] if action == "replay" else dict(
+                    self.state.decode_buffers(n, first=False),
+                    z=torch.empty((self.B, self.spec.z_channels, n, self.H, self.W), dtype=torch.float32, device=z.device))
+                g["z"].copy_(zc)
+                out = self.graphs.run(key, action, self.state, self._launch_decode, g)["out"].clone()
+            outs.append(out[:, :, :out.shape[2] - trim] if trim else out)
             self.first = False
             t0 += step
         self.pending = z[:, :, t0:].clone() if t0 < z.shape[2] else None
@@ -533,29 +545,11 @@ class DecodeStream(_Stream):
         return x.to(self.out_dtype)
 
     def _launch_decode(self, g: Dict):
-        ws = g["ws"]
-        N.check(self.native.lib.vt_decode_chunk(self.state.handle, 0, _ptr(g["z"]), self.spec.z_channels, g["n"], _ptr(g["out"]),
-                                                _ptr(ws), ws.numel(), _stream_ptr(self.native.device)))
-
+        self.state.decode(g["z"], False, out=g)
 
 # ---------------------------------------------------------------------------------------------------------------------
 # Pools: many videos, each starting and ending on its own, through one batched chunk state
 # ---------------------------------------------------------------------------------------------------------------------
-def check_pool_recipe(version: int, tdf: int, t_chunk: Optional[int], use_overlap: bool, is_decoder: bool):
-    """The options a pool accepts (ValueError otherwise): every pool has a chunk length, t_chunk frames (encoder, a
-    multiple of tdf) or latent frames (decoder); v1.1 pools follow the stream recipe's rules."""
-    if t_chunk is None:
-        raise ValueError("a pool needs t_chunk: the batched chunks of all its slots have one length")
-    if version == 1:
-        check_recipe(version, tdf, t_chunk, use_overlap, is_decoder)
-        return
-    if use_overlap:
-        raise ValueError("use_overlap needs a v1.1 model and t_chunk (the look-ahead follows the tile_decode chunks)")
-    if int(t_chunk) < 1 or (not is_decoder and int(t_chunk) % tdf != 0):
-        raise ValueError(f"t_chunk must be a positive multiple of time_downsample_factor ({tdf}), got {t_chunk}"
-                         if not is_decoder else f"t_chunk must be a positive number of latent frames, got {t_chunk}")
-
-
 class PoolSchedule:
     """The host-side plan of a pool, without device work: which slots hold a video, how many frames (encoder) or latent
     frames (decoder) each has buffered, and where each chunk runs.  Chunks are (frames in, frames consumed, decoded frames
@@ -635,22 +629,12 @@ class PoolSchedule:
         return started, chunks
 
 
-class _Pool:
+class _Pool(_Chunked):
     def __init__(self, model, capacity: int, H: int, W: int, is_decoder: bool, t_chunk: Optional[int],
                  use_overlap: bool = False):
-        if not model.is_causal:
-            raise ValueError("non-causal models cannot stream: their time padding is symmetric, so a frame depends on later frames")
-        self.tdf = int(model.spec.time_downsample_factor)
-        check_pool_recipe(model.spec.version, self.tdf, t_chunk, use_overlap, is_decoder)
-        self.sched = PoolSchedule(capacity, model.spec.version, self.tdf, int(t_chunk), is_decoder, use_overlap)
-        self.S, self.t_chunk, self.use_overlap = self.sched.S, int(t_chunk), bool(use_overlap)
-        rt = model._rt
-        self.model = model
-        self.native = rt.sync()
-        self.spec = model.spec
-        self.precision = rt.precision()
-        self.out_dtype = rt.out_dtype()
-        self.H, self.W = int(H), int(W)
+        super().__init__(model, H, W, is_decoder, t_chunk, use_overlap, check_pool_recipe)
+        self.sched = PoolSchedule(capacity, self.spec.version, self.tdf, self.t_chunk, is_decoder, self.use_overlap)
+        self.S = self.sched.S
         self.main = ChunkState(self.native, self.precision, self.S, self.H, self.W, is_decoder, self.use_overlap)
         self.side = ChunkState(self.native, self.precision, 1, self.H, self.W, is_decoder, self.use_overlap)
         self.park: Optional[ChunkState] = None   # holds the caches of started slots that sit out a batched chunk
@@ -710,20 +694,6 @@ class _Pool:
         return x
 
 
-class _SlotLosses:
-    """One video's running losses, as tile_encode (v1.1: mean over its chunks) or the whole clip (v1.0) forms them."""
-
-    def __init__(self, dev, aux: bool, J: int):
-        self.n_chunks = 0
-        self.kl_sum = torch.zeros((), dtype=torch.float32, device=dev)
-        self.aux_sum = torch.zeros((), dtype=torch.float32, device=dev)
-        self.aux_loss = torch.zeros((), dtype=torch.float32, device=dev)
-        if aux:
-            self.tok_stats = torch.zeros((2,), dtype=torch.float64, device=dev)
-            self.tok_avg = torch.zeros((J,), dtype=torch.float64, device=dev)
-            self.tokens = 0
-
-
 class EncodePool(_Pool):
     """S slots of one encoder, one (H, W).  Each slot holds one video at a time; videos open, push frames and close
     independently, and each video's outputs equal its own tile_encode (v1.1, t_chunk = t_chunk_enc) or its whole-clip
@@ -742,24 +712,19 @@ class EncodePool(_Pool):
         self.Hz, self.Wz = self.native.latent_shape(1, H, W)[1:]
         self.reg = model.regularization
         self.aux = self.spec.regularizer == "fsq" and self.reg.aux_enabled()
-        self.losses: List[Optional[_SlotLosses]] = [None] * self.S
+        self.losses: List[Optional[_Losses]] = [None] * self.S
         self.gens: List[Optional[torch.Generator]] = [None] * self.S
 
     def open(self, generator: Optional[torch.Generator] = None) -> int:
         slot = self._open()
-        J = self.reg.codebook_size if self.aux else 0
-        self.losses[slot] = _SlotLosses(self.native.device, self.aux, J)
+        self.losses[slot] = _Losses(self.model, self.native.device, self.aux)
         self.gens[slot] = generator
         return slot
 
     def push(self, slot: int, frames: torch.Tensor):
         """frames: [1, C, t, H, W] CUDA tensor, any t (buffered until they complete a chunk)."""
         self.sched.check(slot)
-        if not frames.is_cuda:
-            raise RuntimeError("vidtok_b200: inputs must be CUDA tensors; there is no CPU path")
-        if frames.dim() != 5 or tuple(frames.shape[:2]) != (1, self.spec.in_channels) or tuple(frames.shape[3:]) != (self.H, self.W):
-            raise ValueError(f"expected [1,{self.spec.in_channels},t,{self.H},{self.W}] frames, got {tuple(frames.shape)}")
-        self._buffer(slot, frames.detach().to(torch.float32))
+        self._buffer(slot, self._frames(frames, 1))
 
     def step(self) -> Dict[int, Tuple[torch.Tensor, Dict[str, torch.Tensor]]]:
         """Runs every first chunk that is buffered (side state, then transplanted into its slot) and one batched chunk of
@@ -805,17 +770,15 @@ class EncodePool(_Pool):
                 idx = torch.cat([p[1] for p in parts], dim=1) if len(parts) > 1 else parts[0][1]
             else:
                 idx = torch.empty((1, 0, self.Hz, self.Wz), dtype=torch.int32, device=dev)
-            log = {"indices": idx, "aux_loss": L.aux_loss}
-        elif s.version == 1:
-            log = {"kl_loss": EncodeStream._mean(L.kl_sum, L.n_chunks) if L.n_chunks else torch.zeros((), device=dev)}
+            log = {"indices": idx, "aux_loss": L.aux_loss()}
         else:
-            log = {"kl_loss": L.kl_sum}
+            log = {"kl_loss": L.kl_loss()}
         return z.to(self.out_dtype), log
 
     def _run(self, state: ChunkState, rows: Dict[int, torch.Tensor], slot_of: Dict[int, int], first: bool) -> Dict[int, Tuple]:
-        """One chunk of `state` over rows {batch row: frames [1,C,n,H,W]} (other rows zeros); per row (z, indices) and
+        """One chunk of `state` over rows {batch row: frames [1,C,n,H,W]} (other rows zeros); per row (z, indices), and
         the row's video's losses updated from its own slice of the pre-bound latent."""
-        s, lib, dev = self.spec, self.native.lib, self.native.device
+        s, dev = self.spec, self.native.device
         B = self.S if state is self.main else 1
         n = next(iter(rows.values())).shape[2]
         tz = self.native.latent_shape(n, self.H, self.W)[0]
@@ -823,47 +786,19 @@ class EncodePool(_Pool):
         noise = None
         if s.regularizer == "kl" and s.kl_sample:
             noise = torch.zeros((B, s.z_channels, tz, self.Hz, self.Wz), dtype=torch.float32)
-            for r in rows:   # CPU draws, one per video chunk (distributions.py:17), as tile_encode makes them
-                noise[r] = torch.randn((1, s.z_channels, tz, self.Hz, self.Wz), generator=self.gens[slot_of[r]])[0]
+            for r in rows:   # row by row, each with its video's generator
+                noise[r] = chunk_noise(1, s.z_channels, [tz], self.Hz, self.Wz, self.gens[slot_of[r]])[0]
             noise = noise.to(dev)
-        hC = (2 if s.double_z else 1) * s.z_channels
-        z = torch.empty((B, s.z_channels, tz, self.Hz, self.Wz), dtype=torch.float32, device=dev)
-        idx = torch.empty((B, tz, self.Hz, self.Wz), dtype=torch.int32, device=dev) if s.regularizer == "fsq" else None
-        kl_batch = torch.empty((1,), dtype=torch.float32, device=dev) if s.regularizer == "kl" else None
-        h = torch.empty((B, hC, tz, self.Hz, self.Wz), dtype=torch.float32, device=dev)
-        ws = state.workspace(n)
-        N.check(lib.vt_encode_chunk_pre(state.handle, int(first), _ptr(x), s.in_channels, n, _ptr(noise), _ptr(z), _ptr(idx),
-                                        _ptr(kl_batch), _ptr(h), _ptr(ws), ws.numel(), _stream_ptr(dev)))
+        b = state.encode(x, first, noise, want_h=True)
         out = {}
         for r in rows:
-            self._add_losses(self.losses[slot_of[r]], h[r:r + 1], tz)
-            out[r] = (z[r:r + 1], idx[r:r + 1] if idx is not None else None)
+            L, h = self.losses[slot_of[r]], b["h"][r:r + 1]
+            if s.regularizer == "kl":
+                L.add(kl=_loss_terms(self.native, self.reg, h))
+            elif self.aux:
+                L.add(partials=_loss_terms(self.native, self.reg, h), tokens=tz * self.Hz * self.Wz)
+            out[r] = (b["z"][r:r + 1], b["idx"][r:r + 1] if b["idx"] is not None else None)
         return out
-
-    def _add_losses(self, L: _SlotLosses, h: torch.Tensor, tz: int):
-        """one chunk of one video: KL from its pre-bound slice (vt_op_kl), FSQ aux partials (vt_fsq_aux_partials)"""
-        s, dev = self.spec, self.native.device
-        L.n_chunks += 1
-        if s.regularizer == "kl":
-            P = tz * self.Hz * self.Wz
-            zs = torch.empty((1, s.z_channels, tz, self.Hz, self.Wz), dtype=torch.float32, device=dev)
-            kl = torch.empty((), dtype=torch.float32, device=dev)
-            N.check(self.native.lib.vt_op_kl(_ptr(h), None, s.z_channels, P, 1, 0, _ptr(zs), _ptr(kl), _stream_ptr(dev)))
-            L.kl_sum = L.kl_sum + kl   # in chunk order, as tile_encode's mean sums them
-        elif self.aux:
-            stats, avg = self.reg.aux_partials(h)
-            if s.version == 0:   # all of the video's tokens as one segment, as the whole-clip encode
-                tokens = tz * self.Hz * self.Wz
-                L.tok_stats += tokens * stats[0].double()
-                L.tok_avg += tokens * avg[0].double()
-                L.tokens += tokens
-                L.aux_loss = self.reg.aux_finalize((L.tok_stats / L.tokens).float().view(1, 2),
-                                                   (L.tok_avg / L.tokens).float().view(1, -1),
-                                                   n_steps=self.model.global_step // 2, world_size=1)
-            else:                # tile_encode: the mean over the chunks of each chunk's aux
-                aux = self.reg.aux_finalize(stats, avg, n_steps=self.model.global_step // 2, world_size=1)
-                L.aux_sum = L.aux_sum + aux
-                L.aux_loss = EncodeStream._mean(L.aux_sum, L.n_chunks)
 
 
 class DecodePool(_Pool):
@@ -884,16 +819,7 @@ class DecodePool(_Pool):
 
     def push(self, slot: int, z: torch.Tensor):
         self.sched.check(slot)
-        if not z.is_cuda:
-            raise RuntimeError("vidtok_b200: inputs must be CUDA tensors; there is no CPU path")
-        s = self.spec
-        if z.dim() == 4 and not z.is_floating_point():
-            if s.regularizer != "fsq":
-                raise ValueError("token indices need an FSQ model")
-            z = self.model.indices_to_latent(z)
-        if z.dim() != 5 or tuple(z.shape[:2]) != (1, s.z_channels) or tuple(z.shape[3:]) != (self.H, self.W):
-            raise ValueError(f"expected a [1,{s.z_channels},tz,{self.H},{self.W}] latent, got {tuple(z.shape)}")
-        self._buffer(slot, z.detach().to(torch.float32))
+        self._buffer(slot, self._latents(z, 1))
 
     def step(self) -> Dict[int, torch.Tensor]:
         """Runs every first chunk that is buffered (side state, then transplanted into its slot) and one batched chunk of
@@ -933,13 +859,8 @@ class DecodePool(_Pool):
         return x.to(self.out_dtype)
 
     def _run(self, state: ChunkState, rows: Dict[int, torch.Tensor], chunk: Tuple[int, int, int], first: bool) -> Dict[int, torch.Tensor]:
-        s, dev = self.spec, self.native.device
         B = self.S if state is self.main else 1
-        n, _, trim = chunk
-        To = self.native.decoded_frames(n) if (first or s.version == 1) else n * self.tdf
-        z = self._stack(rows, B)
-        out = torch.empty((B, s.out_ch, To, self.H * self.f, self.W * self.f), dtype=torch.float32, device=dev)
-        ws = state.workspace(n)
-        N.check(self.native.lib.vt_decode_chunk(state.handle, int(first), _ptr(z), s.z_channels, n, _ptr(out), _ptr(ws), ws.numel(),
-                                                _stream_ptr(dev)))
+        trim = chunk[2]
+        out = state.decode(self._stack(rows, B), first)
+        To = out.shape[2]
         return {r: out[r:r + 1, :, :To - trim] if trim else out[r:r + 1] for r in rows}
